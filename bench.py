@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- atom-steps/s (energy + forces) of the NequIP hot path on B200.
+"""bench.py -- atom-steps/s (energy + forces) of the NequIP hot path on H100.
 
-  python bench.py --gpus N --steps K --warmup W            (own arm: sm_100a kernels)
+  python bench.py --gpus N --steps K --warmup W            (own arm: sm_90a kernels)
   python bench.py --impl reference --gpus N --steps K ...  (reference arm: the e3nn-formulation
                                                             CPU path = oracle port, all host threads,
                                                             bounded sample of the same workload)
@@ -15,8 +15,12 @@ r_max 5 A -- on a synthetic ~10k-atom Li3PO4-like periodic box (10 648 atoms, ~5
 `e2e_device_neighbor_list`: as `e2e`, but only positions travel and the neighbour list is built on the GPU.
 `roofline`: every hot kernel class of every layer timed ALONE (CUDA events on the launching stream, step-sized
            inputs > L2); the class with the largest share of the step is the headline, the rest is under
-           `roofline.by_kernel` (HBM fraction of the measured copy peak; for the tcgen05 GEMMs also the 3xTF32
-           issue rate against half the measured bf16 cuBLAS rate, and the ncu tensor-pipe activity).
+           `roofline.by_kernel` (HBM fraction of the H100 SXM data-sheet bandwidth; for the wgmma GEMMs also the
+           3xTF32 issue rate against the data-sheet dense TF32 rate).
+`--dump-outputs DIR`: after the timed steps, what the last timed step returned is written as DIR/<name>.npy (float64):
+           total_energy and forces (plus atomic_energy from an eager single-frame step, --no-graph); in halo mode rank 0
+           writes the forces of its owned atoms only.  Inputs and model weights are seeded, so the same arguments give
+           the same inputs and two builds can be compared output for output.
 N > 1 (default): ONE frame partitioned by atoms into N bricks with halo (ghost) atoms -- the north_star
 partition: per-layer NCCL halo exchange of ghost features, energy all-reduce, ghost-force reduction to the
 owners; the whole sharded step is one CUDA-graph replay per rank.  `--scaling weak` (default) grows the frame
@@ -57,13 +61,9 @@ REF_ARM_BUDGET_S = 300.0  # --impl reference: all of its --steps + --warmup step
 R_MAX = 5.0
 
 
-def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+# NVIDIA H100 SXM data sheet (700 W board): HBM3 bandwidth and dense TF32 tensor rate.  Ceilings, not measured rates.
+H100_HBM_GBS = 3350.0
+H100_TF32_TFLOPS = 495.0
 
 
 class ClockSampler:
@@ -245,21 +245,6 @@ def cpu_baseline(workload):
                        f"E={sysd['edge_index'].shape[1]}, {cores} of {os.cpu_count()} host threads (fastest of a short sweep)")}
 
 
-def ncu_summary(kernel, field):
-    """A per-launch metric of ``kernel`` from the committed ``ncu --set full`` summaries of this round
-    (profiles/r02_ncu_full_summary.json; falls back to round 1's), or None."""
-    for name in ("r02_ncu_full_summary.json", "r01_ncu_full_summary.json"):
-        try:
-            rows = json.load(open(os.path.join(ROOT, "profiles", name)))[kernel]
-            r = max(rows, key=lambda x: x["ms"])
-            if field == "traffic":
-                return int(round((r["dram_read_GB"] + r["dram_write_GB"]) * 1e9))
-            return r.get(field)
-        except Exception:
-            continue
-    return None
-
-
 def force_sum_vector(forces):
     """[sum Fx, sum Fy, sum Fz, sum |F|, 1] (float64) of one rank's forces -- summed over the ranks this is the
     size-independent parity property of the step: the forces of a periodic frame add up to zero (Newton's third law),
@@ -388,6 +373,17 @@ def halo_exchange_profile(dims, plan, halo, dev, world, reps=10):
     return out
 
 
+def dump_outputs(path, out):
+    """What the timed step returned to its caller, as float64 .npy files (rank 0's outputs; a few MB at most).  A graph
+    replay returns total_energy and forces; an eager step also atomic_energy."""
+    import numpy as np
+
+    os.makedirs(path, exist_ok=True)
+    for name in ("total_energy", "atomic_energy", "forces"):
+        if out.get(name) is not None:
+            np.save(os.path.join(path, name + ".npy"), out[name].detach().to("cpu", torch.float64).numpy())
+
+
 def _time_cuda(fn, reps):
     for _ in range(3):
         fn()
@@ -412,13 +408,8 @@ def kernel_rooflines(model, resident, n_atoms, n_edges, reps, ms_step, dev):
     from nequip_b200.nn import dense
     from nequip_b200.nn.model import ScalarLinearLayer
 
-    peak_hbm, peak_src = load_peaks()
-    try:
-        pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        tf32_peak = float(pk["bf16_tflops_sustained"]) / 2.0  # no TF32 measurement exists: half the measured bf16 rate
-        tf32_src = "estimated: measured sustained bf16 cuBLAS rate / 2"
-    except Exception:
-        tf32_peak, tf32_src = 1590.0 / 2.0, "estimated: fallback bf16 rate / 2"
+    peak_hbm, peak_src = H100_HBM_GBS, "H100 SXM data sheet (HBM3)"
+    tf32_peak, tf32_src = H100_TF32_TFLOPS, "H100 SXM data sheet (dense TF32)"
     N, E = n_atoms, n_edges
     ei = resident["edge_index"]
     csr = ops.build_csr(ei[0].contiguous(), N)
@@ -472,17 +463,16 @@ def kernel_rooflines(model, resident, n_atoms, n_edges, reps, ms_step, dev):
                 ms = _time_cuda(lambda: ops.tp_fused_fwd(fused.fw, x, y, h, src, csr, want_w=True), reps)
                 alg = 4 * (N * sig.d_in + E * sig.s_dim + E * K + N * sig.d_out + E * W) + 16 * E + 8 * K * W
                 tfl = flops3 / (ms * 1e-3) / 1e12
-                add("tp_fused_fwd_kernel", hbm_entry("tp_fused_fwd_kernel (radial GEMM + TP + scatter, tcgen05 + FFMA2)", ms, alg, li, {
+                add("tp_fused_fwd_kernel", hbm_entry("tp_fused_fwd_kernel (radial GEMM + TP + scatter, wgmma + CUDA cores)", ms, alg, li, {
                     "tensor": {"achieved": tfl, "peak": tf32_peak, "unit": "TFLOP/s (3xTF32 issue)", "frac": tfl / tf32_peak,
                                "peak_source": tf32_src}}))
             else:
                 ms = _time_cuda(lambda: mlp.fwd.run(h, w, E), reps)
                 alg = 4 * E * (K + W) + 8 * K * W
                 tfl = flops3 / (ms * 1e-3) / 1e12
-                add("k_gemm3x", hbm_entry("k_gemm3x (radial MLP last layer forward, tcgen05 3xTF32)", ms, alg, li, {
+                add("k_gemm3x", hbm_entry("k_gemm3x (radial MLP last layer forward, wgmma 3xTF32)", ms, alg, li, {
                     "tensor": {"achieved": tfl, "peak": tf32_peak, "unit": "TFLOP/s (3xTF32 issue)", "frac": tfl / tf32_peak,
-                               "peak_source": tf32_src,
-                               "pipe_tensor_cycles_active_pct": ncu_summary("k_gemm3x", "pipe_tensor_pct")}}))
+                               "peak_source": tf32_src}}))
                 ms = _time_cuda(lambda: ops.tp_scatter(plan, x, y, w, ei[0], src, csr=csr), reps)
                 name = "tp_fwd2_kernel" if TPGen(sig, plan.opts).ring_fwd() else "tp_fwd_kernel<float>"
                 add(name, hbm_entry(name + " (fused TP + scatter forward)", ms, tp_algorithmic_bytes(sig, N, E), li))
@@ -497,22 +487,20 @@ def kernel_rooflines(model, resident, n_atoms, n_edges, reps, ms_step, dev):
             tfl = flops3 / (ms * 1e-3) / 1e12
             add("k_gemm3x", hbm_entry("k_gemm3x (radial MLP last layer backward, K = W)", ms, alg, li, {
                 "tensor": {"achieved": tfl, "peak": tf32_peak, "unit": "TFLOP/s (3xTF32 issue)", "frac": tfl / tf32_peak,
-                           "peak_source": tf32_src,
-                           "pipe_tensor_cycles_active_pct": ncu_summary("k_gemm3x", "pipe_tensor_pct")}}))
+                           "peak_source": tf32_src}}))
             del x, y, emb, go, h, w, gh
     for k, c in classes.items():
         c["share_of_step"] = c["ms_per_step"] / ms_step
     top_name = max(classes, key=lambda k: classes[k]["ms_per_step"])
     top = dict(classes[top_name]["largest"])
-    top["traffic"] = ncu_summary(top_name.split("<")[0], "traffic")
     top["peak_source"] = peak_src
     top["share_of_step"] = classes[top_name]["share_of_step"]
     top["selection"] = ("kernel class with the largest summed isolated time over the layers of one step; numbers are for "
                         "its largest launch")
-    top["inputs"] = "per-edge operands of the step's size (>> 126 MB L2)"
+    top["inputs"] = "per-edge operands of the step's size (>> 50 MB L2)"
     top["by_kernel"] = {k: {"ms_per_step_isolated": c["ms_per_step"], "share_of_step": c["share_of_step"],
                             "launches_per_step": c["launches_per_step"],
-                            "traffic": ncu_summary(k.split("<")[0], "traffic"), **c["largest"]}
+                            **c["largest"]}
                         for k, c in sorted(classes.items(), key=lambda kv: -kv[1]["ms_per_step"])}
     return top
 
@@ -550,8 +538,11 @@ def main():
                          "along x); 'strong' = the workload's own frame split N ways")
     ap.add_argument("--no-graph", action="store_true", help="eager step (no CUDA-graph replay)")
     ap.add_argument("--profile-step", action="store_true",
-                    help="run one warm-up step, then ONE step between cudaProfilerStart/Stop (for ncu "
-                         "--profile-from-start off); prints no bench line")
+                    help="run one warm-up step, then ONE step between cudaProfilerStart/Stop (for an external "
+                         "profiler started with capture off); prints no bench line")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step (total_energy, forces; atomic_energy when eager) to "
+                         "DIR/<name>.npy (float64); in halo mode rank 0's owned atoms only")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
@@ -697,9 +688,10 @@ def main():
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         n0 = _capi.launch_count()
+        out = None
         e0.record()
         for _ in range(steps):
-            fn()
+            out = fn()
         e1.record()
         torch.cuda.synchronize()
         if world > 1:
@@ -712,7 +704,7 @@ def main():
             t = torch.tensor([ms], dtype=torch.float64, device=dev)
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
             ms = float(t.item())
-        return ms, launches
+        return ms, launches, out
 
     if args.profile_step:
         step_resident()
@@ -726,11 +718,14 @@ def main():
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    ms_res, launches = timed(step_resident, args.steps, args.warmup)
-    ms_e2e, _ = timed(step_e2e, args.steps, 1)
+    ms_res, launches, last = timed(step_resident, args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
+    del last  # graph replays write into the same static buffers
+    ms_e2e, _, _ = timed(step_e2e, args.steps, 1)
     ms_e2e_nl = None
     if world == 1 and "cell" in sysd:
-        ms_e2e_nl, _ = timed(step_e2e_device_nl, args.steps, 1)
+        ms_e2e_nl, _, _ = timed(step_e2e_device_nl, args.steps, 1)
     clocks = sampler.stop() if rank == 0 else None
     if graphed is not None:
         graphed.check_sorted()  # the in-graph "edges grouped by destination" flag of the last replay

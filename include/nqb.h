@@ -1,5 +1,5 @@
 /*
- * nqb.h -- C ABI of the B200-native NequIP hot path (libnqb.so).
+ * nqb.h -- C ABI of the H100-native NequIP hot path (libnqb.so).
  *
  * Plain C: raw device pointers, sizes, a CUDA stream.  No torch / C++ types cross
  * this boundary.  Every tensor is caller-allocated (torch caching allocator on the
@@ -107,6 +107,13 @@ int nqb_tp_scatter_gy_slices(const nqb_plan* plan, int dtype);
 int nqb_segment_sum(int dtype, const void* rows /* [R, D] */, int D, const int64_t* perm, const int64_t* seg_ptr /* [N+1] */,
                     int64_t N, void* out /* [N, D] */, nqb_stream_t st);
 
+/* Real spherical harmonics, "component" normalisation, input normalised (lmax <= 3).
+ *   vec [E,3] f64 -> y [E,(lmax+1)^2] of out_dtype (computed in f64, then cast). */
+int nqb_sh_fwd(int lmax, const double* vec, int64_t E, int out_dtype, void* y, nqb_stream_t st);
+/*   grad_vec [E,3] f64 = J^T grad_y (includes the normalisation Jacobian); overwritten */
+int nqb_sh_bwd(int lmax, const double* vec, int64_t E, int out_dtype, const void* grad_y,
+               double* grad_vec, nqb_stream_t st);
+
 /* Fused "last radial-MLP layer -> tensor product -> scatter" forward (SURVEY.md section 8f-1):
  *   out[n] = sum_{e: dst[e] = n} TP_uvu(x[src[e]], y[e], w[e]),   w[e] = h[e, :K] @ (W2 * alpha2)
  * i.e. nequip/nn/mlp.py:262-268 (the last ScalarLinearLayer built at nequip/nn/interaction_block.py:119-127)
@@ -114,8 +121,9 @@ int nqb_segment_sum(int dtype, const void* rows /* [R, D] */, int D, const int64
  * tensor is never written (w_out == NULL) -- or is written once on the side for an unfused backward.
  * float32, ir_mul node layout, edges grouped by destination (row_ptr; no permutation), K <= 128, K % 8 == 0.
  * nqb_tp_fused_slices(plan): number of 128-row weight slices of the signature, 0 = no fused kernel built.
- * w2_prepared: nqb_gemm_t_prepare() of the [K, 128 * slices] weight matrix whose COLUMNS are in slice order
- *   (nequip_b200/codegen.py TPGenerator.fused_layout()["cols"], -1 = zero column), scaled by alpha2.
+ * w2_prepared: per slice, the tf32 hi and lo parts of the [128 x 128] block W2^T (rows = the slice's columns of the
+ *   weight matrix in nequip_b200/codegen.py TPGenerator.fused_layout()["cols"] order, -1 = zero row; K zero padded
+ *   to 128), scaled by alpha2, each block in the canonical K-major core-matrix order (ops.FusedTPWeights).
  * slice_cta0 [slices + 1] (device, int32): CTAs [cta0[s], cta0[s+1]) process slice s; nctas = cta0[slices]
  *   (one CTA per SM; the host splits the grid in proportion to the slices' costs). */
 int nqb_tp_fused_slices(const nqb_plan* plan);
@@ -171,19 +179,18 @@ int nqb_nl_fill(int64_t N, int64_t E, const double* cell_host, const double* inv
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).
  * Together with nqb_gemm_grouped for the second layer this is ScalarMLPFunction (nequip/nn/mlp.py:80-195). */
 /* h_lo (nullable): the part of h the tensor core does not see, h_lo = rna_tf32(h - trunc_tf32(h)).  It can be
- * handed to nqb_gemm_grouped as a_lo_base, but that form doubles the A reads and limits the producer ring to one
- * piece in flight (measured 1.7x slower, profiles/r01_gemm_roles.txt): the product path passes NULL for both. */
+ * handed to nqb_gemm_grouped as a_lo_base, but that form doubles the A reads: the product path passes NULL for both. */
 int nqb_mlp_hidden_fwd(const float* emb, const float* W1s, int64_t E, int num_bessel, int hidden, float* h,
                        float* h_lo, nqb_stream_t st);
 int nqb_mlp_hidden_bwd(const float* emb, const float* W1s, const float* grad_h, int64_t E, int num_bessel,
                        int hidden, float* grad_emb, nqb_stream_t st);
-/* Kernel generation of the two calls above: 2 = batched kernels (32 edges per warp, prefetched basis values, packed
- * FFMA2, one 128-byte grad_emb row per four edges), 1 = the round-1 kernels (one edge per warp iteration).  Returns the
+/* Kernel generation of the two calls above: 2 = batched kernels (32 edges per warp, prefetched basis values, float2
+ * arithmetic, one 128-byte grad_emb row per four edges), 1 = the round-1 kernels (one edge per warp iteration).  Returns the
  * previous value; 0 only queries.  Default: the library's build-time choice, overridden by the environment variable
  * NQB_HIDDEN_VARIANT=1|2.  Not thread safe -- call between launches (A/B timing, parity tests). */
 int nqb_mlp_hidden_set_variant(int variant);
 
-/* Grouped fp32-accurate GEMM on the tensor cores (tcgen05 kind::tf32, 3xTF32, segmented fp32
+/* Grouped fp32-accurate GEMM on the tensor cores (wgmma tf32, 3xTF32, segmented fp32
  * accumulation):  C_p[M, N_p] (+)= rowscale_p[m] * A_p[M, K_p] @ B_p[K_p, N_p]  for a list of problems
  * sharing M.  Replaces the dense algebra around the convolution: ScalarMLPFunction's torch.mm
  * (nequip/nn/mlp.py:262-268), e3nn o3.Linear linear_1/linear_2 and the self-connection
@@ -207,15 +214,6 @@ int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_total, const i
                      int sched_ctas, const float* a_base,
                      const float* a_lo_base, const float* prepared_base, float* c_base,
                      const float* rowscale_base, int64_t rs_ld, int64_t M, nqb_stream_t st);
-
-/* EXPERIMENTAL (not used by the model yet): the same product for ONE problem with K <= 128, computed transposed
- * with the weights resident in tensor memory as the MMA's A operand (nequip_b200/csrc/nqb_gemm_t.cu).
- * prepared: nqb_gemm_t_prepared_floats(K, N) floats written by nqb_gemm_t_prepare. */
-int64_t nqb_gemm_t_prepared_floats(int K, int N);
-int nqb_gemm_t_prepare(const float* B, int64_t ldb, int K, int N, int transposed, float scale, float* prepared,
-                       nqb_stream_t st);
-int nqb_gemm_t_run(const float* prepared, int K, int N, const float* A, int64_t lda, float* C, int64_t ldc, int64_t M,
-                   nqb_stream_t st);
 
 /* Gate nonlinearity (e3nn nn.Gate with normalize2mom'd SiLU for even / tanh for odd scalars and gates,
  * nequip/nn/convnetlayer.py:42-56,104-112), one kernel per direction.  Column tables (device, int32) are

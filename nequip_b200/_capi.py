@@ -43,10 +43,10 @@ SIGNATURES = {
     "nqb_tp_scatter_fwd": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
     "nqb_tp_scatter_bwd": (
         _i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i32, _vp]),
-    "nqb_tp_scatter_gy_slices": (_i32, [_vp, _i32]),
-    "nqb_segment_sum": (_i32, [_i32, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),
     "nqb_tp_fused_slices": (_i32, [_vp]),
     "nqb_tp_fused_fwd": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i32, _vp]),
+    "nqb_tp_scatter_gy_slices": (_i32, [_vp, _i32]),
+    "nqb_segment_sum": (_i32, [_i32, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),
     "nqb_nl_bin": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp]),
     "nqb_nl_count": (_i32, [_i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nqb_nl_fill": (_i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
@@ -61,9 +61,6 @@ SIGNATURES = {
     "nqb_mlp_hidden_set_variant": (_i32, [_i32]),
     "nqb_gemm_prepared_floats": (_i64, [_i32, _i32]),
     "nqb_gemm_prepare": (_i32, [_vp, _i64, _i32, _i32, _i32, C.c_float, _vp, _vp]),
-    "nqb_gemm_t_prepared_floats": (_i64, [_i32, _i32]),
-    "nqb_gemm_t_prepare": (_i32, [_vp, _i64, _i32, _i32, _i32, C.c_float, _vp, _vp]),
-    "nqb_gemm_t_run": (_i32, [_vp, _i32, _i32, _vp, _i64, _vp, _i64, _i64, _vp]),
     "nqb_gate_fwd": (_i32, [_i32, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "nqb_gate_bwd": (_i32, [_i32, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
     "nqb_gemm_grouped": (_i32, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp]),

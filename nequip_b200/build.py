@@ -1,8 +1,8 @@
-"""In-tree builds of libnqb.so and of the per-signature kernel libraries (sm_100a only).
+"""In-tree builds of libnqb.so and of the per-signature kernel libraries (sm_90a only).
 
-``nvcc -gencode arch=compute_100a,code=sm_100a`` cross-compiles without a GPU, so
-``__graft_entry__.build()`` runs this on the CPU box and the resulting ``.so`` files
-travel to the B200 box with the repo snapshot.  At run time a signature that has no
+``nvcc -gencode arch=compute_90a,code=sm_90a`` cross-compiles without a GPU, so
+``__graft_entry__.build()`` can run on a machine without one; the resulting ``.so`` files
+are loaded from the tree on the H100.  At run time a signature that has no
 prebuilt library is generated and compiled on the spot (the same thing the
 reference's OpenEquivariance backend does with its JIT, nequip/nn/_tp_scatter_oeq.py:29-47);
 if ``nvcc`` is missing that is a hard error -- there is no CPU fallback.
@@ -25,7 +25,7 @@ LIBDIR = os.path.join(_HERE, "lib")
 GENDIR = os.path.join(_HERE, "_gen")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON_FLAGS = ["-O3", "-lineinfo", "-std=c++17", "-shared", "-Xcompiler", "-fPIC"]
 
 _lock = threading.Lock()
@@ -35,7 +35,7 @@ def nvcc_path() -> str:
     p = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(p):
         raise RuntimeError(
-            "nequip_b200: nvcc not found -- the B200 kernels cannot be built and there is no CPU fallback"
+            "nequip_b200: nvcc not found -- the H100 kernels cannot be built and there is no CPU fallback"
         )
     return p
 
@@ -61,21 +61,24 @@ def runtime_lib_path() -> str:
 def ensure_runtime(force: bool = False) -> str:
     """Build (if stale) and return the path of libnqb.so."""
     out = runtime_lib_path()
-    cus = [os.path.join(CSRC, n) for n in ("nqb_runtime.cu", "nqb_mlp.cu", "nqb_gemm.cu", "nqb_gemm_t.cu", "nqb_nl.cu")]
+    cus = [os.path.join(CSRC, n) for n in ("nqb_runtime.cu", "nqb_mlp.cu", "nqb_gemm.cu", "nqb_nl.cu")]
     srcs = cus + [os.path.join(INCLUDE, "nqb.h"), os.path.join(CSRC, "nqb_tc.cuh")]
     with _lock:
         if force or _newer(srcs, out):
             os.makedirs(LIBDIR, exist_ok=True)
             tmp = out + f".tmp{os.getpid()}"
-            extra = os.environ.get("NQB_EXTRA_NVCC_FLAGS", "").split()  # e.g. -DNQB_GEMM_PROF (tools/bench_gemm.py --prof)
-            _run([nvcc_path(), *ARCH_FLAGS, *COMMON_FLAGS, *extra, "-I", INCLUDE, "-Xptxas", "-v", "-o", tmp, *cus, "-ldl"])
+            _run([nvcc_path(), *ARCH_FLAGS, *COMMON_FLAGS, "-I", INCLUDE, "-Xptxas", "-v", "-o", tmp, *cus, "-ldl"])
             os.replace(tmp, out)
     return out
 
 
 def _device_header_hash() -> str:
-    with open(os.path.join(CSRC, "nqb_tp_device.cuh"), "rb") as f:
-        return hashlib.sha1(f.read()).hexdigest()[:8]
+    """Hash of the headers every generated kernel library includes (part of its file name)."""
+    h = hashlib.sha1()
+    for name in ("nqb_tc.cuh", "nqb_tp_device.cuh", "nqb_tp_fused.cuh"):
+        with open(os.path.join(CSRC, name), "rb") as f:
+            h.update(f.read())
+    return h.hexdigest()[:8]
 
 
 def spec_lib_path(sig: TPSignature, opts: Optional[GenOptions] = None) -> str:

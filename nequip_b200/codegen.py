@@ -1,4 +1,4 @@
-"""CUDA source generator for the fused tensor-product + scatter kernels (sm_100a).
+"""CUDA source generator for the fused tensor-product + scatter kernels (sm_90a).
 
 One translation unit per ``TensorProductScatter`` signature (the three irreps and
 the instruction list that ``InteractionBlock.__init__`` builds,
@@ -8,8 +8,7 @@ the instruction list that ``InteractionBlock.__init__`` builds,
 
     out[dst, u, k] += coef_p * w[e, p, u] * sum_ij C_p[i, j, k] x[src, u, i] Y[e, j]
 
-Kernel design (see DESIGN.md for the roofline accounting and the measurements
-that led here):
+Kernel design (see DESIGN.md for the roofline accounting):
 
 * edges are visited in destination-CSR order (``row_ptr``/``perm``); a *work item*
   is ``(destination node, path group, channel block)`` and is owned by ONE warp,
@@ -17,19 +16,14 @@ that led here):
   and writes each output element exactly once -- no atomics, no ``[E, D_mid]``
   intermediate, deterministic;
 * lane = channel pair: fp32 kernels carry two adjacent channels per lane as a
-  ``float2`` so that every multiply-accumulate is a packed ``FFMA2``/``FMUL2`` (the
-  Clebsch-Gordan constants ride along as 32-bit immediates broadcast to both
-  halves).  ``FFMA2`` does not raise the FMA-pipe peak (measured 128 FMA/clk/SM
-  either way) but halves the issue slots, which leaves room to co-issue the
-  loads/address math of the dominant ``w[e, p, :]`` stream;
+  ``float2`` (two independent FMAs per operation; the Clebsch-Gordan constants
+  ride along as 32-bit immediates broadcast to both halves);
 * path groups partition the *input chunks*, so every ``x[src]`` element and every
   weight is loaded exactly once per edge, with coalesced 8-byte loads;
 * everything per-edge is register math: for each (input chunk, harmonic degree)
   block the products ``t_ij = x_i Y_j`` are formed once and fanned out into all
   output degrees ``l3`` through the sparse CG constants, then scaled by the path
-  weight into the accumulators.  (A shared-memory ``M = C.Y`` formulation was
-  measured first: broadcast ``LDS.128`` issues at 0.5/clk/SM on B200, which caps it
-  at ~60% of the FMA peak -- tools/microbench/pipes.cu.)
+  weight into the accumulators.
 * when a node has fewer channel pairs than lanes (mul < 64) the warp works on
   ``EPW = 32 / lanes_per_edge`` edges of the node at once and folds the partial
   accumulators with shuffles at the end;
@@ -47,7 +41,7 @@ from typing import Dict, List, Tuple
 from . import cg
 from .irreps import Irreps
 
-CODEGEN_VERSION = 21
+CODEGEN_VERSION = 23
 
 
 # ---------------------------------------------------------------------------
@@ -176,7 +170,6 @@ class GenOptions:
     bwd_ring: bool = True  # backward v2 (same weight ring)
     split_groups: bool = False  # register (v1) kernels: one launch per path group instead of one launch for all --
     #                              every SM then executes ONE group's (large, fully unrolled) body at a time
-    fused_prof: bool = False  # per-role stall counters in the fused radial-MLP + TP kernel (tools/bench_fused.py --prof)
     layout: str = "mul_ir"  # node-feature layout of x / out: "mul_ir" (the reference's, e3nn) or
     #                         "ir_mul" (channel-contiguous: every chunk is [2l+1, mul]; all node-feature
     #                         traffic becomes unit-stride 8-byte accesses; used between our own kernels)
@@ -184,7 +177,7 @@ class GenOptions:
     def tag(self) -> str:
         return (f"w{self.nwarp}_a{self.acc_cap}_b{self.acc_cap_bwd}_p{int(self.prefetch)}{int(self.idx_ahead)}"
                 f"_m{self.min_blocks_fwd}{self.min_blocks_bwd}_r{int(self.red_v2)}_{self.layout}_g{int(self.fwd_ring)}{self.ring_stages}{int(self.bwd_ring)}"
-                + ("_fp" if self.fused_prof else "") + ("_sg" if self.split_groups else ""))
+                + ("_sg" if self.split_groups else ""))
 
 
 # ---------------------------------------------------------------------------
@@ -825,9 +818,8 @@ class TPGenerator:
         """Slices of the path-parallel fused kernel, or None when the signature is not eligible.
 
         A slice is 128 consecutive (path, channel) rows = 128 // mul whole paths; paths that read the same
-        input chunk are kept together (one staged x row per edge and slice).  Returns a dict with
-        ``slices`` (lists of Path), per-slice ``segs`` [(x offset, floats)], ``cols`` (weight column of every
-        row, -1 = padding), ``cost`` per slice, ``xrow`` (max staged floats per edge) and ``nxs`` (ring stages)."""
+        input chunk are kept together.  Returns a dict with
+        ``slices`` (lists of Path), ``cols`` (weight column of every row, -1 = padding) and ``cost`` per slice."""
         sig = self.sig
         if self.opts.layout != "ir_mul":
             return None
@@ -855,38 +847,22 @@ class TPGenerator:
         while rest:
             slices.append(rest[:pps])
             rest = rest[pps:]
-        segs, xrow = [], 0
-        for grp in slices:
-            chunks = sorted({p.i1 for p in grp})
-            sg = [(sig.irreps_in1.offsets()[i1], sig.irreps_in1[i1][0] * sig.irreps_in1[i1][1].dim, i1) for i1 in chunks]
-            if len(sg) > 4:
-                return None
-            segs.append(sg)
-            xrow = max(xrow, sum(n for (_o, n, _i) in sg))
-        if xrow % 4 or sig.d_in % 4:
-            return None
-        fixed = 2 * 2 * 64 * 128 * 4 + 2 * 4 * 7 * 32 * 4 + 1024  # h tiles (hi, lo) x 2 stages, set hand-over, barriers
-        stage = 8 * (xrow + sig.s_dim) * 4
-        nxs = min(16, (227 * 1024 - 1024 - fixed) // stage)
-        if nxs < 6:
-            return None
         cols = []
         for grp in slices:
             for p in grp:
                 cols += [p.woff + u for u in range(mul)]
             cols += [-1] * (128 - mul * len(grp))
-        # per-tile time of a slice = a path-independent part (h tile, weights MMA, staging: ~5.3 k cycles measured)
-        # + the consumer arithmetic (~13 cycles per cost unit): profiles/r02_fused_v2b.txt
+        # per-tile time of a slice = a path-independent part (h tile, MMAs) + the consumer arithmetic
         cost = [400 + sum(self.path_cost(p) for p in grp) * (mul // 32) for grp in slices]
-        return dict(mul=mul, pps=pps, slices=slices, segs=segs, xrow=xrow, nxs=int(nxs), cols=cols, cost=cost)
+        return dict(mul=mul, pps=pps, slices=slices, cols=cols, cost=cost)
 
-    def _emit_fused_path(self, em: _Emitter, p: Path, xs_off: int, mul: int):
+    def _emit_fused_path(self, em: _Emitter, p: Path, mul: int):
         sig = self.sig
         n1, n2, n3 = 2 * p.l1 + 1, 2 * p.l2 + 1, 2 * p.l3 + 1
         boff, mtot, ubase = self.out_ir_mul(p.io)
         em.block(f"struct FtPath{p.idx}")
         em("static constexpr bool ACTIVE = true;")
-        em(f"static constexpr int N1 = {n1}, N2 = {n2}, N3 = {n3}, XS_OFF = {xs_off}, Y_OFF = {p.yoff}, W_OFF = {p.woff}, MUL = {mul};")
+        em(f"static constexpr int N1 = {n1}, N2 = {n2}, N3 = {n3}, XG_OFF = {sig.irreps_in1.offsets()[p.i1]}, Y_OFF = {p.yoff}, W_OFF = {p.woff}, MUL = {mul};")
         em.block("static __device__ __forceinline__ void fma(const float2* x, const float2* y, float2 w, float2* a)")
         if p.l2 == 0:
             kappa = p.coef * cg.real_w3j(p.l1, 0, p.l3)[0][0][0]
@@ -913,9 +889,9 @@ class TPGenerator:
                 if k in started:
                     em(f"a[{k}] = vfma(w, v{k}, a[{k}]);")
         em.end()
-        em.block("static __device__ __forceinline__ void store(float* __restrict__ o, int u, const float2* a)")
+        em.block("static __device__ __forceinline__ void store(float* __restrict__ o, int u, const float* v)")
         for k in range(n3):
-            em(f"o[{boff + ubase + k * mtot} + u] = a[{k}].x + a[{k}].y;")
+            em(f"o[{boff + ubase + k * mtot} + u] = v[{k}];")
         em.end()
         em.block("static __device__ __forceinline__ void store_zero(float* __restrict__ o, int u)")
         for k in range(n3):
@@ -928,42 +904,23 @@ class TPGenerator:
         if lay is None:
             return False
         sig = self.sig
-        mul, slices, segs = lay["mul"], lay["slices"], lay["segs"]
-        ns = len(slices)
-        for si, grp in enumerate(slices):
-            soff = {}
-            o = 0
-            for (_goff, n, i1) in segs[si]:
-                soff[i1] = o
-                o += n
+        mul, slices = lay["mul"], lay["slices"]
+        for grp in slices:
             for p in grp:
-                self._emit_fused_path(em, p, soff[p.i1], mul)
-        flat_len, flat_goff, cnt = [], [], []
-        for si in range(ns):
-            sg = segs[si] + [(0, 0, -1)] * (4 - len(segs[si]))
-            cnt.append(len(segs[si]))
-            flat_goff += [g for (g, _n, _i) in sg]
-            flat_len += [n for (_g, n, _i) in sg]
-        em(f"__constant__ int FT_SEG_CNT[{ns}] = {{{', '.join(map(str, cnt))}}};")
-        em(f"__constant__ int FT_SEG_GOFF[{ns * 4}] = {{{', '.join(map(str, flat_goff))}}};")
-        em(f"__constant__ int FT_SEG_LEN[{ns * 4}] = {{{', '.join(map(str, flat_len))}}};")
+                self._emit_fused_path(em, p, mul)
         em.block("struct FtSpec")
-        em(f"static constexpr int MUL = {mul}, S = {sig.s_dim}, D_IN = {sig.d_in}, D_OUT = {sig.d_out}, W = {sig.weight_numel}, "
-           f"NSLICE = {ns}, XROW = {lay['xrow']}, NXS = {lay['nxs']};")
-        em("static __device__ __forceinline__ int seg_count(int s) { return FT_SEG_CNT[s]; }")
-        em("static __device__ __forceinline__ int seg_goff(int s, int k) { return FT_SEG_GOFF[s * 4 + k]; }")
-        em("static __device__ __forceinline__ int seg_len(int s, int k) { return FT_SEG_LEN[s * 4 + k]; }")
-        em.block("static __device__ __forceinline__ void consume(int slice, int set, int quad, int lane, const FusedFwdArgs& a, "
-                 "FtSmem& S, const float* xring, uint32_t tmem)")
-        em.block("switch (slice * 4 + quad)")
-        wpp = mul // 32  # warps per path
+        em(f"static constexpr int S = {sig.s_dim}, D_IN = {sig.d_in}, D_OUT = {sig.d_out}, W = {sig.weight_numel}, "
+           f"NSLICE = {len(slices)};")
+        em("template <class Op, class... A>")
+        em.block("static __device__ __forceinline__ void dispatch(int slice, int block, A&... args)")
+        em.block("switch (slice * 8 + block)")
+        bpp = mul // 16  # 16-row blocks per path
         for si, grp in enumerate(slices):
-            for q in range(4):
-                slot = q // wpp
-                if slot < len(grp):
-                    p = grp[slot]
-                    em(f"case {si * 4 + q}: ft_consumer<FtPath{p.idx}, FtSpec>(a, S, xring, tmem, set, quad, lane, {(q % wpp) * 32} + lane); break;")
-        em("default: ft_consumer<FtNullPath, FtSpec>(a, S, xring, tmem, set, quad, lane, lane); break;")
+            for b in range(8):
+                if b // bpp < len(grp):
+                    p = grp[b // bpp]
+                    em(f"case {si * 8 + b}: Op::template run<FtPath{p.idx}>({(b % bpp) * 16}, args...); break;")
+        em("default: Op::template run<FtNullPath>(0, args...); break;")
         em.end()
         em.end()
         em.end("};")
@@ -989,8 +946,6 @@ class TPGenerator:
         em(f"// options: {self.opts.tag()}  fwd_groups={len(self.fwd_groups)} bwd_groups={len(self.bwd_groups)}")
         em(f"// forward multiply-accumulates per (edge, channel): {sig.fma_count()}")
         em("#include <cuda_runtime.h>")
-        if self.opts.fused_prof:
-            em("#define FT_PROF 1")
         em('#include "nqb_tc.cuh"')
         em("namespace {")
         em(f"constexpr int NWARP = {self.opts.nwarp};")
@@ -1019,7 +974,7 @@ class TPGenerator:
         ring_bytes = self.opts.ring_stages * self.geometry(2)[1] * sig.weight_numel * 4 + 2 * self.opts.ring_stages * 8 + 256 * 16
         # ... and only when one edge fills the warp (mul >= 64 -> EPW == 1): with two or more edges per warp iteration the
         # ring is EPW x larger per CTA (70-140 KB for the l_max = 3 layers -> 1-3 CTAs per SM) and the register kernels
-        # are up to 3.4x faster (a-Si layer 3: 5.8 / 14.0 ms against 17.2 / 49.3 ms, profiles/r02_tune_tp_lmax3_ring_vs_register.jsonl)
+        # keep more warps resident
         ring_fits = ring_bytes <= 200 * 1024 and self.geometry(2)[1] == 1
         self.use_ring = bool(self.opts.fwd_ring and sig.weight_numel % 4 == 0 and len(self.fwd_groups) >= 2 and ring_fits)
         if self.use_ring:
@@ -1263,12 +1218,10 @@ class TPGenerator:
         # fused radial-MLP last layer + TP + scatter forward (SURVEY section 8f-1); -1 = not built for this signature
         em.block('extern "C" int nqb_spec_fused_info(int* nslice, int* nxs, int* xrow)')
         if self.has_fused:
-            em("*nslice = FtSpec::NSLICE; *nxs = FtSpec::NXS; *xrow = FtSpec::XROW; return 0;")
+            em("*nslice = FtSpec::NSLICE; *nxs = 0; *xrow = 0; return 0;")
         else:
             em("*nslice = 0; *nxs = 0; *xrow = 0; return -1;")
         em.end()
-        if self.opts.fused_prof and self.has_fused:
-            em('extern "C" int nqb_spec_fused_prof(unsigned long long* out) { return (int)cudaMemcpyFromSymbol(out, ft_prof, sizeof(unsigned long long) * 160 * 32); }')
         em.block('extern "C" int nqb_spec_fused_fwd(const float* x, const float* y, const float* h, int64_t ldh, int K, '
                  "const float* wprep, const int64_t* row_ptr, const int64_t* src, int64_t N, int64_t E, float* out, "
                  "float* w_out, const int32_t* slice_cta0, int nctas, cudaStream_t st)")

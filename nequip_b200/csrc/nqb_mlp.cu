@@ -1,4 +1,4 @@
-// Radial-MLP hidden layer (K = 8) on CUDA cores, sm_100a.
+// Radial-MLP hidden layer (K = 8) on CUDA cores, sm_90a.
 //
 // Reference op (paths under /root/reference):
 //   edge_weight = ScalarMLPFunction(edge_embedding)            nequip/nn/mlp.py:80-195, 262-268
@@ -26,7 +26,20 @@ constexpr int NB = 8;        // Bessel functions
 // kernel; a warp walks over edges (grid-stride), reads the 8 basis values of the edge (one broadcast
 // 32-byte load) and writes the edge's 128 activations as one 512-byte row.  (The first version re-staged
 // the 4 KB weight matrix per 8 edges -- as many bytes as it wrote.)
-__device__ __forceinline__ float sigmoid_fast(float p) { return __fdividef(1.0f, 1.0f + expf(-p)); }
+// both kernel generations use this sigmoid, so that their activations agree bit for bit (h is computed by either,
+// depending on whether the tf32 low part is requested)
+__device__ __forceinline__ float ex2_approx(float x) {
+  float r;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+  return r;
+}
+__device__ __forceinline__ float rcp_approx(float x) {
+  float r;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+  return r;
+}
+// 1 / (1 + exp(-p));  p -> -inf gives rcp(inf) = 0, p -> +inf gives rcp(1) = 1
+__device__ __forceinline__ float sigmoid_v2(float p) { return rcp_approx(1.0f + ex2_approx(p * -1.4426950408889634f)); }
 
 __global__ void __launch_bounds__(256) k_hidden_fwd(const float* __restrict__ emb, const float* __restrict__ W1s,
                                                     int64_t E, float* __restrict__ h, float* __restrict__ h_lo) {
@@ -48,7 +61,7 @@ __global__ void __launch_bounds__(256) k_hidden_fwd(const float* __restrict__ em
       float p = 0.f;
 #pragma unroll
       for (int k = 0; k < NB; ++k) p = fmaf(x[k], w[k][q], p);
-      o[q] = p * sigmoid_fast(p);
+      o[q] = p * sigmoid_v2(p);
     }
     __stcs(reinterpret_cast<float4*>(h + e * H + m0), make_float4(o[0], o[1], o[2], o[3]));
     if (h_lo) __stcs(reinterpret_cast<float4*>(h_lo + e * H + m0), make_float4(tf32_lo(o[0]), tf32_lo(o[1]), tf32_lo(o[2]), tf32_lo(o[3])));
@@ -79,7 +92,7 @@ __global__ void __launch_bounds__(256) k_hidden_bwd(const float* __restrict__ em
     float p = 0.f;
 #pragma unroll
     for (int k = 0; k < NB; ++k) p = fmaf(x[k], w[k][q], p);
-    const float sg = sigmoid_fast(p);
+    const float sg = sigmoid_v2(p);
     const float gp = g[q] * (sg * (1.0f + p * (1.0f - sg)));
 #pragma unroll
     for (int k = 0; k < NB; ++k) acc[k] = fmaf(gp, w[k][q], acc[k]);
@@ -112,34 +125,19 @@ __global__ void __launch_bounds__(256) k_hidden_bwd(const float* __restrict__ em
 
 
 // ---------------------------------------------------------------------------------------------
-// v2 of the two kernels (round 2).  The ncu launch list of one step (profiles/r02_launches_li3po4_step.csv)
-// has k_hidden_fwd at 109 us and k_hidden_bwd at 183 us per layer -- 2.4x / 3.5x their HBM floors
-// (0.32 GB each way).  v1 runs 4 CTAs per SM (55-63 registers) with ONE edge per warp iteration and the
+// v2 of the two kernels.  v1 runs 4 CTAs per SM (55-63 registers) with ONE edge per warp iteration and the
 // edge's basis values fetched by a dependent broadcast load at the top of every iteration: 32 edges in
 // flight per SM, each paying a full DRAM latency before its arithmetic starts.  v2:
 //   * a warp owns a BATCH of 32 consecutive edges; lane j fetches edge j's 8 basis values with two
 //     coalesced 16-byte loads (1 KB per warp) and the batch after that is already in flight while the
 //     current one is computed; inside the batch the values of edge j are broadcast with warp shuffles,
 //     so no load sits on the critical path of an edge;
-//   * packed FFMA2 arithmetic (two hidden units per instruction), sigmoid from ex2.approx / rcp.approx
-//     (5 instructions; <= 2 ulp each, the result agrees with v1 to ~1e-7 relative);
+//   * float2 arithmetic on two hidden units at a time, sigmoid from ex2.approx / rcp.approx (as v1);
 //   * backward: four edges per inner iteration -- their four grad_h rows are loaded up front and the
 //     4 x 8 partial sums are reduced with one 32-value halving butterfly (31 shuffles instead of
 //     4 x 9) that leaves element `lane` in lane `lane`: grad_emb is written as one 128-byte row.
 // Selected by hidden_variant() below (NQB_HIDDEN_VARIANT / nqb_mlp_hidden_set_variant).
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float ex2_approx(float x) {
-  float r;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-__device__ __forceinline__ float rcp_approx(float x) {
-  float r;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-// 1 / (1 + exp(-p));  p -> -inf gives rcp(inf) = 0, p -> +inf gives rcp(1) = 1
-__device__ __forceinline__ float sigmoid_v2(float p) { return rcp_approx(1.0f + ex2_approx(p * -1.4426950408889634f)); }
 
 struct Basis8 { float4 a, b; };
 __device__ __forceinline__ Basis8 load_basis(const float* __restrict__ emb, int64_t e, int64_t E) {
@@ -168,8 +166,8 @@ __device__ __forceinline__ void preact4(const float (&x)[NB], const float2 (&w01
 #pragma unroll
   for (int k = 0; k < NB; ++k) {
     const float2 xx = make_float2(x[k], x[k]);
-    p01 = __ffma2_rn(xx, w01[k], p01);
-    p23 = __ffma2_rn(xx, w23[k], p23);
+    p01 = fma2_rn(xx, w01[k], p01);
+    p23 = fma2_rn(xx, w23[k], p23);
   }
 }
 
@@ -250,7 +248,7 @@ __global__ void __launch_bounds__(256) k_hidden_bwd2(const float* __restrict__ e
         const float2 gp23 = make_float2(g[u].z * (s2 * fmaf(p23.x, 1.0f - s2, 1.0f)), g[u].w * (s3 * fmaf(p23.y, 1.0f - s3, 1.0f)));
 #pragma unroll
         for (int k = 0; k < NB; ++k) {
-          const float2 t = __ffma2_rn(gp23, w23[k], __fmul2_rn(gp01, w01[k]));
+          const float2 t = fma2_rn(gp23, w23[k], fmul2_rn(gp01, w01[k]));
           v[u * 8 + k] = t.x + t.y;
         }
       }
@@ -291,7 +289,7 @@ static unsigned hidden_grid(int64_t threads) {
   dev &= 63;
   if (sms_dev[dev] == 0) {
     cudaDeviceGetAttribute(&sms_dev[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sms_dev[dev] <= 0) sms_dev[dev] = 148;
+    if (sms_dev[dev] <= 0) sms_dev[dev] = 132;
   }
   const int sms = sms_dev[dev];
   const int64_t need = (threads + 255) / 256, cap = (int64_t)sms * 8;
@@ -330,7 +328,7 @@ static unsigned hidden_grid2(K kernel, int which, int64_t E) {
     int sms = 0, occ = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, 256, 0) != cudaSuccess || occ <= 0) occ = 2;
-    ctas_dev[which][dev] = (sms > 0 ? sms : 148) * occ;
+    ctas_dev[which][dev] = (sms > 0 ? sms : 132) * occ;
   }
   const int64_t need = (((E + 31) >> 5) + 7) / 8;  // 8 warps per CTA, one batch of 32 edges per warp
   return (unsigned)(need < ctas_dev[which][dev] ? need : ctas_dev[which][dev]);

@@ -1,4 +1,4 @@
-// Neighbour list on the GPU (cell list, full list, periodic images), sm_100a.        SURVEY.md section 8(f)-2
+// Neighbour list on the GPU (cell list, full list, periodic images), sm_90a.         SURVEY.md section 8(f)-2
 //
 // Reference contract (paths under /root/reference):
 //   compute_neighborlist_ / backends            nequip/data/_nl.py:60-152, 292-361 -- full list (both directions), no

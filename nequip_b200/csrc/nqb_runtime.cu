@@ -1,4 +1,4 @@
-// libnqb.so -- C-ABI runtime of the B200-native NequIP hot path (see include/nqb.h).
+// libnqb.so -- C-ABI runtime of the H100-native NequIP hot path (see include/nqb.h).
 //
 //  * plan registry: binds a TensorProductScatter signature to the specialised kernel
 //    library generated for it (nequip_b200/codegen.py) via dlopen;
@@ -285,7 +285,7 @@ extern "C" int nqb_csr_check_sorted(const int64_t* keys, int64_t E, int32_t* fla
   if (E > 1) {
     if (!keys) return fail("nqb_csr_check_sorted: null keys");
     int blocks = (int)((E + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     k_check_sorted<<<blocks, 256, 0, (cudaStream_t)st>>>(keys, E, flag_dev);
     NQB_LAUNCH_CHECK("nqb_csr_check_sorted");
   }
@@ -707,7 +707,7 @@ __global__ void k_gate_bwd(const T* __restrict__ x, const T* __restrict__ gout, 
 
 static unsigned gate_grid(int64_t total) {
   const int64_t need = (total + 255) / 256;
-  return (unsigned)(need < 148 * 16 ? need : 148 * 16);
+  return (unsigned)(need < 132 * 16 ? need : 132 * 16);
 }
 
 extern "C" int nqb_gate_fwd(int dtype, const void* x, int64_t N, int d_in, int d_out, const int32_t* src,

@@ -1,6 +1,6 @@
 // Device-side vocabulary shared by every generated tensor-product kernel
 // (nequip_b200/codegen.py).  fp32 kernels work on channel PAIRS held in a float2 so
-// that all arithmetic is packed FFMA2 / FMUL2 (sm_100a); fp64 kernels are scalar.
+// that every operation covers two channels (fma2_rn / fmul2_rn); fp64 kernels are scalar.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -18,11 +18,11 @@ template <> __device__ __forceinline__ float2 vzero<float>() { return make_float
 template <> __device__ __forceinline__ double vzero<double>() { return 0.0; }
 
 // ---- arithmetic -----------------------------------------------------------------
-__device__ __forceinline__ float2 vmul(float2 a, float2 b) { return __fmul2_rn(a, b); }
-__device__ __forceinline__ float2 vfma(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
-// immediate forms: the constant is broadcast to both halves (FFMA2 R, R.F32x2, imm, R)
-__device__ __forceinline__ float2 vmuli(float2 a, float c) { return __fmul2_rn(a, make_float2(c, c)); }
-__device__ __forceinline__ float2 vfmai(float2 a, float c, float2 b) { return __ffma2_rn(a, make_float2(c, c), b); }
+__device__ __forceinline__ float2 vmul(float2 a, float2 b) { return fmul2_rn(a, b); }
+__device__ __forceinline__ float2 vfma(float2 a, float2 b, float2 c) { return fma2_rn(a, b, c); }
+// immediate forms: the constant is broadcast to both halves
+__device__ __forceinline__ float2 vmuli(float2 a, float c) { return fmul2_rn(a, make_float2(c, c)); }
+__device__ __forceinline__ float2 vfmai(float2 a, float c, float2 b) { return fma2_rn(a, make_float2(c, c), b); }
 __device__ __forceinline__ double vmul(double a, double b) { return a * b; }
 __device__ __forceinline__ double vfma(double a, double b, double c) { return fma(a, b, c); }
 __device__ __forceinline__ double vmuli(double a, double c) { return a * c; }

@@ -1,36 +1,27 @@
-// Fused radial-MLP last layer -> tensor product -> scatter, forward (sm_100a).   SURVEY.md section 8(f)-1.
+// Fused radial-MLP last layer -> tensor product -> scatter, forward (sm_90a).   SURVEY.md section 8(f)-1.
 //
-// Reference ops fused here (paths under /root/reference):
+// Reference ops fused here:
 //   edge_weight = h @ (W2 * alpha2)                      nequip/nn/mlp.py:262-268 (last ScalarLinearLayer of
 //                                                         the radial MLP, built at interaction_block.py:119-127)
 //   out = scatter(tp(x[src], edge_attr, edge_weight))     nequip/nn/_tp_scatter_base.py:35-38,
 //                                                         nequip/nn/interaction_block.py:193-199
-// so that the [E, W] edge-weight tensor (92 % of the unfused kernel's bytes) never leaves the SM.
+// so that the [E, W] edge-weight tensor never leaves the SM in an inference-only forward.
 //
-// Decomposition: PATH-parallel.  The W columns (path p, channel u) are cut into slices of 128; a CTA owns ONE
-// slice for a contiguous node range, keeps the slice's second-layer weights W2^T[128 (p,u), K <= 128] (tf32 hi and
-// lo parts) RESIDENT in tensor memory as the MMA "A" operand for its whole life, and streams its edges through
-//   D^T[(p,u), e] = sum_k W2^T[(p,u), k] * h[e, k]            (tcgen05.mma kind::tf32, 3xTF32 split, A from TMEM,
-//                                                              B = the h rows, K-major canonical layout in smem)
-// one destination node (<= 64 edges) per MMA tile.  D^T has TMEM lane = (p,u) and column = edge, which is exactly
-// the thread mapping of the tensor-product arithmetic (thread = one channel of one path, loop over the node's
-// edges): consumer warps read their weights straight from TMEM with tcgen05.ld -- no shared-memory transpose --
-// contract two edges at a time as packed FFMA2 (x = {x[src_e0], x[src_e1]}, Y = {Y_e0, Y_e1}, w = adjacent TMEM
-// columns), keep the node's output in registers and write each output element exactly once (deterministic, no
-// atomics, no zero fill).  Weights are never re-streamed: 128 KB per CTA once, instead of 1.8 MB per 128 edges.
+// Decomposition: PATH-parallel.  The W columns (path p, channel u) are cut into slices of 128 rows; a CTA owns ONE
+// slice for a contiguous node range and keeps the slice's second-layer weights W2^T[128 (p,u), K <= 128] (tf32 hi
+// and lo parts, 128 KB) RESIDENT in shared memory as the wgmma A operand for its whole life.  Per destination node
+// (<= 64 edges per tile) it stages the node's h rows (fp32 = tf32 high operand, plus their low parts) and computes
+//   D^T[(p,u), e] = sum_k W2^T[(p,u), k] * h[e, k]          (wgmma m64n64k8 tf32, 3xTF32 split, fp32 accumulators)
+// Warpgroup g issues the MMAs of rows 64 g .. 64 g + 63, so the weights arrive in its registers in the accumulator
+// fragment layout: thread = rows r, r + 8 (two channels of one path: paths are whole 32-channel blocks) x edge columns
+// 8 j + 2 (lane % 4) + {0, 1}.  That is the thread mapping of the tensor-product arithmetic: each thread contracts
+// its edge PAIRS (x = {x[src_e0], x[src_e1]}, w = adjacent accumulator columns) into per-channel float2 sums held in
+// registers across the node's tiles; at the end of the node the four lanes that share a row add their sums in a fixed
+// order (deterministic, no atomics) and one writes the output element.  Padded edges have weight exactly 0 (their h
+// rows are zero-filled) and finite operands.
 //
-// Roles (512 threads; a first version with one warp per role and quadrant was a set of single-warp latency chains,
-// 10-40 k cycles per tile -- profiles/r02_fused_v1.jsonl):
-//   warps 0-7   consumers: two sets (set = warp / 4) x TMEM lane quadrant (warp % 4); of every 8-edge stage set 0
-//               takes edges 0-3 and set 1 edges 4-7, two edge PAIRS each, branch-free (padded edges have weight
-//               exactly 0 and finite stale operands), so the loads and FFMA2 chains of the pairs interleave; at the
-//               end of a node set 1 hands its partial sums to set 0 through shared memory (fixed order: deterministic)
-//   warps 8-11  h producers: cp.async of the node's h rows (one tile ahead) + tf32 low part
-//   warp  12    MMA issue (one elected lane), TMEM allocation
-//   warps 13-15 x / Y stagers (stage xs belongs to stager xs % 3): 16-byte cp.async pieces of the gathered x rows
-//               (fixed lane -> piece map, source rows fetched one tile ahead) and 4-byte cp.async for the Y pairs.
-//               (One cp.async.bulk per (edge, chunk) was tried first: the bulk-copy unit retires only about one
-//               such request per 100-150 cycles per SM -- 9 k cycles per 55-edge tile, profiles/r02_fused_v2a.txt.)
+// CTA = 2 warpgroups (256 threads), one CTA per SM (about 192 KB of shared memory); h tiles are staged by all
+// threads with 16-byte cp.async into the canonical K-major core-matrix layout.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -39,18 +30,17 @@
 
 namespace {
 
-constexpr int FT_TE = 64;                       // max edges per tile = MMA N
-constexpr int FT_KMAX = 128;                    // resident K (hidden width of the radial MLP)
-constexpr int FT_SUB = 8;                       // edges per x/Y ring stage
-constexpr int FT_TILE_FLOATS = FT_TE * FT_KMAX; // 32 KB
-constexpr int FT_THREADS = 512;
-constexpr int FT_MAXSEG = 4;                    // distinct input chunks a slice may stage per edge
+constexpr int FT_TE = 64;                        // max edges per tile = wgmma N
+constexpr int FT_KMAX = 128;                     // resident K (hidden width of the radial MLP)
+constexpr int FT_ROWS = 128;                     // (path, channel) rows per slice
+constexpr int FT_THREADS = 256;
+constexpr int FT_N3MAX = 7;                      // output components of a path (l <= 3)
 
 struct FusedFwdArgs {
   const float* x;        // [N, D_IN]  ir_mul layout
   const float* y;        // [E, S]
   const float* h;        // [E, ldh]   hidden activations of the radial MLP
-  const float* wprep;    // [NSLICE][hi|lo][128][FT_KMAX]  (nqb_gemm_t_prepare layout, rows in slice order)
+  const float* wprep;    // [NSLICE][hi|lo][128 x FT_KMAX] canonical core-matrix order (ops.FusedTPWeights.prepare)
   const int64_t* row_ptr;
   const int64_t* src;
   float* out;            // [N, D_OUT]
@@ -60,83 +50,10 @@ struct FusedFwdArgs {
   int K;                 // hidden width, multiple of 8, <= FT_KMAX
 };
 
-// tcgen05.mma with the A operand in tensor memory
-__device__ __forceinline__ void ft_umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void ft_tmem_st32(uint32_t taddr, const float* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])),
-      "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])),
-      "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])), "r"(__float_as_uint(v[23])),
-      "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])), "r"(__float_as_uint(v[27])),
-      "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-      : "memory");
-}
-__device__ __forceinline__ void ft_tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// two 32-lane x 16-column loads (hi*hi and cross-term accumulators), one wait
-__device__ __forceinline__ void ft_tmem_ld16x2(uint32_t ta, uint32_t tb, float* va, float* vb) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%32];\n\t"
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%33];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(ta), "r"(tb)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) { va[i] = __uint_as_float(r[i]); vb[i] = __uint_as_float(r[16 + i]); }
-}
-
-__device__ __forceinline__ void ft_cp_async4(void* dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(src_bytes) : "memory");
-}
-// arrive on `bar` once all cp.async operations this thread has issued so far have landed (the arrival is counted
-// in the barrier's expected count: .noinc)
-__device__ __forceinline__ void ft_cp_async_arrive(uint64_t* bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// Per-role stall accounting (generated with GenOptions(fused_prof=True), tools/bench_fused.py --prof): cycles CTA 0's
-// lane 0 of each role spends in each mbarrier wait, and the role's total.
-#ifdef FT_PROF
-__device__ unsigned long long ft_prof[160 * 32];  // per CTA: 4 roles x {6 sections, total, tiles}
-#define FTP_DECL long long pw_[6] = {0, 0, 0, 0, 0, 0}; const long long pt0_ = clock64();
-#define FTP_WAIT(i, stmt) { const long long t_ = clock64(); stmt; pw_[i] += clock64() - t_; }
-#define FTP_END(base, ntiles) { if (blockIdx.x < 160 && (threadIdx.x & 31) == 0) { \
-    for (int i_ = 0; i_ < 6; ++i_) ft_prof[blockIdx.x * 32 + (base) + i_] = (unsigned long long)pw_[i_]; \
-    ft_prof[blockIdx.x * 32 + (base) + 6] = (unsigned long long)(clock64() - pt0_); \
-    ft_prof[blockIdx.x * 32 + (base) + 7] = (unsigned long long)(ntiles); } }
-#else
-#define FTP_DECL
-#define FTP_WAIT(i, stmt) { stmt; }
-#define FTP_END(base, ntiles) {}
-#endif
-
-// shared memory: fixed part; the x/Y ring (NXS stages of STAGE_FLOATS floats) follows it
 struct FtSmem {
-  float hraw[2][FT_TILE_FLOATS];   // h tiles (the fp32 tile is the tf32 high operand: the tensor core truncates)
-  float hlo[2][FT_TILE_FLOATS];    // their tf32 low parts
-  float comb[2][4][7][32];         // set 1 -> set 0 partial sums of a node: [slot][quadrant][component][lane]
-  uint64_t a_full[2], a_done[2], acc_full[2], acc_empty[2], w_full;
-  uint64_t x_full[16], x_empty[16];
-  uint32_t tmem_base;
+  float w[2][FT_ROWS * FT_KMAX];   // W2^T hi, lo
+  float hraw[FT_TE * FT_KMAX];     // h tile (the fp32 values are the tf32 high operand: the tensor core truncates)
+  float hlo[FT_TE * FT_KMAX];      // its tf32 low parts
   int slice, pad_;
   int64_t n0, n1;
 };
@@ -151,184 +68,114 @@ __device__ __forceinline__ int64_t ft_lower_bound(const int64_t* __restrict__ ro
   return lo;
 }
 
-// 32 lanes x 4 columns from each of four TMEM addresses, one wait
-__device__ __forceinline__ void ft_tmem_ld4x4(uint32_t t0, uint32_t t1, uint32_t t2, uint32_t t3, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%16];\n\t"
-      "tcgen05.ld.sync.aligned.32x32b.x4.b32 {%4, %5, %6, %7}, [%17];\n\t"
-      "tcgen05.ld.sync.aligned.32x32b.x4.b32 {%8, %9, %10, %11}, [%18];\n\t"
-      "tcgen05.ld.sync.aligned.32x32b.x4.b32 {%12, %13, %14, %15}, [%19];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(t0), "r"(t1), "r"(t2), "r"(t3)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-// 32 lanes x 4 columns from each of two TMEM addresses, one wait
-__device__ __forceinline__ void ft_tmem_ld4x2(uint32_t t0, uint32_t t1, float* v) {
-  uint32_t r[8];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%8];\n\t"
-      "tcgen05.ld.sync.aligned.32x32b.x4.b32 {%4, %5, %6, %7}, [%9];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-      : "r"(t0), "r"(t1)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void ft_bar_consumers() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-
-// ---------------------------------------------------------------------------------------------------------
-// consumer: one warp = 32 channels of one path (TMEM lanes quad*32 .. +31), half of the edges of every stage
-// PathT (generated): ACTIVE, N1/N2/N3 (= 2l+1), XS_OFF (float offset of the input chunk inside a staged edge row),
-// Y_OFF, W_OFF, MUL, and  fma(x[N1], y[N2], w, acc[N3]),  store(out_row, u, acc),  store_zero(out_row, u)
-// ---------------------------------------------------------------------------------------------------------
-template <class P, class Spec>
-__device__ __forceinline__ void ft_consumer(const FusedFwdArgs& a, FtSmem& S, const float* xring, uint32_t tmem, int set,
-                                            int quad, int lane, int u) {
-  constexpr int NXS = Spec::NXS, XROW = Spec::XROW, SD = Spec::S;
-  constexpr int STAGE_FLOATS = FT_SUB * (XROW + SD);
-  constexpr int NA = P::N3 > 0 ? P::N3 : 1;
-  const uint32_t tlane = tmem + ((uint32_t)(quad * 32) << 16);
-  const int64_t n0 = S.n0, n1 = S.n1;
-  float2 acc[NA];
-#pragma unroll
-  for (int k = 0; k < P::N3; ++k) acc[k] = make_float2(0.f, 0.f);
-  uint32_t it = 0, xs = 0, slot = 0;
-  FTP_DECL
-  for (int64_t n = n0; n < n1; ++n) {
-    const int64_t beg = a.row_ptr[n], end = a.row_ptr[n + 1];
-    if (beg == end) {
-      if (P::ACTIVE && set == 0) P::store_zero(a.out + n * Spec::D_OUT, u);
-      continue;
-    }
-    for (int64_t t0 = beg; t0 < end; t0 += FT_TE, ++it) {
-      const int cnt = (int)((end - t0 < FT_TE) ? (end - t0) : FT_TE);
-      const uint32_t buf = it & 1;
-      FTP_WAIT(0, mbar_wait(&S.acc_full[buf], (it >> 1) & 1))
-      tc_fence_after();
-      // one 8-edge stage per iteration (rolled: the loop body must stay small -- with the stages unrolled the
-      // consumer, producer and stager code of one SM sub-partition exceeded its instruction cache and EVERY
-      // 128-byte line of instructions missed: 44 % of all stall samples were "no instruction",
-      // profiles/r02_ncu_fused_v2_stalls.txt)
-#pragma unroll 1
-      for (int e0 = 0; e0 < cnt; e0 += FT_SUB) {
-        // this set's weights of the stage: TMEM columns e0 + 4 set + {0..3} of the hi*hi and the cross-term accumulator
-        float w[4];
-        {
-          float t[8];
-          const uint32_t b0 = tlane + 256 + buf * 128 + e0 + 4 * set;
-          FTP_WAIT(2, ft_tmem_ld4x2(b0, b0 + 64, t))
-#pragma unroll
-          for (int j = 0; j < 4; ++j) w[j] = t[j] + t[4 + j];
-        }
-        if (e0 + FT_SUB >= cnt) {  // every needed column of this buffer has been read
-          tc_fence_before();
-          mbar_arrive(&S.acc_empty[buf]);
-        }
-        if (P::ACTIVE && a.w_out != nullptr) {
-          float* wo = a.w_out + (t0 + e0 + 4 * set) * (int64_t)Spec::W + P::W_OFF + u;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (e0 + 4 * set + j < cnt) wo[(int64_t)j * Spec::W] = w[j];
-        }
-        const uint32_t st = xs % NXS;
-        FTP_WAIT(1, mbar_wait(&S.x_full[st], (xs / NXS) & 1))
-        if (P::ACTIVE) {
-          // edges e0 + 4 set + {0,1} and {2,3}: no bounds tests -- an edge beyond the node has weight 0
-          const float* xb = xring + (size_t)st * STAGE_FLOATS + (4 * set) * XROW + P::XS_OFF + u;
-          const float2* yb = reinterpret_cast<const float2*>(xring + (size_t)st * STAGE_FLOATS + FT_SUB * XROW) +
-                             (2 * set) * SD + P::Y_OFF;
-          float2 xa[P::N1], ya[P::N2], xc[P::N1], yc[P::N2];
-#pragma unroll
-          for (int i = 0; i < P::N1; ++i) {
-            xa[i] = make_float2(xb[i * P::MUL], xb[XROW + i * P::MUL]);
-            xc[i] = make_float2(xb[2 * XROW + i * P::MUL], xb[3 * XROW + i * P::MUL]);
-          }
-#pragma unroll
-          for (int j = 0; j < P::N2; ++j) { ya[j] = yb[j]; yc[j] = yb[SD + j]; }
-          P::fma(xa, ya, make_float2(w[0], w[1]), acc);
-          P::fma(xc, yc, make_float2(w[2], w[3]), acc);
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&S.x_empty[st]);
-        ++xs;
-      }
-    }
-    // node done: set 1 -> shared memory -> set 0 adds (always in this order) and writes the row
-    if (P::ACTIVE && set == 1) {
-#pragma unroll
-      for (int k = 0; k < P::N3; ++k) S.comb[slot][quad][k][lane] = acc[k].x + acc[k].y;
-    }
-    ft_bar_consumers();
-    if (P::ACTIVE && set == 0) {
-#pragma unroll
-      for (int k = 0; k < P::N3; ++k) acc[k] = make_float2((acc[k].x + acc[k].y) + S.comb[slot][quad][k][lane], 0.f);
-      FTP_WAIT(3, P::store(a.out + n * Spec::D_OUT, u, acc))
-    }
-#pragma unroll
-    for (int k = 0; k < P::N3; ++k) acc[k] = make_float2(0.f, 0.f);
-    slot ^= 1;
-  }
-  if (quad == 0 && set == 0) FTP_END(0, it)
-}
-
 struct FtNullPath {
   static constexpr bool ACTIVE = false;
-  static constexpr int N1 = 1, N2 = 1, N3 = 0, XS_OFF = 0, Y_OFF = 0, W_OFF = 0, MUL = 32;
+  static constexpr int N1 = 1, N2 = 1, N3 = 0, XG_OFF = 0, Y_OFF = 0, W_OFF = 0, MUL = 32;
   static __device__ __forceinline__ void fma(const float2*, const float2*, float2, float2*) {}
-  static __device__ __forceinline__ void store(float*, int, const float2*) {}
+  static __device__ __forceinline__ void store(float*, int, const float*) {}
   static __device__ __forceinline__ void store_zero(float*, int) {}
 };
 
-// tile walker shared by the roles: the node's edges in chunks of FT_TE
-struct FtTile { int64_t t0; int cnt; bool ok; };
-struct FtWalker {
-  const int64_t* row_ptr; int64_t n, n1, off;
-  __device__ FtWalker(const int64_t* rp, int64_t n0_, int64_t n1_) : row_ptr(rp), n(n0_), n1(n1_), off(0) {}
-  __device__ __forceinline__ FtTile next() {
-    FtTile t; t.ok = false; t.t0 = 0; t.cnt = 0;
-    while (n < n1) {
-      const int64_t beg = row_ptr[n], end = row_ptr[n + 1];
-      if (beg + off < end) {
-        t.t0 = beg + off;
-        t.cnt = (int)((end - t.t0 < FT_TE) ? (end - t.t0) : FT_TE);
-        t.ok = true;
-        off += FT_TE;
-        if (beg + off >= end) { ++n; off = 0; }
-        return t;
+// ---------------------------------------------------------------------------------------------------------
+// per-path pieces.  PathP (generated): N1/N2/N3 (= 2l+1), XG_OFF (float offset of the input chunk in an x row),
+// Y_OFF, W_OFF, MUL, and  fma(x[N1], y[N2], w, acc[N3]) on edge pairs,  store(out_row, u, v),  store_zero(out_row, u)
+// ---------------------------------------------------------------------------------------------------------
+// one tile: this thread's edge pairs for channels u0 and u0 + 8 (accumulator rows r, r + 8)
+template <class P, class Spec>
+__device__ __forceinline__ void ft_tile(const FusedFwdArgs& a, int64_t t0, int cnt, int q, int u0, const float* hh,
+                                        const float* xx, float2 (&acc)[2][FT_N3MAX]) {
+  if constexpr (P::ACTIVE) {
+#pragma unroll
+    for (int j = 0; j < FT_TE / 8; ++j) {
+      const int c = 8 * j + 2 * q;
+      if (c < cnt) {
+        // past the node's last edge the second edge of the pair repeats the first: its weights are exactly 0
+        const int64_t e0 = t0 + c, e1 = (c + 1 < cnt) ? e0 + 1 : e0;
+        const float2 w0 = make_float2(hh[4 * j] + xx[4 * j], hh[4 * j + 1] + xx[4 * j + 1]);
+        const float2 w1 = make_float2(hh[4 * j + 2] + xx[4 * j + 2], hh[4 * j + 3] + xx[4 * j + 3]);
+        const float* x0 = a.x + __ldg(a.src + e0) * Spec::D_IN + P::XG_OFF + u0;
+        const float* x1 = a.x + __ldg(a.src + e1) * Spec::D_IN + P::XG_OFF + u0;
+        const float* y0 = a.y + e0 * Spec::S + P::Y_OFF;
+        const float* y1 = a.y + e1 * Spec::S + P::Y_OFF;
+        float2 xa[P::N1], xb[P::N1], ya[P::N2];
+#pragma unroll
+        for (int i = 0; i < P::N1; ++i) {
+          xa[i] = make_float2(__ldg(x0 + i * P::MUL), __ldg(x1 + i * P::MUL));
+          xb[i] = make_float2(__ldg(x0 + i * P::MUL + 8), __ldg(x1 + i * P::MUL + 8));
+        }
+#pragma unroll
+        for (int i = 0; i < P::N2; ++i) ya[i] = make_float2(__ldg(y0 + i), __ldg(y1 + i));
+        P::fma(xa, ya, w0, acc[0]);
+        P::fma(xb, ya, w1, acc[1]);
+        if (a.w_out != nullptr) {
+          float* wo = a.w_out + e0 * (int64_t)Spec::W + P::W_OFF + u0;
+          wo[0] = w0.x;
+          wo[8] = w1.x;
+          if (c + 1 < cnt) { wo[Spec::W] = w0.y; wo[Spec::W + 8] = w1.y; }
+        }
       }
-      ++n; off = 0;
     }
-    return t;
+  }
+}
+
+// end of a node: the four lanes of a row add their sums (fixed order), lane q == 0 writes both channels
+template <class P>
+__device__ __forceinline__ void ft_finish(float* o, int q, int u0, float2 (&acc)[2][FT_N3MAX]) {
+  if constexpr (P::ACTIVE) {
+    float v0[P::N3], v1[P::N3];
+#pragma unroll
+    for (int k = 0; k < P::N3; ++k) {
+      v0[k] = acc[0][k].x + acc[0][k].y;
+      v1[k] = acc[1][k].x + acc[1][k].y;
+      v0[k] += __shfl_xor_sync(0xffffffffu, v0[k], 1);
+      v1[k] += __shfl_xor_sync(0xffffffffu, v1[k], 1);
+      v0[k] += __shfl_xor_sync(0xffffffffu, v0[k], 2);
+      v1[k] += __shfl_xor_sync(0xffffffffu, v1[k], 2);
+    }
+    if (q == 0) {
+      P::store(o, u0, v0);
+      P::store(o, u0 + 8, v1);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < FT_N3MAX; ++k) { acc[0][k] = make_float2(0.f, 0.f); acc[1][k] = make_float2(0.f, 0.f); }
+}
+
+// the per-path steps, called through Spec::dispatch<Op>(slice, block, args...) as Op::run<PathT>(first channel of the
+// warp's 16-row block, args...)
+struct FtZeroOp {
+  template <class P>
+  static __device__ __forceinline__ void run(int ub, float* const& orow, const int& lane) {
+    if ((lane & 3) == 0) { P::store_zero(orow, ub + (lane >> 2)); P::store_zero(orow, ub + (lane >> 2) + 8); }
+  }
+};
+template <class Spec>
+struct FtTileOp {
+  template <class P>
+  static __device__ __forceinline__ void run(int ub, const FusedFwdArgs& a, const int64_t& t0, const int& cnt,
+                                             const int& lane, float (&hh)[32], float (&xx)[32], float2 (&acc)[2][FT_N3MAX]) {
+    ft_tile<P, Spec>(a, t0, cnt, lane & 3, ub + (lane >> 2), hh, xx, acc);
+  }
+};
+struct FtFinishOp {
+  template <class P>
+  static __device__ __forceinline__ void run(int ub, float* const& orow, const int& lane, float2 (&acc)[2][FT_N3MAX]) {
+    ft_finish<P>(orow, lane & 3, ub + (lane >> 2), acc);
   }
 };
 
 // ---------------------------------------------------------------------------------------------------------
-// the kernel.  Spec (generated): MUL, S, D_IN, D_OUT, W, NSLICE, XROW, NXS, seg tables, consume(slice, set, quad, ...)
+// the kernel.  Spec (generated): S, D_IN, D_OUT, W, NSLICE, and dispatch<Op>(slice, block, args...) for the path that
+// owns rows 16 block .. 16 block + 15 of the slice.
+// The MMAs and barriers are outside the per-path code: every thread of a warpgroup runs the same instructions.
 // ---------------------------------------------------------------------------------------------------------
 template <class Spec>
 __global__ void __launch_bounds__(FT_THREADS, 1) tp_fused_fwd_kernel(const FusedFwdArgs a) {
   extern __shared__ __align__(1024) uint8_t ft_smem_raw[];
   FtSmem& S = *reinterpret_cast<FtSmem*>(ft_smem_raw);
-  float* xring = reinterpret_cast<float*>(ft_smem_raw + ((sizeof(FtSmem) + 127) / 128) * 128);
-  constexpr int NXS = Spec::NXS, XROW = Spec::XROW, SD = Spec::S;
-  constexpr int STAGE_FLOATS = FT_SUB * (XROW + SD);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
 
   if (tid == 0) {
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&S.a_full[s], 128); mbar_init(&S.a_done[s], 1);
-      mbar_init(&S.acc_full[s], 1); mbar_init(&S.acc_empty[s], 256);
-    }
-    for (int s = 0; s < NXS; ++s) { mbar_init(&S.x_full[s], 32); mbar_init(&S.x_empty[s], 8); }
-    mbar_init(&S.w_full, 128);
-    fence_barrier_init();
-    // which slice / node range
     int s = 0;
     while (s + 1 < Spec::NSLICE && (int)blockIdx.x >= a.slice_cta0[s + 1]) ++s;
     const int j = (int)blockIdx.x - a.slice_cta0[s], ns = a.slice_cta0[s + 1] - a.slice_cta0[s];
@@ -337,239 +184,82 @@ __global__ void __launch_bounds__(FT_THREADS, 1) tp_fused_fwd_kernel(const Fused
     S.n0 = (j == 0) ? 0 : ft_lower_bound(a.row_ptr, a.N, t_lo);
     S.n1 = (j + 1 == ns) ? a.N : ft_lower_bound(a.row_ptr, a.N, t_hi);
   }
-  // the x / Y ring starts out as zeros: slots of edges beyond a node's last edge are never written, their weights
-  // are exactly 0 and whatever (finite) operands a slot still holds then contribute nothing
-  for (int i = tid; i < NXS * STAGE_FLOATS / 4; i += FT_THREADS) reinterpret_cast<float4*>(xring)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (warp == 12) tmem_alloc(&S.tmem_base, 512);
-  fence_proxy_async();  // the zero fill is ordered before the bulk copies into the ring
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = S.tmem_base;
   const int slice = S.slice;
   const int64_t n0 = S.n0, n1 = S.n1;
-  const int ksteps = a.K / 8;
-  // TMEM columns: [0,128) W hi, [128,256) W lo, per accumulator buffer b: [256 + 128 b, +64) hi*hi, [+64, +128) cross terms
-
-  if (warp < 8) {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 168;");
-    // ================= consumers: set 0 uploads the slice's weights, then the tensor product =================
-    const int set = warp >> 2, quad = warp & 3;
-    if (set == 0) {
-      const uint32_t tlane = tmem + ((uint32_t)(quad * 32) << 16);
-      const float* wrow = a.wprep + ((int64_t)slice * 2 * 128 + quad * 32 + lane) * FT_KMAX;
-#pragma unroll 1
-      for (int part = 0; part < 2; ++part) {
-#pragma unroll 1
-        for (int c = 0; c < FT_KMAX / 32; ++c) {
-          float v[32];
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 t = __ldg(reinterpret_cast<const float4*>(wrow + (int64_t)part * 128 * FT_KMAX + c * 32 + q * 4));
-            v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
-          }
-          ft_tmem_st32(tlane + part * 128 + c * 32, v);
-        }
-      }
-      ft_tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(&S.w_full);
-    }
-    Spec::consume(slice, set, quad, lane, a, S, xring, tmem);
-  } else if (warp < 12) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 80;");
-    // ================= h producers ============================================================================
-    const int pw = warp - 8;
-    const int r8 = lane & 7, kq = lane >> 3;
-    const int kgroups = ksteps * 2;  // 16-byte k-groups the MMAs read
-    FTP_DECL
-    // thread -> rows rg * 8 + r8 (rg < nrg), k-groups kg = (pw + 4 j) * 4 + kq; all addresses by increments
-    const int kg0 = pw * 4 + kq, nkj = (kgroups - pw * 4 + 15) / 16;  // this warp's k-group blocks: kb = pw, pw + 4, ...
-    const int64_t rstep = 8 * a.ldh;
-    auto issue_h = [&](uint32_t it, int64_t t0, int cnt) {
-      float* dst0 = S.hraw[it & 1] + kg0 * 32 + r8 * 4;
-      const float* src0 = a.h + (t0 + r8) * a.ldh + kg0 * 4;
-      const int nrg = ((cnt + 15) & ~15) / 8;  // 8-row groups the MMA reads (N rounded up to 16)
-#pragma unroll 1
-      for (int j = 0; j < nkj; ++j) {
-        float* dst = dst0 + j * (16 * 32);
-        const float* src = src0 + j * 64;
-#pragma unroll 1
-        for (int rg = 0; rg < nrg; rg += 2) {  // nrg is even (N is a multiple of 16)
-          const bool in0 = rg * 8 + r8 < cnt, in1 = rg * 8 + 8 + r8 < cnt;
-          cp_async16(dst, in0 ? src : a.h, in0 ? 16u : 0u);
-          cp_async16(dst + FT_KMAX / 4 * 32, in1 ? (src + rstep) : a.h, in1 ? 16u : 0u);
-          dst += 2 * (FT_KMAX / 4 * 32);
-          src += 2 * rstep;
-        }
-      }
-    };
-    auto lo_pass = [&](uint32_t it, int cnt) {
-      const float* raw0 = S.hraw[it & 1] + kg0 * 32 + r8 * 4;
-      float* lo0 = S.hlo[it & 1] + kg0 * 32 + r8 * 4;
-      const int nrg = ((cnt + 15) & ~15) / 8;
-#pragma unroll 1
-      for (int j = 0; j < nkj; ++j) {
-        const float* raw = raw0 + j * (16 * 32);
-        float* lo = lo0 + j * (16 * 32);
-#pragma unroll 1
-        for (int rg = 0; rg < nrg; rg += 2) {  // nrg is even (N is a multiple of 16)
-          const float4 t0 = *reinterpret_cast<const float4*>(raw), t1 = *reinterpret_cast<const float4*>(raw + FT_KMAX / 4 * 32);
-          *reinterpret_cast<float4*>(lo) = make_float4(tf32_lo(t0.x), tf32_lo(t0.y), tf32_lo(t0.z), tf32_lo(t0.w));
-          *reinterpret_cast<float4*>(lo + FT_KMAX / 4 * 32) = make_float4(tf32_lo(t1.x), tf32_lo(t1.y), tf32_lo(t1.z), tf32_lo(t1.w));
-          raw += 2 * (FT_KMAX / 4 * 32);
-          lo += 2 * (FT_KMAX / 4 * 32);
-        }
-      }
-    };
-    // h one tile ahead: group(it) = { h of tile it }
-    FtWalker wk(a.row_ptr, n0, n1);
-    uint32_t it = 0;
-    FtTile cur = wk.next();
-    if (cur.ok) issue_h(0, cur.t0, cur.cnt);
+  {  // the slice's weights, once (waited for with the first h tile)
+    const float4* src = reinterpret_cast<const float4*>(a.wprep + (int64_t)slice * 2 * FT_ROWS * FT_KMAX);
+    float4* dst = reinterpret_cast<float4*>(&S.w[0][0]);
+    for (int i = tid; i < 2 * FT_ROWS * FT_KMAX / 4; i += FT_THREADS) cp_async16(dst + i, src + i, 16u);
     cp_async_commit();
-    while (cur.ok) {
-      const FtTile nxt = wk.next();
-      if (nxt.ok) {
-        if (it + 1 >= 2) FTP_WAIT(0, mbar_wait(&S.a_done[(it + 1) & 1], (((it + 1) >> 1) - 1) & 1))  // MMAs of tile it - 1 done
-        FTP_WAIT(5, issue_h(it + 1, nxt.t0, nxt.cnt))
+  }
+  const int ksteps = a.K / 8;
+  // h staging: thread -> rows 8 i + r8 (i < 8), k-group kg; a quarter warp writes one 128-byte core matrix
+  const int r8 = tid & 7, kg = tid >> 3;
+  const bool kin = kg < a.K / 4;  // k-groups beyond K are never read by the MMAs
+  const int my_off = kg * 32 + r8 * 4;
+  constexpr uint32_t LBO = 128, SBO = (FT_KMAX / 4) * 128;
+  const uint32_t wg_rows = (uint32_t)wg * (64 / 8) * SBO;  // byte offset of row 64 wg in a weight block
+  const uint64_t dWhi = make_desc(smem_u32(S.w[0]) + wg_rows, LBO, SBO);
+  const uint64_t dWlo = make_desc(smem_u32(S.w[1]) + wg_rows, LBO, SBO);
+  const uint64_t dH = make_desc(smem_u32(S.hraw), LBO, SBO);
+  const uint64_t dL = make_desc(smem_u32(S.hlo), LBO, SBO);
+  const int block = wg * 4 + warp;  // this warp's 16 rows of the slice
+  float2 acc[2][FT_N3MAX];
+#pragma unroll
+  for (int k = 0; k < FT_N3MAX; ++k) { acc[0][k] = make_float2(0.f, 0.f); acc[1][k] = make_float2(0.f, 0.f); }
+  float hh[32], xx[32];
+
+  for (int64_t n = n0; n < n1; ++n) {
+    const int64_t beg = a.row_ptr[n], end = a.row_ptr[n + 1];
+    float* orow = a.out + n * Spec::D_OUT;
+    if (beg == end) {
+      Spec::template dispatch<FtZeroOp>(slice, block, orow, lane);
+      continue;
+    }
+    for (int64_t t0 = beg; t0 < end; t0 += FT_TE) {
+      const int cnt = (int)((end - t0 < FT_TE) ? (end - t0) : FT_TE);
+      __syncthreads();  // both warpgroups' MMAs of the previous tile have completed: h may be overwritten
+      if (kin) {
+#pragma unroll
+        for (int i = 0; i < FT_TE / 8; ++i) {
+          const int row = 8 * i + r8;
+          const bool in = row < cnt;
+          cp_async16(S.hraw + i * (FT_KMAX / 4 * 32) + my_off, in ? a.h + (t0 + row) * a.ldh + kg * 4 : a.h, in ? 16u : 0u);
+        }
       }
       cp_async_commit();
-      FTP_WAIT(2, cp_async_wait<1>())  // h of tile `it` has landed
-      FTP_WAIT(3, lo_pass(it, cur.cnt))
-      fence_proxy_async();
-      mbar_arrive(&S.a_full[it & 1]);
-      cur = nxt;
-      ++it;
-    }
-    cp_async_wait<0>();
-    if (warp == 8) FTP_END(8, it)
-  } else {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-    if (warp == 12) {
-      // ================= MMA issue ===========================================================================
-      const bool leader = elect_one();
-      constexpr uint32_t SBO = (FT_KMAX / 4) * 128, LBO = 128;
-      const uint64_t dR0 = make_desc(smem_u32(S.hraw[0]), LBO, SBO);
-      const uint64_t dL0 = make_desc(smem_u32(S.hlo[0]), LBO, SBO);
-      constexpr uint32_t STAGE = (FT_TILE_FLOATS * sizeof(float)) >> 4;
-      mbar_wait(&S.w_full, 0);
-      tc_fence_after();
-      uint32_t it = 0;
-      FTP_DECL
-      for (int64_t n = n0; n < n1; ++n) {
-        const int64_t beg = a.row_ptr[n], end = a.row_ptr[n + 1];
-        for (int64_t t0 = beg; t0 < end; t0 += FT_TE, ++it) {
-          const int cnt = (int)((end - t0 < FT_TE) ? (end - t0) : FT_TE);
-          const uint32_t buf = it & 1, s = it & 1;
-          const uint32_t idesc = make_idesc(128, (cnt + 15) & ~15);
-          if (it >= 2) { FTP_WAIT(0, mbar_wait(&S.acc_empty[buf], ((it >> 1) - 1) & 1)) tc_fence_after(); }
-          const uint64_t b_hi = dR0 + (uint64_t)(s * STAGE), b_lo = dL0 + (uint64_t)(s * STAGE);
-          const uint32_t d_hh = tmem + 256 + buf * 128, d_x = d_hh + 64;
-          FTP_WAIT(1, mbar_wait(&S.a_full[s], (it >> 1) & 1))
-          if (leader) {
-            // one k-step = 8 tf32 = 8 TMEM columns of the weights, 2 core matrices (16 descriptor units) of the h rows
-#pragma unroll 4
-            for (int ks = 0; ks < ksteps; ++ks) ft_umma_ts(d_hh, tmem + ks * 8, b_hi + ks * 16, idesc, ks > 0);
-#pragma unroll 4
-            for (int ks = 0; ks < ksteps; ++ks) ft_umma_ts(d_x, tmem + 128 + ks * 8, b_hi + ks * 16, idesc, ks > 0);
-#pragma unroll 4
-            for (int ks = 0; ks < ksteps; ++ks) ft_umma_ts(d_x, tmem + ks * 8, b_lo + ks * 16, idesc, 1);
-            umma_commit(&S.a_done[s]);
-            umma_commit(&S.acc_full[buf]);
-          }
-          __syncwarp();
-        }
-      }
-      FTP_END(16, it)
-    } else {
-      // ================= x / Y stagers (warps 13, 14, 15) =====================================================
-      const int sid = warp - 13;
-      const int nseg = Spec::seg_count(slice);
-      int ppe = 0;  // 16-byte pieces per edge
-      for (int sgi = 0; sgi < nseg; ++sgi) ppe += Spec::seg_len(slice, sgi) / 4;
-      constexpr int PCL = (XROW / 4 + 31) / 32;  // pieces per lane and edge
-      int pg[PCL], ps[PCL];
-#pragma unroll
-      for (int i = 0; i < PCL; ++i) {
-        int k = lane + 32 * i, sgi = 0, soff = 0;
-        pg[i] = -1; ps[i] = 0;
-        if (k < ppe) {
-          while (sgi + 1 < nseg && k >= Spec::seg_len(slice, sgi) / 4) { k -= Spec::seg_len(slice, sgi) / 4; soff += Spec::seg_len(slice, sgi); ++sgi; }
-          pg[i] = Spec::seg_goff(slice, sgi) + k * 4;
-          ps[i] = soff + k * 4;
-        }
-      }
-      constexpr int YPL = (FT_SUB * SD + 31) / 32;  // Y elements per lane and stage
-      int ye[YPL], yj[YPL];
-#pragma unroll
-      for (int q = 0; q < YPL; ++q) { const int idx = lane + 32 * q; ye[q] = idx / SD; yj[q] = idx - ye[q] * SD; }
-      FtWalker wk(a.row_ptr, n0, n1);
-      FtTile cur = wk.next();
-      int64_t r0 = 0, r1 = 0, q0 = 0, q1 = 0;  // source rows of the tile's edges lane and 32 + lane (current / next tile)
-      if (cur.ok) {
-        r0 = (lane < cur.cnt) ? __ldg(a.src + cur.t0 + lane) : 0;
-        r1 = (32 + lane < cur.cnt) ? __ldg(a.src + cur.t0 + 32 + lane) : 0;
-      }
-      uint32_t xs = 0, it = 0;
-      FTP_DECL
-      while (cur.ok) {
-        const FtTile nxt = wk.next();
-        if (nxt.ok) {
-          q0 = (lane < nxt.cnt) ? __ldg(a.src + nxt.t0 + lane) : 0;
-          q1 = (32 + lane < nxt.cnt) ? __ldg(a.src + nxt.t0 + 32 + lane) : 0;
-        }
-#pragma unroll 1
-        for (int sb = 0; sb < FT_TE / FT_SUB; ++sb) {
-          const int e0 = sb * FT_SUB;
-          if (e0 < cur.cnt) {
-            if ((int)(xs % 3) == sid) {
-              const uint32_t st = xs % NXS;
-              if (xs >= (uint32_t)NXS) FTP_WAIT(1, mbar_wait(&S.x_empty[st], ((xs / NXS) - 1) & 1))
-              float* stage = xring + (size_t)st * STAGE_FLOATS;
-              const int ne = (cur.cnt - e0 < FT_SUB) ? (cur.cnt - e0) : FT_SUB;
-              const int64_t rsel = (sb < 4) ? r0 : r1;
-              // four edges per iteration: the shuffle -> address -> cp.async chains of the edges interleave
-#pragma unroll 1
-              for (int eb = 0; eb < ne; eb += 4) {
-                const float* xrow[4];
-#pragma unroll
-                for (int q = 0; q < 4; ++q) xrow[q] = a.x + __shfl_sync(0xffffffffu, rsel, (e0 + eb + q) & 31) * Spec::D_IN;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  if (eb + q < ne) {
-                    float* drow = stage + (eb + q) * XROW;
-#pragma unroll
-                    for (int i = 0; i < PCL; ++i)
-                      if (pg[i] >= 0) cp_async16(drow + ps[i], xrow[q] + pg[i], 16u);
-                  }
-                }
-              }
-              float* ys = stage + FT_SUB * XROW;  // [pair][S][2]
-#pragma unroll
-              for (int q = 0; q < YPL; ++q)
-                if (ye[q] < ne) ft_cp_async4(ys + ((ye[q] >> 1) * SD + yj[q]) * 2 + (ye[q] & 1), a.y + (cur.t0 + e0 + ye[q]) * SD + yj[q], 4u);
-              ft_cp_async_arrive(&S.x_full[st]);
-            }
-            ++xs;
-          }
-        }
-        r0 = q0; r1 = q1;
-        cur = nxt;
-        ++it;
-      }
       cp_async_wait<0>();
-      if (sid == 0) FTP_END(24, it)
+      if (kin) {
+#pragma unroll
+        for (int i = 0; i < FT_TE / 8; ++i) {
+          const float4 t = *reinterpret_cast<const float4*>(S.hraw + i * (FT_KMAX / 4 * 32) + my_off);
+          *reinterpret_cast<float4*>(S.hlo + i * (FT_KMAX / 4 * 32) + my_off) =
+              make_float4(tf32_lo(t.x), tf32_lo(t.y), tf32_lo(t.z), tf32_lo(t.w));
+        }
+      }
+      fence_proxy_async();  // generic-proxy writes -> visible to the tensor core
+      __syncthreads();
+      wgmma_fence();
+      // k-step advance = 2 core matrices = 256 bytes = 16 descriptor units
+#pragma unroll 1
+      for (int ks = 0; ks < ksteps; ++ks) wgmma_tf32_m64n64(hh, dWhi + ks * 16, dH + ks * 16, ks > 0);
+#pragma unroll 1
+      for (int ks = 0; ks < ksteps; ++ks) wgmma_tf32_m64n64(xx, dWlo + ks * 16, dH + ks * 16, ks > 0);
+#pragma unroll 1
+      for (int ks = 0; ks < ksteps; ++ks) wgmma_tf32_m64n64(xx, dWhi + ks * 16, dL + ks * 16, 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      Spec::template dispatch<FtTileOp<Spec>>(slice, block, a, t0, cnt, lane, hh, xx, acc);
     }
+    Spec::template dispatch<FtFinishOp>(slice, block, orow, lane, acc);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 12) tmem_dealloc(tmem, 512);
+  cp_async_wait<0>();
 }
 
 template <class Spec>
 inline size_t ft_smem_bytes() {
-  return ((sizeof(FtSmem) + 127) / 128) * 128 + (size_t)Spec::NXS * FT_SUB * (Spec::XROW + Spec::S) * sizeof(float) + 1024;
+  return sizeof(FtSmem) + 1024;
 }
 
 }  // namespace

@@ -1,7 +1,6 @@
 """CUDA-graph replay of the energy + forces step for a fixed (atoms, edges) shape.
 
-One eager step of the 4-layer model is ~260 kernel launches; at 10 k atoms the GPU work is ~15 ms but
-the launch gaps add ~3 ms (profiles/r01_launches_step.md).  The whole step -- edge embedding, every
+One eager step of the 4-layer model is ~260 kernel launches, and the gaps between them add up.  The whole step -- edge embedding, every
 interaction layer, readout and the backward pass that yields the forces -- is captured once into a CUDA
 graph and replayed; inputs are copied into static buffers, outputs are read from static buffers.
 

@@ -1,4 +1,4 @@
-"""Irreps bookkeeping for the B200 hot path (host side, pure Python).
+"""Irreps bookkeeping for the H100 hot path (host side, pure Python).
 
 Mirrors the part of ``e3nn.o3.Irrep`` / ``e3nn.o3.Irreps`` that the reference's
 hot path touches (``nequip/nn/interaction_block.py:89-109`` builds the path

@@ -150,8 +150,7 @@ class _RadialMLPGemmFn(torch.autograd.Function):
         E, hid = emb.shape[0], w1s.shape[1]
         fast = emb.shape[1] == 8 and hid == 128  # fused CUDA-core kernels for the K = 8 layer
         if fast:
-            # (no pre-split low part: handing `a_lo` to k_gemm3x collapses its producer pipeline to one
-            # piece in flight -- 1.7x slower in-step, VERDICT r01 / profiles/r01_gemm_roles.txt)
+            # (no pre-split low part: k_gemm3x computes it from the staged A chunk, which reads A once)
             h = torch.empty((E, hid), dtype=emb.dtype, device=emb.device)
             ops.mlp_hidden_fwd(emb, w1s, h, None)
         else:
@@ -198,7 +197,7 @@ class RadialMLPGemm:
 # ---------------------------------------------------------------------------------------
 class _FusedRadialTPFn(torch.autograd.Function):
     """``out = scatter(TP(x[src], y, silu(emb @ W1 a1) @ W2 a2))`` with the last radial layer fused into the
-    tensor-product kernel (forward: the [E, W] weights are produced in tensor memory and consumed in place;
+    tensor-product kernel (forward: the [E, W] weights are produced in registers and consumed in place;
     they are written once on the side only when a backward pass will need them)."""
 
     @staticmethod

@@ -367,7 +367,7 @@ class InteractionBlock(torch.nn.Module):
         return self._fused_choice
 
     def _note_fallback(self, reason: str):
-        """The library (torch.matmul / cuBLAS) formulation is about to run instead of the tcgen05 blocks: say so
+        """The library (torch.matmul / cuBLAS) formulation is about to run instead of the wgmma blocks: say so
         once per block and reason, or raise when the model was built with ``strict_fast_path=True`` (bench.py,
         smoke(): a silent library fallback would be timed as if it were the product)."""
         if getattr(self, "strict_fast_path", False):
@@ -379,7 +379,7 @@ class InteractionBlock(torch.nn.Module):
             import warnings
 
             warnings.warn(f"nequip_b200 InteractionBlock: dense blocks run through torch.matmul (cuBLAS), not the "
-                          f"tcgen05 kernels: {reason}", RuntimeWarning, stacklevel=3)
+                          f"wgmma kernels: {reason}", RuntimeWarning, stacklevel=3)
 
     def forward(self, x, node_attrs, edge_attrs, edge_embedding, edge_index, types=None, type_table=None,
                 n_own: Optional[int] = None, halo=None):
@@ -393,14 +393,14 @@ class InteractionBlock(torch.nn.Module):
             types = None if types is None else types[:n_own]
         tc = self._tensor_core_blocks(x, types, type_table)
         if tc is not None:
-            # inference fast path: every dense block is one grouped 3xTF32 tcgen05 GEMM launch
+            # inference fast path: every dense block is one grouped 3xTF32 wgmma GEMM launch
             x_in = x
             # 1/sqrt(avg_num_neighbors): folded into the prepared weights (global) or a per-atom row scale (per type)
             x = tc["lin1"](x) if self.norm_shortcut else tc["lin1"](x, self.norm_const.view(-1)[types].view(1, -1).contiguous())
             if halo is not None and not self.is_first_layer:
                 x = halo(x)
             if tc["fused"] is not None and self._use_fused(tc, edge_embedding, x, edge_attrs, edge_index):
-                # one kernel: last radial layer (tcgen05, weights resident in tensor memory) -> TP -> scatter
+                # one kernel: last radial layer (wgmma, weights resident in shared memory) -> TP -> scatter
                 y = tc["fused"](edge_embedding, x, edge_attrs, edge_index[0], edge_index[1])
                 if y is not None:
                     x = y
@@ -570,7 +570,7 @@ class NequIPEnergyModel(torch.nn.Module):
         self.set_strict_fast_path(strict_fast_path)
 
     def set_strict_fast_path(self, on: bool = True):
-        """Raise instead of warning when an interaction block cannot use the tcgen05 dense blocks."""
+        """Raise instead of warning when an interaction block cannot use the wgmma dense blocks."""
         for layer in self.layers:
             layer.conv.strict_fast_path = bool(on)
         return self

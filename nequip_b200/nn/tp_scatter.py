@@ -1,4 +1,4 @@
-"""Drop-in ``TensorProductScatter`` backed by the fused sm_100a kernels.
+"""Drop-in ``TensorProductScatter`` backed by the fused sm_90a kernels.
 
 Mirrors, for the fused CUDA path, what the reference ships for its two third-party
 kernel back-ends:
@@ -143,7 +143,7 @@ def _replace_submodules(model: torch.nn.Module, target_cls, factory) -> torch.nn
 
 
 def enable_B200TensorProductScatter(model: torch.nn.Module) -> torch.nn.Module:
-    """Model modifier: swap every ``TensorProductScatter`` for the fused sm_100a kernel.
+    """Model modifier: swap every ``TensorProductScatter`` for the fused sm_90a kernel.
 
     Same role as ``TensorProductScatter.enable_OpenEquivariance``
     (nequip/nn/_tp_scatter_base.py:40-77).  CPU models are rejected like the
@@ -151,7 +151,7 @@ def enable_B200TensorProductScatter(model: torch.nn.Module) -> torch.nn.Module:
     try:
         p = next(model.parameters())
         if p.device.type == "cpu" and not torch.cuda.is_available():
-            raise RuntimeError("enable_B200TensorProductScatter: CUDA (sm_100a) device required")
+            raise RuntimeError("enable_B200TensorProductScatter: CUDA (sm_90a) device required")
     except StopIteration:
         pass
     return _replace_submodules(model, _Base if not _HAVE_NEQUIP else _RefTensorProductScatter, _factory)

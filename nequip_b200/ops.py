@@ -39,7 +39,7 @@ def _require_cuda(*ts: torch.Tensor):
     for t in ts:
         if t is not None and not t.is_cuda:
             raise RuntimeError(
-                "nequip_b200 kernels run on CUDA (sm_100a) only; got a CPU tensor and there is no CPU fallback"
+                "nequip_b200 kernels run on CUDA (sm_90a) only; got a CPU tensor and there is no CPU fallback"
             )
 
 
@@ -250,8 +250,8 @@ def tp_scatter(plan: TPPlan, x, edge_attr, edge_weight, edge_dst, edge_src, csr:
 # ---------------------------------------------------------------------------------------
 class FusedTPWeights:
     """Second-layer radial-MLP weights ``W2 [K, W]`` (times ``alpha2``) permuted into the slice order of the
-    signature's fused kernel, split hi/lo and laid out for tensor memory (once per model), plus the split of
-    the grid (one CTA per SM) over the slices in proportion to their cost."""
+    signature's fused kernel, split into tf32 hi/lo parts and laid out in the order the kernel's shared memory holds
+    them (once per model), plus the split of the grid (one CTA per SM) over the slices in proportion to their cost."""
 
     def __init__(self, plan: TPPlan, W2: torch.Tensor, alpha2: float, device):
         from .codegen import TPGenerator
@@ -271,12 +271,25 @@ class FusedTPWeights:
         Wp = torch.zeros((K, cols.numel()), dtype=torch.float32, device=device)
         ok = cols >= 0
         Wp[:, ok] = W2d[:, cols[ok]]
-        self.prepared = torch.empty(int(L.nqb_gemm_t_prepared_floats(K, Wp.shape[1])), dtype=torch.float32, device=device)
-        _capi.check(L.nqb_gemm_t_prepare(_ptr(Wp), Wp.shape[1], K, Wp.shape[1], 0, float(alpha2), _ptr(self.prepared),
-                                         _stream()), "nqb_gemm_t_prepare")
+        self.prepared = self.prepare(Wp * float(alpha2), nslice)
         G = torch.cuda.get_device_properties(device).multi_processor_count
         self.cta0, self.nctas = self.split_grid(lay["cost"], G)
         self.cta0_dev = torch.tensor(self.cta0, dtype=torch.int32, device=device)
+
+    @staticmethod
+    def prepare(Wp: torch.Tensor, nslice: int) -> torch.Tensor:
+        """[K, 128 * nslice] -> per slice: hi and lo of W^T [128 rows, 128 k] (K zero padded), each in the canonical
+        K-major core-matrix order of the wgmma A operand: element (r, k) at (r // 8) * 1024 + (k // 4) * 32 +
+        (r % 8) * 4 + k % 4.  hi = round-to-nearest tf32 (ties away from zero), lo = the exact remainder."""
+        K = Wp.shape[0]
+        wt = torch.zeros((nslice, 128, 128), dtype=torch.float32, device=Wp.device)
+        wt[:, :, :K] = Wp.t().reshape(nslice, 128, K)
+        bits = wt.view(torch.int32)
+        hi = ((bits + 0x1000) & -0x2000).view(torch.float32)
+        lo = wt - hi
+        both = torch.stack([hi, lo], 1)  # [slice, part, r, k]
+        both = both.reshape(nslice, 2, 16, 8, 32, 4).permute(0, 1, 2, 4, 3, 5)  # [.., r // 8, k // 4, r % 8, k % 4]
+        return both.contiguous().reshape(-1)
 
     @staticmethod
     def split_grid(cost, G: int):
@@ -544,7 +557,7 @@ def edge_embed(pos, edge_index, shift=None, cell=None, *, lmax: int, num_bessel:
 
 
 # ---------------------------------------------------------------------------------------
-# grouped fp32-accurate GEMM on the tensor cores (tcgen05 3xTF32) -- nqb_gemm_grouped
+# grouped fp32-accurate GEMM on the tensor cores (wgmma 3xTF32) -- nqb_gemm_grouped
 # ---------------------------------------------------------------------------------------
 @dataclass
 class GemmProblem:
@@ -738,32 +751,6 @@ def gate(x: torch.Tensor, tabs: GateTables) -> torch.Tensor:
     if x.dtype not in _DT or x.dim() != 2 or x.shape[1] != tabs.d_in:
         raise ValueError("gate: x must be [N, %d] float32/float64" % tabs.d_in)
     return _GateFn.apply(x, tabs)
-
-
-# ---------------------------------------------------------------------------------------
-# EXPERIMENTAL: transposed K <= 128 GEMM with TMEM-resident weights -- nqb_gemm_t_* (opt-in tests only)
-# ---------------------------------------------------------------------------------------
-class GemmT:
-    """``C[M, N] = A[M, K] @ B[K, N]`` for K <= 128 with ``B`` prepared once."""
-
-    def __init__(self, B: torch.Tensor, device, scale: float = 1.0):
-        L = _capi.lib()
-        self.K, self.N = int(B.shape[0]), int(B.shape[1])
-        if self.K > 128 or self.K % 4:
-            raise ValueError("GemmT: K must be a multiple of 4 and <= 128")
-        Bc = B.detach().to(device=device, dtype=torch.float32).contiguous()
-        self.prepared = torch.empty(int(L.nqb_gemm_t_prepared_floats(self.K, self.N)), dtype=torch.float32, device=device)
-        _capi.check(L.nqb_gemm_t_prepare(_ptr(Bc), Bc.shape[1], self.K, self.N, 0, float(scale), _ptr(self.prepared),
-                                         _stream()), "nqb_gemm_t_prepare")
-
-    def run(self, a: torch.Tensor, c: torch.Tensor) -> torch.Tensor:
-        _require_cuda(a, c)
-        if a.dtype != torch.float32 or c.dtype != torch.float32 or a.stride(1) != 1 or c.stride(1) != 1:
-            raise TypeError("GemmT.run: float32 row-major only")
-        M = a.shape[0]
-        _capi.check(_capi.lib().nqb_gemm_t_run(_ptr(self.prepared), self.K, self.N, _ptr(a), a.stride(0), _ptr(c),
-                                               c.stride(0), M, _stream()), "nqb_gemm_t_run")
-        return c
 
 
 # ---------------------------------------------------------------------------------------

@@ -5,7 +5,7 @@ model as owned + ghost atoms and a per-layer ghost-feature exchange hook
 (``nequip/nn/_ghost_exchange_base.py:8-57``, ``nequip/nn/_ghost_exchange_lmp_mliap.py:11-64``,
 ``nequip/nn/interaction_block.py:159-199``; inputs in the ML-IAP convention,
 ``nequip/integrations/lammps_mliap/lmp_mliap_wrapper.py:202-219``).  This module is the
-B200-native equivalent with ``torch.distributed`` (NCCL over NVLink; gloo in the CPU tests):
+H100-native equivalent with ``torch.distributed`` (NCCL over NVLink; gloo in the CPU tests):
 
 * atoms are split into ``gx x gy x gz`` bricks of equal atom counts (``brick_grid`` picks the
   factorisation with the smallest halo volume: slabs for an elongated box, 3-D bricks for a cubic

@@ -16,7 +16,7 @@ def pytest_configure(config):
         torch.set_num_threads(min(16, os.cpu_count() or 1))
     except Exception:
         pass
-    config.addinivalue_line("markers", "gpu: test needs a CUDA (sm_100a) device")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA (sm_90a) device")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,5 +1,5 @@
 """The two generations of the radial-MLP hidden-layer kernels (nequip_b200/csrc/nqb_mlp.cu: v1 = one edge per warp
-iteration, v2 = batches of 32 edges with prefetched basis values, FFMA2, ex2/rcp sigmoid, four-edge gradient
+iteration, v2 = batches of 32 edges with prefetched basis values, float2 arithmetic, four-edge gradient
 reduction) against each other and against the fp64 restatement of ``silu(emb @ W1 a1)`` and its gradient
 (nequip/nn/mlp.py:262-268), including edge counts that are not multiples of 32 or 4."""
 import math

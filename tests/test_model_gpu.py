@@ -1,4 +1,4 @@
-"""End-to-end energy + force parity: NequIPEnergyModel on the B200 kernels vs the CPU oracle
+"""End-to-end energy + force parity: NequIPEnergyModel on the H100 kernels vs the CPU oracle
 (e3nn formulation) on identical AtomicDataDict-shaped batches -- north_star's 1e-5 relative
 (float32) bar -- plus the reference's property tests restated (finite-difference forces
 model_tests_basic.py:631-672, permutation equivariance :450-461, smooth cutoff :810-843)."""
@@ -99,7 +99,7 @@ def test_permutation_equivariance():
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize("name", ["water_l2_f32", "li3po4_l2_f64feat", "asi_l3"])
 def test_energy_forces_inference_path_tensor_core_mlp(name):
-    """Frozen parameters (inference): the radial MLP runs on the tcgen05 3xTF32 kernels."""
+    """Frozen parameters (inference): the radial MLP runs on the wgmma 3xTF32 kernels."""
     from nequip_b200 import _capi
 
     model, sysd = _build(name, torch.float32)
@@ -196,7 +196,7 @@ def test_edge_force_branch_matches_oracle():
 @pytest.mark.timeout(900)
 def test_bench_size_fp32_kernels_vs_fp64_kernels():
     """The frame bench.py times (10 648 atoms, 588 616 edges, l_max 2, 64 features): the float32 product path
-    (tcgen05 3xTF32 GEMMs, FFMA2 TP kernels, graph-free eager call) against the float64 kernels of the same model
+    (wgmma 3xTF32 GEMMs, float2 TP kernels, graph-free eager call) against the float64 kernels of the same model
     and weights -- no oracle can run at this size in seconds, the fp64 path (itself oracle-checked at 125-1000 atoms)
     is the yardstick.  1e-5 relative on forces, energy and per-atom energies."""
     sysd = D.make_system("li3po4", 22, r_max=5.0, seed=0)

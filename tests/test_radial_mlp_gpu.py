@@ -1,5 +1,5 @@
 """GPU parity of the radial MLP on the product path (CUDA-core hidden layer k_hidden_fwd/bwd + grouped
-tcgen05 3xTF32 GEMM, nequip_b200/nn/dense.py RadialMLPGemm) against the fp64 restatement of
+wgmma 3xTF32 GEMM, nequip_b200/nn/dense.py RadialMLPGemm) against the fp64 restatement of
 ScalarMLPFunction (nequip/nn/mlp.py:80-195, 262-268)."""
 import math
 

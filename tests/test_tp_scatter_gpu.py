@@ -1,7 +1,7 @@
 """GPU parity of the fused TP+scatter kernels against the CPU oracle.
 
 Modelled on the reference's own kernel test
-(/root/reference/tests/unit/nn/test_tp_scatter_kernel.py:34-179): same irreps grid,
+(tests/unit/nn/test_tp_scatter_kernel.py:34-179): same irreps grid,
 same N=8 / E=15 random graph, forward plus gradients w.r.t. x, edge_attr and
 edge_weight, atol = rtol = 1e-5 (float32) / 1e-10 (float64).  The "base
 implementation" it is compared with is oracle.tp (the e3nn formulation restated

@@ -26,21 +26,7 @@ def timeit(fn, reps=20, warm=3):
     return e0.elapsed_time(e1) / reps
 
 
-def prof(tag):
-    import ctypes
-
-    from nequip_b200 import _capi
-
-    buf = (ctypes.c_ulonglong * 16)()
-    _capi.lib().nqb_gemm_prof_read(buf)
-    v = list(buf)
-    print(json.dumps({"prof": tag, "producer": {"wait_a_done": v[0], "wait_group": v[1], "fence_arrive": v[2], "total": v[3]},
-                      "epilogue": {"wait_acc_full": v[4], "tmem_ld": v[5], "emit": v[6], "total": v[7]},
-                      "mma": {"wait_acc_empty": v[8], "wait_b_full": v[9], "wait_a_full": v[10], "total": v[11]}}), flush=True)
-
-
 def main():
-    PROF = "--prof" in sys.argv
     N, T = 10648, 3
     dev = "cuda"
     layers = layer_irreps(2, 64, 4, True)
@@ -59,12 +45,7 @@ def main():
             gx = torch.zeros(N, blk.d_in, device=dev)
             rs = torch.nn.functional.one_hot(types, T).float().t().contiguous() if name == "sc" else None
             f = timeit(lambda: blk.fwd.run(x, out, N, rs))
-            if PROF and li == 2:
-                prof(f"L{li} {name} fwd")
             b = timeit(lambda: blk.bwd.run(out, gx, N, rs))
-            if PROF and li == 2:
-                prof(f"L{li} {name} bwd")
-                print(json.dumps({"bwd_problems": [(p.B.shape[0], p.B.shape[1], p.transposed, p.atomic, p.accumulate) for p in blk.bwd.problems][:8]}))
             flops = 2.0 * N * sum(p.B.shape[0] * p.B.shape[1] for p in blk.fwd.problems)
             print(json.dumps({"layer": li, "block": name, "d_in": blk.d_in, "d_out": blk.d_out,
                               "problems": len(blk.fwd.problems), "ntiles": blk.fwd.ntiles_total,

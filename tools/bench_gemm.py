@@ -38,7 +38,6 @@ def main():
     ap.add_argument("--cases", default="")
     ap.add_argument("--no-cublas", action="store_true")
     ap.add_argument("--presplit", action="store_true", help="also hand the kernel pre-split low parts of A")
-    ap.add_argument("--prof", action="store_true", help="print per-role stall cycles (library built with -DNQB_GEMM_PROF)")
     args = ap.parse_args()
     torch.backends.cuda.matmul.allow_tf32 = False
     E, Nat = int(588616 * args.scale), int(10648 * args.scale)
@@ -56,17 +55,6 @@ def main():
         if args.presplit:
             A_lo = tf32_lo(A)
             ms = timeit(lambda: gg.run(A, C, M, a_lo=A_lo))
-        if args.prof:
-            import ctypes
-
-            from nequip_b200 import _capi
-
-            buf = (ctypes.c_ulonglong * 16)()
-            _capi.lib().nqb_gemm_prof_read(buf)
-            v = list(buf)
-            print(json.dumps({"case": name, "producer": {"wait_a_empty": v[0], "fetch": v[1], "fence_arrive": v[2], "total": v[3]},
-                              "epilogue": {"wait_acc_full": v[4], "tmem_ld": v[5], "emit": v[6], "total": v[7]},
-                              "mma": {"wait_acc_empty": v[8], "wait_b_full": v[9], "wait_a_full": v[10], "total": v[11]}}))
         ref = A[:4096].double() @ B.double()
         err = float((C[:4096].double() - ref).abs().max() / ref.abs().max())
         ms_t = 0.0 if args.no_cublas else timeit(lambda: torch.mm(A, B, out=C), reps=3, warm=1)

@@ -9,7 +9,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
-from bench import WORKLOADS, build_system, load_peaks, tp_algorithmic_bytes, R_MAX  # noqa: E402
+from bench import H100_HBM_GBS, WORKLOADS, build_system, tp_algorithmic_bytes, R_MAX  # noqa: E402
 from nequip_b200 import ops  # noqa: E402
 from nequip_b200 import data as D  # noqa: E402
 from nequip_b200.nn.model import NequIPEnergyModel, ScalarLinearLayer  # noqa: E402
@@ -35,7 +35,7 @@ def main():
     ap.add_argument("--skip-mlp", action="store_true")
     args = ap.parse_args()
     dev = torch.device("cuda")
-    peak, src = load_peaks()
+    peak, src = H100_HBM_GBS, "H100 SXM data sheet (HBM3)"
     sysd, meta, mk = build_system(args.workload, seed=0)
     N, E = sysd["pos"].shape[0], sysd["edge_index"].shape[1]
     model = NequIPEnergyModel(r_max=R_MAX, type_names=meta["type_names"], parity=True,

@@ -25,7 +25,6 @@ VARIANTS = {
     "irmul_noring_split_a64": GenOptions(layout="ir_mul", fwd_ring=False, bwd_ring=False, split_groups=True, acc_cap=64, acc_cap_bwd=64),
     "irmul_ring_a16": GenOptions(layout="ir_mul", acc_cap=16, acc_cap_bwd=16),
 }
-# earlier sweeps (register prefetch, accumulator caps, warps per CTA, red.v2): profiles/r01_tune_tp_variants_*.jsonl
 
 
 def main():
@@ -44,10 +43,10 @@ def main():
     if args.build_only:
         print("built", len(todo))
         return
-    from bench import build_system, tp_algorithmic_bytes, load_peaks
+    from bench import H100_HBM_GBS, build_system, tp_algorithmic_bytes
     from nequip_b200 import ops
 
-    peak, _ = load_peaks()
+    peak = H100_HBM_GBS
     wl = {(2, 64): "li3po4_10k_l2_f64", (2, 32): "water_1k_l2_f32", (3, 32): "asi_50k_l3_f32"}[(lm, nf)]
     sysd, meta, mk = build_system(wl, seed=0)
     dev = torch.device("cuda")
