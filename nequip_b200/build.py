@@ -86,58 +86,31 @@ def spec_lib_path(sig: TPSignature, opts: Optional[GenOptions] = None) -> str:
     return os.path.join(LIBDIR, f"nqbspec_{sig.key(opts)}_{_device_header_hash()}.so")
 
 
-def ensure_spec(sig: TPSignature, opts: Optional[GenOptions] = None, force: bool = False, verbose: bool = False) -> str:
+def ensure_spec(sig: TPSignature, opts: Optional[GenOptions] = None) -> str:
     """Generate + compile the kernel library of one signature (cached in-tree)."""
-    opts = opts or GenOptions()
     out = spec_lib_path(sig, opts)
-    if os.path.exists(out) and not force:
+    if os.path.exists(out):
         return out
-    with _lock:
-        if os.path.exists(out) and not force:
-            return out
-        os.makedirs(LIBDIR, exist_ok=True)
-        os.makedirs(GENDIR, exist_ok=True)
-        # several ranks may JIT the same signature at once: every process writes its own source and
-        # temporary library, the final rename is atomic
-        cu = os.path.join(GENDIR, os.path.basename(out)[:-3] + f".{os.getpid()}.cu")
-        with open(cu, "w") as f:
-            f.write(generate(sig, opts))
-        final_cu = os.path.join(GENDIR, os.path.basename(out)[:-3] + ".cu")
-        tmp = out + f".tmp{os.getpid()}"
-        cmd = [nvcc_path(), *ARCH_FLAGS, *COMMON_FLAGS, "-I", CSRC, "-o", tmp, cu]
-        if verbose:
-            cmd.insert(1, "-Xptxas=-v")
-        log = _run(cmd)
-        os.replace(tmp, out)
-        os.replace(cu, final_cu)
-        if verbose:
-            print(log)
+    os.makedirs(LIBDIR, exist_ok=True)
+    os.makedirs(GENDIR, exist_ok=True)
+    # several processes (ranks) or threads may build the same signature at once: each writes its own source and
+    # temporary library, and the final renames are atomic
+    stem = os.path.join(GENDIR, os.path.basename(out)[:-3])
+    uniq = f"{os.getpid()}_{threading.get_ident()}"
+    cu, tmp = f"{stem}.{uniq}.cu", f"{out}.tmp{uniq}"
+    with open(cu, "w") as f:
+        f.write(generate(sig, opts))
+    _run([nvcc_path(), *ARCH_FLAGS, *COMMON_FLAGS, "-I", CSRC, "-o", tmp, cu])
+    os.replace(tmp, out)
+    os.replace(cu, stem + ".cu")
     return out
 
 
 def ensure_specs(sigs: Iterable[Tuple[TPSignature, Optional[GenOptions]]], jobs: int = 0) -> List[str]:
     """Parallel build of many signatures (used by __graft_entry__.build)."""
-    todo = list(sigs)
     jobs = jobs or min(8, os.cpu_count() or 1)
-
-    def one(item):
-        sig, opts = item
-        opts = opts or GenOptions()
-        out = spec_lib_path(sig, opts)
-        if os.path.exists(out):
-            return out
-        os.makedirs(LIBDIR, exist_ok=True)
-        os.makedirs(GENDIR, exist_ok=True)
-        cu = os.path.join(GENDIR, os.path.basename(out)[:-3] + ".cu")
-        with open(cu, "w") as f:
-            f.write(generate(sig, opts))
-        tmp = out + f".tmp{os.getpid()}_{threading.get_ident()}"
-        _run([nvcc_path(), *ARCH_FLAGS, *COMMON_FLAGS, "-I", CSRC, "-o", tmp, cu])
-        os.replace(tmp, out)
-        return out
-
     with ThreadPoolExecutor(max_workers=jobs) as ex:
-        return list(ex.map(one, todo))
+        return list(ex.map(lambda item: ensure_spec(*item), sigs))
 
 
 __all__ = [

@@ -157,27 +157,21 @@ class TPSignature:
 
 @dataclass
 class GenOptions:
-    nwarp: int = 4  # warps (= destination nodes) per CTA
-    acc_cap: int = 32  # max output components per channel held by one warp (forward)
-    acc_cap_bwd: int = 32
-    prefetch: bool = True  # software-pipelined edge loop (loads of edge i+1 in flight during compute of i)
-    idx_ahead: bool = True  # edge/source indices fetched two iterations ahead (breaks the dependent-load chain)
-    min_blocks_fwd: int = 4  # __launch_bounds__ minBlocksPerSM (0 = unset); occupancy beats everything else here
-    min_blocks_bwd: int = 3
-    red_v2: bool = True  # grad_x via red.global.add.v2.f32 (two adjacent floats per atomic)
-    fwd_ring: bool = True  # forward v2: one CTA per node, weight rows streamed through a cp.async.bulk smem ring
-    ring_stages: int = 4
-    bwd_ring: bool = True  # backward v2 (same weight ring)
-    split_groups: bool = False  # register (v1) kernels: one launch per path group instead of one launch for all --
-    #                              every SM then executes ONE group's (large, fully unrolled) body at a time
     layout: str = "mul_ir"  # node-feature layout of x / out: "mul_ir" (the reference's, e3nn) or
     #                         "ir_mul" (channel-contiguous: every chunk is [2l+1, mul]; all node-feature
     #                         traffic becomes unit-stride 8-byte accesses; used between our own kernels)
 
     def tag(self) -> str:
-        return (f"w{self.nwarp}_a{self.acc_cap}_b{self.acc_cap_bwd}_p{int(self.prefetch)}{int(self.idx_ahead)}"
-                f"_m{self.min_blocks_fwd}{self.min_blocks_bwd}_r{int(self.red_v2)}_{self.layout}_g{int(self.fwd_ring)}{self.ring_stages}{int(self.bwd_ring)}"
-                + ("_sg" if self.split_groups else ""))
+        return self.layout
+
+
+# Fixed kernel parameters, the same for every signature.
+NWARP = 4  # warps (= destination nodes) per CTA of the register kernels
+ACC_CAP = 32  # max output components per channel held by one warp: the budget of a path group
+# __launch_bounds__ minBlocksPerSM of the register kernels; occupancy beats everything else here
+MIN_BLOCKS_FWD, MIN_BLOCKS_BWD = 4, 3
+RING_STAGES = 4  # depth of the shared-memory weight ring of the ring kernels
+RING_CAP = 256  # edges whose ids the ring kernels stage in shared memory per pass
 
 
 # ---------------------------------------------------------------------------
@@ -216,6 +210,44 @@ def _pow2ceil(n: int) -> int:
     while p < n:
         p *= 2
     return p
+
+
+def _aligned(*offsets: int) -> str:
+    """Template argument telling a vector access whether its 8-byte (two-float) accesses are aligned: every row
+    width and offset that goes into the address is even."""
+    return "true" if all(o % 2 == 0 for o in offsets) else "false"
+
+
+def _ring_names(bwd: bool) -> Tuple[str, str, str]:
+    """Per-direction names in the ring-form source: constant prefix, group count, CTA barrier."""
+    return ("B2", "NGB", "cta_sync_b") if bwd else ("F2", "NGF", "cta_sync")
+
+
+def _emit_switch(em: _Emitter, on: str, calls: List[str]):
+    em.block(f"switch ({on})")
+    for gid, call in enumerate(calls):
+        em(f"case {gid}: {call}; break;")
+    em("default: break;")
+    em.end()
+
+
+def _emit_smem_attr(em: _Emitter, kernels: List[str], nbytes: str):
+    """Raise the dynamic shared-memory limit of ``kernels`` to ``nbytes``, once per device."""
+    em("static bool attr_set[64] = {false};  // per device")
+    em("int dev_ = 0; cudaGetDevice(&dev_); dev_ &= 63;")
+    em.block("if (!attr_set[dev_])")
+    for i, k in enumerate(kernels):
+        em(("cudaError_t e_ = " if i == 0 else "if (e_ == cudaSuccess) e_ = ")
+           + f"cudaFuncSetAttribute({k}, cudaFuncAttributeMaxDynamicSharedMemorySize, {nbytes});")
+    em("if (e_ != cudaSuccess) return (int)e_;")
+    em("attr_set[dev_] = true;")
+    em.end()
+
+
+def _emit_v1_launch(em: _Emitter, ng: str, tname: str, kernel: str, args: str):
+    """Launch of a register (v1) kernel: all path groups in one grid (blockIdx.y = group, channel block)."""
+    em(f"{{ dim3 grid_((unsigned)((N + NWARP - 1) / NWARP), {ng} * VT<{tname}>::CB); "
+       f"{kernel}<<<grid_, block, 0, st>>>({args}, 0); }}")
 
 
 def _partition(sig: TPSignature, acc_cap: int) -> List[List[Path]]:
@@ -267,8 +299,20 @@ class TPGenerator:
         self.sig = sig
         self.opts = opts or GenOptions()
         self.mul_max = max(p.mul for p in sig.paths)
-        self.fwd_groups = _partition(sig, self.opts.acc_cap)
-        self.bwd_groups = _partition(sig, self.opts.acc_cap_bwd)
+        self.groups = _partition(sig, ACC_CAP)  # the same path groups in the forward and the backward
+        # dynamic shared memory of a ring kernel: weight ring + its full/empty mbarriers + staged edge and source ids
+        epw = self.geometry(2)[1]
+        self.ring_smem_bytes = RING_STAGES * epw * sig.weight_numel * 4 + 2 * RING_STAGES * 8 + RING_CAP * 16
+        # the ring pays off when several warps (path groups) share one node's weight rows; single-group
+        # signatures (3-4 paths: first/last layer) keep the register-resident v1 kernel (measured)
+        # (and only while the ring fits: a signature whose ring would exceed ~200 KB keeps the register kernel)
+        # ... and only when one edge fills the warp (mul >= 64 -> EPW == 1): with two or more edges per warp iteration the
+        # ring is EPW x larger per CTA (70-140 KB for the l_max = 3 layers -> 1-3 CTAs per SM) and the register kernels
+        # keep more warps resident
+        self.use_ring = (sig.weight_numel % 4 == 0 and len(self.groups) >= 2 and epw == 1
+                         and self.ring_smem_bytes <= 200 * 1024)
+        self.use_ring_bwd = self.use_ring  # same groups, same ring: both directions make the same choice
+        self.has_fused = self.fused_layout() is not None
 
     def out_ir_mul(self, io: int):
         """ir_mul placement of output chunk ``io``: the layout is defined over
@@ -317,48 +361,63 @@ class TPGenerator:
         em("V " + ", ".join(n + sfx for n in names) + ";")
         em(f"bool valid{sfx}; int64_t e{sfx}, sn{sfx};")
 
-    def _emit_index_loads(self, em: _Emitter, sfx: str, sbase: str):
+    def _emit_chunk_ptr(self, em: _Emitter, ptr: str, base: str, row: str, c: int, out: bool):
+        """Declare ``ptr``, this lane's first element of chunk ``c`` of row ``row`` of ``base`` (an input-1 row, or an
+        output row when ``out``), in the generator's layout.  Returns the template arguments of the vload / vstore
+        family for the chunk and the distance between its components."""
+        sig = self.sig
+        irr, width = (sig.irreps_out, sig.d_out) if out else (sig.irreps_in1, sig.d_in)
+        mul, ir = irr[c]
+        if self.opts.layout == "ir_mul":
+            if out:
+                boff, mtot, ubase = self.out_ir_mul(c)
+                off, stride, al = boff + ubase, mtot, _aligned(width, boff, mtot, ubase)
+            else:
+                off, stride = irr.offsets()[c], mul
+                al = _aligned(width, off, mul)
+            em(f"{ptr} = {base} + {row} * {width} + {off} + ch0;")
+            return f"{mul}, {al}", stride
+        em(f"{ptr} = {base} + {row} * {width} + {irr.offsets()[c]} + (int64_t)ch0 * {ir.dim};")
+        return f"{ir.dim}, {mul}", 1
+
+    def _emit_yx_loads(self, em: _Emitter, paths: List[Path], sfx: str, decl: str):
+        """Load the harmonics of edge ``e{sfx}`` and gather the x row of its source ``sn{sfx}`` into ``y{j}{sfx}`` and
+        ``x{i1}_{i}{sfx}``; ``decl`` is "" (assign) or "const V " (declare)."""
+        yused, _ = self._edge_vars(paths)
+        for j in yused:
+            em(f"{decl}y{j}{sfx} = vsplat(__ldg(y + e{sfx} * {self.sig.s_dim} + {j}));")
+        ld = "vloadc" if self.opts.layout == "ir_mul" else "vload"
+        for i1 in sorted({p.i1 for p in paths}):
+            targs, stride = self._emit_chunk_ptr(em, f"const T* xp{i1}", "x", f"sn{sfx}", i1, out=False)
+            for i in range(self.sig.irreps_in1[i1][1].dim):
+                em(f"{decl}x{i1}_{i}{sfx} = {ld}<{targs}>(xp{i1} + {i * stride}, ch0);")
+
+    def _emit_index_loads(self, em: _Emitter, sbase: str):
+        """Edge id and source index of slot ``sbase + sub`` into the look-ahead set N."""
         em.block()
         em(f"int64_t s = {sbase} + sub;")
-        em(f"valid{sfx} = s < end;")
-        em(f"if (!valid{sfx}) s = beg;")
-        em(f"e{sfx} = perm ? perm[s] : s;")
-        em(f"sn{sfx} = src[e{sfx}];")
+        em("validN = s < end;")
+        em("if (!validN) s = beg;")
+        em("eN = perm ? perm[s] : s;")
+        em("snN = src[eN];")
         em.end()
 
     def _emit_data_loads(self, em: _Emitter, paths: List[Path], sfx: str, mask_w: bool):
         """Issue the data loads of one edge iteration into the ``sfx`` register set: the streamed
         weights first (they only need the edge id), then the harmonics, then the gathered x row."""
-        sig = self.sig
-        S = sig.s_dim
+        W = self.sig.weight_numel
+        zero = f"valid{sfx}" if mask_w else "true"
         em.block()
         for p in paths:
-            zero = f"valid{sfx}" if mask_w else "true"
-            al = "true" if (sig.weight_numel % 2 == 0 and p.woff % 2 == 0) else "false"
-            em(f"w{p.idx}{sfx} = vloadw<{p.mul}, {al}>(w + e{sfx} * {sig.weight_numel} + {p.woff} + ch0, ch0, {zero});")
-        yused, _ = self._edge_vars(paths)
-        for j in yused:
-            em(f"y{j}{sfx} = vsplat(__ldg(y + e{sfx} * {S} + {j}));")
-        for i1 in sorted({p.i1 for p in paths}):
-            mul, ir = sig.irreps_in1[i1]
-            n1 = ir.dim
-            xoff = sig.irreps_in1.offsets()[i1]
-            if self.opts.layout == "ir_mul":
-                al = "true" if (sig.d_in % 2 == 0 and xoff % 2 == 0 and mul % 2 == 0) else "false"
-                em(f"const T* xp{i1} = x + sn{sfx} * {sig.d_in} + {xoff} + ch0;")
-                for i in range(n1):
-                    em(f"x{i1}_{i}{sfx} = vloadc<{mul}, {al}>(xp{i1} + {i * mul}, ch0);")
-            else:
-                em(f"const T* xp{i1} = x + sn{sfx} * {sig.d_in} + {xoff} + (int64_t)ch0 * {n1};")
-                for i in range(n1):
-                    em(f"x{i1}_{i}{sfx} = vload<{n1}, {mul}>(xp{i1} + {i}, ch0);")
+            em(f"w{p.idx}{sfx} = vloadw<{p.mul}, {_aligned(W, p.woff)}>(w + e{sfx} * {W} + {p.woff} + ch0, ch0, {zero});")
+        self._emit_yx_loads(em, paths, sfx, "")
         em.end()
 
-    def _emit_pipelined_loop(self, em: _Emitter, paths: List[Path], body: "_Emitter", mask_w: bool):
+    def _emit_pipelined_loop(self, em: _Emitter, paths: List[Path], body: _Emitter, mask_w: bool):
         """Software-pipelined edge loop: the loads of iteration i+1 are in flight while iteration i
-        computes (two explicit register sets A/B, loop unrolled by two, no register moves); with
-        ``idx_ahead`` the edge id / source index of iteration i+2 are fetched during iteration i so the
-        dependent chain perm -> src -> x[src] never stalls the issue of the data loads."""
+        computes (two explicit register sets A/B, loop unrolled by two, no register moves); the edge id /
+        source index of iteration i+2 are fetched during iteration i (set N) so the dependent chain
+        perm -> src -> x[src] never stalls the issue of the data loads."""
         import re
 
         _, names = self._edge_vars(paths)
@@ -370,64 +429,114 @@ class TPGenerator:
                 em(pat.sub(lambda m: m.group(1) + sfx, ln))
             em.end()
 
-        if not self.opts.prefetch:
-            self._emit_edge_decls(em, paths, "")
-            em.block("for (int64_t s0 = beg; s0 < end; s0 += EPW)")
-            self._emit_index_loads(em, "", "s0")
-            self._emit_data_loads(em, paths, "", mask_w)
-            emit_body("")
-            em.end()
-            return
         self._emit_edge_decls(em, paths, "A")
         self._emit_edge_decls(em, paths, "B")
         em.block("if (beg < end)")
         em("int64_t s0 = beg;")
-        if not self.opts.idx_ahead:
-            self._emit_index_loads(em, "A", "s0")
-            self._emit_data_loads(em, paths, "A", mask_w)
-            em.block("while (true)")
-            for cur, nxt in (("A", "B"), ("B", "A")):
-                self._emit_index_loads(em, nxt, "(s0 + EPW)")
-                self._emit_data_loads(em, paths, nxt, mask_w)
-                emit_body(cur)
-                em("s0 += EPW; if (s0 >= end) break;")
-            em.end()
-        else:
-            em("bool validN; int64_t eN, snN;")
-            self._emit_index_loads(em, "N", "s0")
-            em("validA = validN; eA = eN; snA = snN;")
-            self._emit_index_loads(em, "N", "(s0 + EPW)")
-            self._emit_data_loads(em, paths, "A", mask_w)
-            em.block("while (true)")
-            for cur, nxt in (("A", "B"), ("B", "A")):
-                em(f"valid{nxt} = validN; e{nxt} = eN; sn{nxt} = snN;")
-                self._emit_index_loads(em, "N", "(s0 + 2 * EPW)")
-                self._emit_data_loads(em, paths, nxt, mask_w)
-                emit_body(cur)
-                em("s0 += EPW; if (s0 >= end) break;")
-            em.end()
+        em("bool validN; int64_t eN, snN;")
+        self._emit_index_loads(em, "s0")
+        em("validA = validN; eA = eN; snA = snN;")
+        self._emit_index_loads(em, "(s0 + EPW)")
+        self._emit_data_loads(em, paths, "A", mask_w)
+        em.block("while (true)")
+        for cur, nxt in (("A", "B"), ("B", "A")):
+            em(f"valid{nxt} = validN; e{nxt} = eN; sn{nxt} = snN;")
+            self._emit_index_loads(em, "(s0 + 2 * EPW)")
+            self._emit_data_loads(em, paths, nxt, mask_w)
+            emit_body(cur)
+            em("s0 += EPW; if (s0 >= end) break;")
+        em.end()
         em.end()
 
-    # -- forward ---------------------------------------------------------------------
-    def _emit_fwd_group(self, em: _Emitter, gid: int, paths: List[Path]):
-        sig = self.sig
+    def _emit_ring_loop(self, em: _Emitter, paths: List[Path], body: _Emitter, bwd: bool, mask_w: bool):
+        """Edge loop of the ring form: per pass, the ids of up to RING_CAP edges are staged in shared memory and
+        their weight rows are streamed into the ring by one elected lane of warp 0."""
+        W = self.sig.weight_numel
+        P, NG, sync = _ring_names(bwd)
+        em("uint32_t base = 0;" + ("" if bwd else "  // ring iterations completed in earlier passes"))
+        em.block(f"for (int64_t c0 = beg; c0 < end; c0 += {P}_CAP)")
+        em(f"const int cnt = (int)((end - c0 < {P}_CAP) ? (end - c0) : {P}_CAP);")
+        em(f"{sync}();")
+        em.block(f"for (int i = warp * 32 + lane; i < cnt; i += 32 * {NG})")
+        em("const int64_t e_ = perm ? perm[c0 + i] : (c0 + i);")
+        em("eids[i] = e_; srcs[i] = src[e_];")
+        em.end()
+        em(f"{sync}();")
+        em("const int niter = (cnt + EPW - 1) / EPW;")
+        # producer helper
+        em.block("auto issue = [&](int j)")
+        em(f"const uint32_t gj = base + j, sj = gj % {P}_STAGES;")
+        em(f"if (gj >= {P}_STAGES) mbar_wait(&empty[sj], ((gj / {P}_STAGES) - 1) & 1);")
+        em("const int r0 = j * EPW;")
+        em("const int rows = (cnt - r0 < EPW) ? (cnt - r0) : EPW;")
+        em(f"mbar_expect_tx(&full[sj], (uint32_t)rows * {W * 4}u);")
+        em(f"for (int r = 0; r < rows; ++r) bulk_g2s(ring + (size_t)(sj * EPW + r) * {W}, w + eids[r0 + r] * {W}, {W * 4}u, &full[sj]);")
+        em.end("};")
+        em.block("if (warp == 0 && lane == 0)")
+        em(f"for (int j = 0; j < {P}_STAGES - 1 && j < niter; ++j) issue(j);")
+        em.end()
+        em.block("for (int it = 0; it < niter; ++it)")
+        em(f"if (warp == 0 && lane == 0 && it + {P}_STAGES - 1 < niter) issue(it + {P}_STAGES - 1);")
+        em(f"const uint32_t gi = base + it, st = gi % {P}_STAGES;")
+        em("int slot = it * EPW + sub;")
+        em("const bool valid = slot < cnt;")
+        em("if (!valid) slot = 0;")
+        em("const int64_t e = eids[slot], sn = srcs[slot];")
+        # x and y first (global / L2), then wait for the ring
+        self._emit_yx_loads(em, paths, "", "const V ")
+        em(f"mbar_wait(&full[st], (gi / {P}_STAGES) & 1);")
+        em(f"const float* wrow = ring + (size_t)(st * EPW + (valid ? sub : 0)) * {W};")
+        for p in paths:
+            em(f"const V w{p.idx} = vloadws<{p.mul}, {_aligned(W, p.woff)}>(wrow + {p.woff} + ch0, ch0, {'valid' if mask_w else 'true'});")
+        em("__syncwarp();")
+        em("if (lane == 0) mbar_arrive(&empty[st]);")
+        em.block()
+        for ln in body.lines:
+            em(ln)
+        em.end()
+        em.end()  # it loop
+        em("base += niter;")
+        em.end()  # pass loop
+
+    def _emit_group(self, em: _Emitter, gid: int, paths: List[Path], bwd: bool, ring: bool):
+        """Device function of one path group: ``fwd_g*`` / ``bwd_g*`` (register form, float or double) or
+        ``fwd2_g*`` / ``bwd2_g*`` (ring form, float)."""
+        T = "float" if ring else "T"
+        tparams = ([] if ring else ["typename T"]) + (["bool WANT_GX"] if bwd else [])
+        args = [f"const {T}* __restrict__ x", f"const {T}* __restrict__ y", f"const {T}* __restrict__ w",
+                "const int64_t* __restrict__ perm", "const int64_t* __restrict__ src"]
+        args += [f"const {T}* __restrict__ gout"] if bwd else []
+        args += ["int64_t n", "int64_t beg", "int64_t end", "int ch0", "int sub"] + (["int cl"] if bwd else [])
+        if ring:
+            args += ["int warp", "int lane", "float* ring", "uint64_t* full", "uint64_t* empty", "int64_t* eids", "int64_t* srcs"]
+        args += ([f"{T}* __restrict__ gx", f"{T}* __restrict__ gy", f"{T}* __restrict__ gw", "bool det"] if bwd
+                 else [f"{T}* __restrict__ out"])
+        name = ("bwd" if bwd else "fwd") + ("2" if ring else "") + f"_g{gid}"
+        em.block((f"template <{', '.join(tparams)}> " if tparams else "")
+                 + f"__device__ __forceinline__ void {name}(" + ", ".join(args) + ")")
+        if ring:
+            em("typedef float T; typedef VT<float>::V V; constexpr int EPW = VT<float>::EPW; constexpr int LPE = VT<float>::LPE;")
+        else:
+            em("typedef typename VT<T>::V V; constexpr int EPW = VT<T>::EPW; constexpr int LPE = VT<T>::LPE;")
         outs = sorted({p.io for p in paths})
-        em.block(
-            f"template <typename T> __device__ __forceinline__ void fwd_g{gid}("
-            "const T* __restrict__ x, const T* __restrict__ y, const T* __restrict__ w, "
-            "const int64_t* __restrict__ perm, const int64_t* __restrict__ src, "
-            "int64_t n, int64_t beg, int64_t end, int ch0, int sub, T* __restrict__ out)"
-        )
-        em("typedef typename VT<T>::V V; constexpr int EPW = VT<T>::EPW; constexpr int LPE = VT<T>::LPE;")
-        for io in outs:
-            n3 = sig.irreps_out[io][1].dim
-            em("V " + ", ".join(f"a{io}_{k} = vzero<T>()" for k in range(n3)) + ";")
-        body = self._fwd_body(paths)
-        self._emit_pipelined_loop(em, paths, body, True)
-        self._emit_fwd_epilogue(em, outs)
+        if bwd:
+            self._emit_bwd_prologue(em, paths)
+        else:
+            for io in outs:
+                n3 = self.sig.irreps_out[io][1].dim
+                em("V " + ", ".join(f"a{io}_{k} = vzero<T>()" for k in range(n3)) + ";")
+        body = self._bwd_body(paths) if bwd else self._fwd_body(paths)
+        mask_w = not bwd  # the forward zeroes the weights of a padding slot; the backward discards its results
+        if ring:
+            self._emit_ring_loop(em, paths, body, bwd, mask_w)
+        else:
+            self._emit_pipelined_loop(em, paths, body, mask_w)
+        if not bwd:
+            self._emit_fwd_epilogue(em, outs)
         em.end()
         em()
 
+    # -- forward ---------------------------------------------------------------------
     def _fwd_body(self, paths: List[Path]) -> _Emitter:
         """Per-edge forward math on un-suffixed names (x{i1}_{i}, y{j}, w{p}, accumulators a{io}_{k})."""
         em = _Emitter()
@@ -480,138 +589,22 @@ class TPGenerator:
                 em(f"a{io}_{k} = vfold<LPE>(a{io}_{k});")
         em.end()
         em.block("if (sub == 0)")
+        st = "vstorew" if self.opts.layout == "ir_mul" else "vstore"
         for io in outs:
-            mul, ir = sig.irreps_out[io]
-            n3 = ir.dim
-            ooff = sig.irreps_out.offsets()[io]
-            if self.opts.layout == "ir_mul":
-                boff, mtot, ubase = self.out_ir_mul(io)
-                al = "true" if (sig.d_out % 2 == 0 and boff % 2 == 0 and mtot % 2 == 0 and ubase % 2 == 0) else "false"
-                em(f"T* op{io} = out + n * {sig.d_out} + {boff + ubase} + ch0;")
-                for k in range(n3):
-                    em(f"vstorew<{mul}, {al}>(op{io} + {k * mtot}, a{io}_{k}, ch0);")
-            else:
-                em(f"T* op{io} = out + n * {sig.d_out} + {ooff} + (int64_t)ch0 * {n3};")
-                for k in range(n3):
-                    em(f"vstore<{n3}, {mul}>(op{io} + {k}, a{io}_{k}, ch0);")
+            targs, stride = self._emit_chunk_ptr(em, f"T* op{io}", "out", "n", io, out=True)
+            for k in range(sig.irreps_out[io][1].dim):
+                em(f"{st}<{targs}>(op{io} + {k * stride}, a{io}_{k}, ch0);")
         em.end()
-
-    def _emit_fwd2_group(self, em: _Emitter, gid: int, paths: List[Path]):
-        """Forward v2 (float): the node's weight rows arrive through a shared-memory ring filled by
-        cp.async.bulk (one elected lane of warp 0), edge/source ids are staged in shared memory."""
-        sig = self.sig
-        S, W = sig.s_dim, sig.weight_numel
-        outs = sorted({p.io for p in paths})
-        em.block(
-            f"__device__ __forceinline__ void fwd2_g{gid}("
-            "const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ w, "
-            "const int64_t* __restrict__ perm, const int64_t* __restrict__ src, "
-            "int64_t n, int64_t beg, int64_t end, int ch0, int sub, int warp, int lane, "
-            "float* ring, uint64_t* full, uint64_t* empty, int64_t* eids, int64_t* srcs, float* __restrict__ out)"
-        )
-        em("typedef float T; typedef VT<float>::V V; constexpr int EPW = VT<float>::EPW; constexpr int LPE = VT<float>::LPE;")
-        for io in outs:
-            n3 = sig.irreps_out[io][1].dim
-            em("V " + ", ".join(f"a{io}_{k} = vzero<T>()" for k in range(n3)) + ";")
-        em("uint32_t base = 0;  // ring iterations completed in earlier passes")
-        em.block("for (int64_t c0 = beg; c0 < end; c0 += F2_CAP)")
-        em("const int cnt = (int)((end - c0 < F2_CAP) ? (end - c0) : F2_CAP);")
-        em("cta_sync();")
-        em.block("for (int i = warp * 32 + lane; i < cnt; i += 32 * NGF)")
-        em("const int64_t e_ = perm ? perm[c0 + i] : (c0 + i);")
-        em("eids[i] = e_; srcs[i] = src[e_];")
-        em.end()
-        em("cta_sync();")
-        em("const int niter = (cnt + EPW - 1) / EPW;")
-        # producer helper
-        em.block("auto issue = [&](int j)")
-        em("const uint32_t gj = base + j, sj = gj % F2_STAGES;")
-        em("if (gj >= F2_STAGES) mbar_wait(&empty[sj], ((gj / F2_STAGES) - 1) & 1);")
-        em("const int r0 = j * EPW;")
-        em("const int rows = (cnt - r0 < EPW) ? (cnt - r0) : EPW;")
-        em(f"mbar_expect_tx(&full[sj], (uint32_t)rows * {W * 4}u);")
-        em(f"for (int r = 0; r < rows; ++r) bulk_g2s(ring + (size_t)(sj * EPW + r) * {W}, w + eids[r0 + r] * {W}, {W * 4}u, &full[sj]);")
-        em.end("};")
-        em.block("if (warp == 0 && lane == 0)")
-        em("for (int j = 0; j < F2_STAGES - 1 && j < niter; ++j) issue(j);")
-        em.end()
-        em.block("for (int it = 0; it < niter; ++it)")
-        em("if (warp == 0 && lane == 0 && it + F2_STAGES - 1 < niter) issue(it + F2_STAGES - 1);")
-        em("const uint32_t gi = base + it, st = gi % F2_STAGES;")
-        em("int slot = it * EPW + sub;")
-        em("const bool valid = slot < cnt;")
-        em("if (!valid) slot = 0;")
-        em("const int64_t e = eids[slot], sn = srcs[slot];")
-        # x and y first (global / L2), then wait for the ring
-        yused, names = self._edge_vars(paths)
-        for j in yused:
-            em(f"const V y{j} = vsplat(__ldg(y + e * {S} + {j}));")
-        for i1 in sorted({p.i1 for p in paths}):
-            mul, ir = sig.irreps_in1[i1]
-            n1 = ir.dim
-            xoff = sig.irreps_in1.offsets()[i1]
-            if self.opts.layout == "ir_mul":
-                al = "true" if (sig.d_in % 2 == 0 and xoff % 2 == 0 and mul % 2 == 0) else "false"
-                em(f"const T* xp{i1} = x + sn * {sig.d_in} + {xoff} + ch0;")
-                for i in range(n1):
-                    em(f"const V x{i1}_{i} = vloadc<{mul}, {al}>(xp{i1} + {i * mul}, ch0);")
-            else:
-                em(f"const T* xp{i1} = x + sn * {sig.d_in} + {xoff} + (int64_t)ch0 * {n1};")
-                for i in range(n1):
-                    em(f"const V x{i1}_{i} = vload<{n1}, {mul}>(xp{i1} + {i}, ch0);")
-        em("mbar_wait(&full[st], (gi / F2_STAGES) & 1);")
-        em(f"const float* wrow = ring + (size_t)(st * EPW + (valid ? sub : 0)) * {W};")
-        for p in paths:
-            al = "true" if (W % 2 == 0 and p.woff % 2 == 0) else "false"
-            em(f"const V w{p.idx} = vloadws<{p.mul}, {al}>(wrow + {p.woff} + ch0, ch0, valid);")
-        em("__syncwarp();")
-        em("if (lane == 0) mbar_arrive(&empty[st]);")
-        body = self._fwd_body(paths)
-        em.block()
-        for ln in body.lines:
-            em(ln)
-        em.end()
-        em.end()  # it loop
-        em("base += niter;")
-        em.end()  # pass loop
-        self._emit_fwd_epilogue(em, outs)
-        em.end()
-        em()
 
     # -- backward ---------------------------------------------------------------------
-    def _emit_bwd_group(self, em: _Emitter, gid: int, paths: List[Path]):
-        em.block(
-            f"template <typename T, bool WANT_GX> __device__ __forceinline__ void bwd_g{gid}("
-            "const T* __restrict__ x, const T* __restrict__ y, const T* __restrict__ w, "
-            "const int64_t* __restrict__ perm, const int64_t* __restrict__ src, const T* __restrict__ gout, "
-            "int64_t n, int64_t beg, int64_t end, int ch0, int sub, int cl, "
-            "T* __restrict__ gx, T* __restrict__ gy, T* __restrict__ gw, bool det)"
-        )
-        em("typedef typename VT<T>::V V; constexpr int EPW = VT<T>::EPW; constexpr int LPE = VT<T>::LPE;")
-        self._emit_bwd_prologue(em, paths)
-        body = self._bwd_body(paths)
-        self._emit_pipelined_loop(em, paths, body, False)
-        em.end()
-        em()
-
     def _emit_bwd_prologue(self, em: _Emitter, paths: List[Path]):
         """grad_out rows of this node (resident in registers for the whole edge loop) + reduce constants."""
         sig = self.sig
-        outs = sorted({p.io for p in paths})
-        for io in outs:
-            mul, ir = sig.irreps_out[io]
-            n3 = ir.dim
-            ooff = sig.irreps_out.offsets()[io]
-            if self.opts.layout == "ir_mul":
-                boff, mtot, ubase = self.out_ir_mul(io)
-                al = "true" if (sig.d_out % 2 == 0 and boff % 2 == 0 and mtot % 2 == 0 and ubase % 2 == 0) else "false"
-                em(f"const T* gp{io} = gout + n * {sig.d_out} + {boff + ubase} + ch0;")
-                for k in range(n3):
-                    em(f"const V g{io}_{k} = vloadc<{mul}, {al}>(gp{io} + {k * mtot}, ch0);")
-            else:
-                em(f"const T* gp{io} = gout + n * {sig.d_out} + {ooff} + (int64_t)ch0 * {n3};")
-                for k in range(n3):
-                    em(f"const V g{io}_{k} = vload<{n3}, {mul}>(gp{io} + {k}, ch0);")
+        ld = "vloadc" if self.opts.layout == "ir_mul" else "vload"
+        for io in sorted({p.io for p in paths}):
+            targs, stride = self._emit_chunk_ptr(em, f"const T* gp{io}", "gout", "n", io, out=True)
+            for k in range(sig.irreps_out[io][1].dim):
+                em(f"const V g{io}_{k} = {ld}<{targs}>(gp{io} + {k * stride}, ch0);")
         yused, _ = self._edge_vars(paths)
         Pq = _pow2ceil(yused[-1] + 1 - yused[0])
         em(f"const int qbase = er_base<LPE, {Pq}>(cl); const bool qlead = er_leader<LPE, {Pq}>(cl);")
@@ -619,7 +612,7 @@ class TPGenerator:
     def _bwd_body(self, paths: List[Path]) -> _Emitter:
         """Per-edge backward math on un-suffixed names (inputs x, y, w, valid, e, sn; resident g)."""
         sig = self.sig
-        S = sig.s_dim
+        S, W = sig.s_dim, sig.weight_numel
         yused, _ = self._edge_vars(paths)
         em = _Emitter()
         em("V " + ", ".join(f"q{j} = vzero<T>()" for j in yused) + ";")
@@ -639,8 +632,7 @@ class TPGenerator:
                     for k in range(1, n1):
                         em(f"r{p.idx} = vfma(x{i1}_{k}, g{p.io}_{k}, r{p.idx});")
                     em(f"const V ky{p.idx} = vmuli(y{yoff}, {_imm(kappa)});")
-                    al = "true" if (sig.weight_numel % 2 == 0 and p.woff % 2 == 0) else "false"
-                    em(f"if (valid) vstorew<{p.mul}, {al}>(gw + e * {sig.weight_numel} + {p.woff} + ch0, vmul(ky{p.idx}, r{p.idx}), ch0);")
+                    em(f"if (valid) vstorew<{p.mul}, {_aligned(W, p.woff)}>(gw + e * {W} + {p.woff} + ch0, vmul(ky{p.idx}, r{p.idx}), ch0);")
                     em(f"q{yoff} = vfma(vmuli(w{p.idx}, {_imm(kappa)}), r{p.idx}, q{yoff});")
                     em.block("if (WANT_GX)")
                     em(f"const V ws = vmul(w{p.idx}, ky{p.idx});")
@@ -683,35 +675,31 @@ class TPGenerator:
                     em(f"V r{p.idx} = vmul(g{p.io}_{ks[0]}, v{p.idx}_{ks[0]});")
                     for k in ks[1:]:
                         em(f"r{p.idx} = vfma(g{p.io}_{k}, v{p.idx}_{k}, r{p.idx});")
-                    al = "true" if (sig.weight_numel % 2 == 0 and p.woff % 2 == 0) else "false"
-                    em(f"if (valid) vstorew<{p.mul}, {al}>(gw + e * {sig.weight_numel} + {p.woff} + ch0, r{p.idx}, ch0);")
+                    em(f"if (valid) vstorew<{p.mul}, {_aligned(W, p.woff)}>(gw + e * {W} + {p.woff} + ch0, r{p.idx}, ch0);")
             em.end()
         # grad_x: atomics into the source row -- or, in deterministic mode, plain stores into the EDGE's own row of a
         # [E, D_in] buffer that nqb_segment_sum reduces over the (source-sorted) edges in a fixed order
         em.block("if (WANT_GX && valid)")
         em("const int64_t gxr = det ? e : sn;")
         for i1 in sorted({p.i1 for p in paths}):
-            mul, ir = sig.irreps_in1[i1]
-            n1 = ir.dim
-            xoff = sig.irreps_in1.offsets()[i1]
+            n1 = sig.irreps_in1[i1][1].dim
+            targs, stride = self._emit_chunk_ptr(em, f"T* gxp{i1}", "gx", "gxr", i1, out=False)
             if self.opts.layout == "ir_mul":
-                al = "true" if (self.opts.red_v2 and sig.d_in % 2 == 0 and xoff % 2 == 0 and mul % 2 == 0) else "false"
-                em(f"T* gxp{i1} = gx + gxr * {sig.d_in} + {xoff} + ch0;")
                 for i in range(n1):
-                    em(f"if (det) vstorew<{mul}, {al}>(gxp{i1} + {i * mul}, d{i1}_{i}, ch0); else vatomicc<{mul}, {al}>(gxp{i1} + {i * mul}, d{i1}_{i}, ch0);")
+                    dst = f"gxp{i1} + {i * stride}, d{i1}_{i}, ch0"
+                    em(f"if (det) vstorew<{targs}>({dst}); else vatomicc<{targs}>({dst});")
                 continue
-            em(f"T* gxp{i1} = gx + gxr * {sig.d_in} + {xoff} + (int64_t)ch0 * {n1};")
             em.block("if (det)")
             for i in range(n1):
-                em(f"vstore<{n1}, {mul}>(gxp{i1} + {i}, d{i1}_{i}, ch0);")
+                em(f"vstore<{targs}>(gxp{i1} + {i}, d{i1}_{i}, ch0);")
             em.end()
             em.block("else")
-            if self.opts.red_v2 and sig.d_in % 2 == 0 and xoff % 2 == 0:
+            if _aligned(sig.d_in, sig.irreps_in1.offsets()[i1]) == "true":  # the row's float2 pairs: red.global.add.v2
                 args = ", ".join(f"d{i1}_{i}" for i in range(n1))
-                em(f"vatomic_row<{n1}, {mul}>(gxp{i1}, ch0, {args});")
+                em(f"vatomic_row<{targs}>(gxp{i1}, ch0, {args});")
             else:
                 for i in range(n1):
-                    em(f"vatomic<{n1}, {mul}>(gxp{i1} + {i}, d{i1}_{i}, ch0);")
+                    em(f"vatomic<{targs}>(gxp{i1} + {i}, d{i1}_{i}, ch0);")
             em.end()
         em.end()
         # grad_Y: halving reduce-scatter over the lanes that share this edge, then one atomic per component
@@ -726,82 +714,6 @@ class TPGenerator:
         em(f"for (int j = 0; j < QC; ++j) if (qbase + j < {y1 - y0}) atomicAdd(gy + e * {S} + {y0} + qbase + j, qv[j]);")
         em.end()
         return em
-
-    def _emit_bwd2_group(self, em: _Emitter, gid: int, paths: List[Path]):
-        """Backward v2 (float): same shared-memory weight ring as forward v2."""
-        sig = self.sig
-        S, W = sig.s_dim, sig.weight_numel
-        em.block(
-            f"template <bool WANT_GX> __device__ __forceinline__ void bwd2_g{gid}("
-            "const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ w, "
-            "const int64_t* __restrict__ perm, const int64_t* __restrict__ src, const float* __restrict__ gout, "
-            "int64_t n, int64_t beg, int64_t end, int ch0, int sub, int cl, int warp, int lane, "
-            "float* ring, uint64_t* full, uint64_t* empty, int64_t* eids, int64_t* srcs, "
-            "float* __restrict__ gx, float* __restrict__ gy, float* __restrict__ gw, bool det)"
-        )
-        em("typedef float T; typedef VT<float>::V V; constexpr int EPW = VT<float>::EPW; constexpr int LPE = VT<float>::LPE;")
-        self._emit_bwd_prologue(em, paths)
-        em("uint32_t base = 0;")
-        em.block("for (int64_t c0 = beg; c0 < end; c0 += B2_CAP)")
-        em("const int cnt = (int)((end - c0 < B2_CAP) ? (end - c0) : B2_CAP);")
-        em("cta_sync_b();")
-        em.block("for (int i = warp * 32 + lane; i < cnt; i += 32 * NGB)")
-        em("const int64_t e_ = perm ? perm[c0 + i] : (c0 + i);")
-        em("eids[i] = e_; srcs[i] = src[e_];")
-        em.end()
-        em("cta_sync_b();")
-        em("const int niter = (cnt + EPW - 1) / EPW;")
-        em.block("auto issue = [&](int j)")
-        em("const uint32_t gj = base + j, sj = gj % B2_STAGES;")
-        em("if (gj >= B2_STAGES) mbar_wait(&empty[sj], ((gj / B2_STAGES) - 1) & 1);")
-        em("const int r0 = j * EPW;")
-        em("const int rows = (cnt - r0 < EPW) ? (cnt - r0) : EPW;")
-        em(f"mbar_expect_tx(&full[sj], (uint32_t)rows * {W * 4}u);")
-        em(f"for (int r = 0; r < rows; ++r) bulk_g2s(ring + (size_t)(sj * EPW + r) * {W}, w + eids[r0 + r] * {W}, {W * 4}u, &full[sj]);")
-        em.end("};")
-        em.block("if (warp == 0 && lane == 0)")
-        em("for (int j = 0; j < B2_STAGES - 1 && j < niter; ++j) issue(j);")
-        em.end()
-        em.block("for (int it = 0; it < niter; ++it)")
-        em("if (warp == 0 && lane == 0 && it + B2_STAGES - 1 < niter) issue(it + B2_STAGES - 1);")
-        em("const uint32_t gi = base + it, st = gi % B2_STAGES;")
-        em("int slot = it * EPW + sub;")
-        em("const bool valid = slot < cnt;")
-        em("if (!valid) slot = 0;")
-        em("const int64_t e = eids[slot], sn = srcs[slot];")
-        yused, names = self._edge_vars(paths)
-        for j in yused:
-            em(f"const V y{j} = vsplat(__ldg(y + e * {S} + {j}));")
-        for i1 in sorted({p.i1 for p in paths}):
-            mul, ir = sig.irreps_in1[i1]
-            n1 = ir.dim
-            xoff = sig.irreps_in1.offsets()[i1]
-            if self.opts.layout == "ir_mul":
-                al = "true" if (sig.d_in % 2 == 0 and xoff % 2 == 0 and mul % 2 == 0) else "false"
-                em(f"const T* xp{i1} = x + sn * {sig.d_in} + {xoff} + ch0;")
-                for i in range(n1):
-                    em(f"const V x{i1}_{i} = vloadc<{mul}, {al}>(xp{i1} + {i * mul}, ch0);")
-            else:
-                em(f"const T* xp{i1} = x + sn * {sig.d_in} + {xoff} + (int64_t)ch0 * {n1};")
-                for i in range(n1):
-                    em(f"const V x{i1}_{i} = vload<{n1}, {mul}>(xp{i1} + {i}, ch0);")
-        em("mbar_wait(&full[st], (gi / B2_STAGES) & 1);")
-        em(f"const float* wrow = ring + (size_t)(st * EPW + (valid ? sub : 0)) * {W};")
-        for p in paths:
-            al = "true" if (W % 2 == 0 and p.woff % 2 == 0) else "false"
-            em(f"const V w{p.idx} = vloadws<{p.mul}, {al}>(wrow + {p.woff} + ch0, ch0, true);")
-        em("__syncwarp();")
-        em("if (lane == 0) mbar_arrive(&empty[st]);")
-        body = self._bwd_body(paths)
-        em.block()
-        for ln in body.lines:
-            em(ln)
-        em.end()
-        em.end()  # it loop
-        em("base += niter;")
-        em.end()  # pass loop
-        em.end()
-        em()
 
     # -- fused radial-MLP + TP + scatter forward (csrc/nqb_tp_fused.cuh) ---------------------
     def path_cost(self, p: Path) -> int:
@@ -899,10 +811,8 @@ class TPGenerator:
         em.end()
         em.end("};")
 
-    def _emit_fused(self, em: _Emitter) -> bool:
+    def _emit_fused(self, em: _Emitter):
         lay = self.fused_layout()
-        if lay is None:
-            return False
         sig = self.sig
         mul, slices = lay["mul"], lay["slices"]
         for grp in slices:
@@ -924,16 +834,80 @@ class TPGenerator:
         em.end()
         em.end()
         em.end("};")
-        return True
 
-    def _emit_v1_launch(self, em: _Emitter, ng: str, tname: str, kernel: str, args: str):
-        """Launch of a register (v1) kernel: all path groups in one grid, or one launch per group (split_groups)."""
-        if self.opts.split_groups:
-            em(f"for (int g_ = 0; g_ < {ng}; ++g_) {{ dim3 grid_((unsigned)((N + NWARP - 1) / NWARP), VT<{tname}>::CB); "
-               f"{kernel}<<<grid_, block, 0, st>>>({args}, g_); }}")
+    # -- kernels ----------------------------------------------------------------------
+    @staticmethod
+    def _kernel_params(T: str, bwd: bool) -> str:
+        p = (f"const {T}* __restrict__ x, const {T}* __restrict__ y, const {T}* __restrict__ w, "
+             "const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ perm, const int64_t* __restrict__ src, ")
+        if bwd:
+            return p + (f"const {T}* __restrict__ gout, int64_t N, "
+                        f"{T}* __restrict__ gx, {T}* __restrict__ gy, {T}* __restrict__ gw, int det, int64_t gy_slice")
+        return p + f"int64_t N, {T}* __restrict__ out"
+
+    def _emit_v1_kernel(self, em: _Emitter, bwd: bool):
+        """Register form: one warp per (node, path group, channel block), NWARP nodes per CTA; opens the kernel body."""
+        if bwd:
+            tparams, name, minb = "typename T, bool WANT_GX", "tp_bwd_kernel", MIN_BLOCKS_BWD
         else:
-            em(f"{{ dim3 grid_((unsigned)((N + NWARP - 1) / NWARP), {ng} * VT<{tname}>::CB); "
-               f"{kernel}<<<grid_, block, 0, st>>>({args}, 0); }}")
+            tparams, name, minb = "typename T", "tp_fwd_kernel", MIN_BLOCKS_FWD
+        em.block(f"template <{tparams}> __global__ void __launch_bounds__(32 * NWARP, {minb}) {name}("
+                 + self._kernel_params("T", bwd) + ", int grp0)")
+        em("constexpr int CB = VT<T>::CB, LPE = VT<T>::LPE, CPT = VT<T>::CPT;")
+        em("const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;")
+        em("const int64_t n = (int64_t)blockIdx.x * NWARP + warp;")
+        em("if (n >= N) return;")
+        em("const int grp = grp0 + blockIdx.y / CB, cb = blockIdx.y % CB;")
+        em("const int sub = lane / LPE, cl = lane % LPE;")
+        em("const int ch0 = (cb * LPE + cl) * CPT;")
+        em("const int64_t beg = row_ptr[n], end = row_ptr[n + 1];")
+        if bwd:
+            calls = [f"bwd_g{g}<T, WANT_GX>(x, y, w, perm, src, gout, n, beg, end, ch0, sub, cl, "
+                     "gx, gy + (int64_t)(grp * CB + cb) * gy_slice, gw, det != 0)" for g in range(len(self.groups))]
+        else:
+            calls = [f"fwd_g{g}<T>(x, y, w, perm, src, n, beg, end, ch0, sub, out)" for g in range(len(self.groups))]
+        _emit_switch(em, "grp", calls)
+
+    def _emit_ring_kernel(self, em: _Emitter, bwd: bool):
+        """Ring form: one CTA per (node, channel block), one warp per path group; carves the dynamic shared memory
+        (weight ring, full/empty mbarriers, staged edge and source ids), initialises the barriers and dispatches the
+        warps to their groups; opens the kernel body."""
+        P, NG, _ = _ring_names(bwd)
+        smem = P.lower() + "_smem"
+        if bwd:
+            minb = max(1, min(16, 384 // (32 * len(self.groups))))
+            em.block(f"template <bool WANT_GX> __global__ void __launch_bounds__(32 * NGB, {minb}) tp_bwd2_kernel("
+                     + self._kernel_params("float", bwd) + ")")
+        else:
+            minb = max(1, min(16, 512 // (32 * len(self.groups))))
+            em.block(f"__global__ void __launch_bounds__(32 * NGF, {minb}) tp_fwd2_kernel(" + self._kernel_params("float", bwd) + ")")
+        em(f"extern __shared__ __align__(16) uint8_t {smem}[];")
+        em("constexpr int LPE = VT<float>::LPE, CPT = VT<float>::CPT, EPW = VT<float>::EPW;")
+        em(f"constexpr size_t RING_FLOATS = (size_t){P}_STAGES * EPW * {self.sig.weight_numel};")
+        em(f"float* ring = reinterpret_cast<float*>({smem});")
+        em(f"uint64_t* full = reinterpret_cast<uint64_t*>({smem} + RING_FLOATS * sizeof(float));")
+        em(f"uint64_t* empty = full + {P}_STAGES;")
+        em(f"int64_t* eids = reinterpret_cast<int64_t*>(empty + {P}_STAGES);")
+        em(f"int64_t* srcs = eids + {P}_CAP;")
+        em("const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;")
+        em("const int64_t n = blockIdx.x;")
+        em("const int cb = blockIdx.y;")
+        em("const int sub = lane / LPE, cl = lane % LPE;")
+        em("const int ch0 = (cb * LPE + cl) * CPT;")
+        em("const int64_t beg = row_ptr[n], end = row_ptr[n + 1];")
+        em.block("if (threadIdx.x == 0)")
+        em(f"for (int s_ = 0; s_ < {P}_STAGES; ++s_) {{ mbar_init(&full[s_], 1); mbar_init(&empty[s_], {NG}); }}")
+        em("fence_barrier_init();")
+        em.end()
+        em("__syncthreads();")
+        if bwd:
+            calls = [f"bwd2_g{g}<WANT_GX>(x, y, w, perm, src, gout, n, beg, end, ch0, sub, cl, warp, lane, "
+                     "ring, full, empty, eids, srcs, gx, gy + (int64_t)(warp * gridDim.y + blockIdx.y) * gy_slice, gw, det != 0)"
+                     for g in range(len(self.groups))]
+        else:
+            calls = [f"fwd2_g{g}(x, y, w, perm, src, n, beg, end, ch0, sub, warp, lane, ring, full, empty, eids, srcs, out)"
+                     for g in range(len(self.groups))]
+        _emit_switch(em, "warp", calls)
 
     # -- translation unit ----------------------------------------------------------------
     def source(self) -> str:
@@ -943,12 +917,12 @@ class TPGenerator:
         lpe_d, epw_d, cb_d = self.geometry(1)
         em(f"// AUTO-GENERATED by nequip_b200/codegen.py (v{CODEGEN_VERSION}) -- do not edit.")
         em(f"// signature: {sig.canonical()}")
-        em(f"// options: {self.opts.tag()}  fwd_groups={len(self.fwd_groups)} bwd_groups={len(self.bwd_groups)}")
+        em(f"// layout: {self.opts.layout}  path_groups={len(self.groups)}  ring={int(self.use_ring)}")
         em(f"// forward multiply-accumulates per (edge, channel): {sig.fma_count()}")
         em("#include <cuda_runtime.h>")
         em('#include "nqb_tc.cuh"')
         em("namespace {")
-        em(f"constexpr int NWARP = {self.opts.nwarp};")
+        em(f"constexpr int NWARP = {NWARP};")
         em("template <typename T> struct VT;")
         em(
             f"template <> struct VT<float> {{ typedef float2 V; static constexpr int CPT = 2, LPE = {lpe_f}, "
@@ -958,64 +932,28 @@ class TPGenerator:
             f"template <> struct VT<double> {{ typedef double V; static constexpr int CPT = 1, LPE = {lpe_d}, "
             f"EPW = {epw_d}, CB = {cb_d}; }};"
         )
-        em(f"constexpr int NGF = {len(self.fwd_groups)};")
-        em(f"constexpr int NGB = {len(self.bwd_groups)};")
+        em(f"constexpr int NGF = {len(self.groups)};")
+        em(f"constexpr int NGB = {len(self.groups)};")
         em("}  // namespace")
         em('#include "nqb_tp_device.cuh"')
         em('#include "nqb_tp_fused.cuh"')
         em("namespace {")
         em()
-        self.has_fused = self._emit_fused(em)
-        for gid, ps in enumerate(self.fwd_groups):
-            self._emit_fwd_group(em, gid, ps)
-        # the ring pays off when several warps (path groups) share one node's weight rows; single-group
-        # signatures (3-4 paths: first/last layer) keep the register-resident v1 kernel (measured)
-        # (and only while the ring fits: a signature whose ring would exceed ~200 KB keeps the register kernel)
-        ring_bytes = self.opts.ring_stages * self.geometry(2)[1] * sig.weight_numel * 4 + 2 * self.opts.ring_stages * 8 + 256 * 16
-        # ... and only when one edge fills the warp (mul >= 64 -> EPW == 1): with two or more edges per warp iteration the
-        # ring is EPW x larger per CTA (70-140 KB for the l_max = 3 layers -> 1-3 CTAs per SM) and the register kernels
-        # keep more warps resident
-        ring_fits = ring_bytes <= 200 * 1024 and self.geometry(2)[1] == 1
-        self.use_ring = bool(self.opts.fwd_ring and sig.weight_numel % 4 == 0 and len(self.fwd_groups) >= 2 and ring_fits)
-        if self.use_ring:
-            em(f"constexpr int F2_STAGES = {self.opts.ring_stages};")
-            em("constexpr int F2_CAP = 256;")
-            em("__device__ __forceinline__ void cta_sync() { asm volatile(\"bar.sync 1, %0;\" ::\"n\"(32 * NGF) : \"memory\"); }")
-            for gid, ps in enumerate(self.fwd_groups):
-                self._emit_fwd2_group(em, gid, ps)
-        for gid, ps in enumerate(self.bwd_groups):
-            self._emit_bwd_group(em, gid, ps)
-        self.use_ring_bwd = bool(self.opts.bwd_ring and sig.weight_numel % 4 == 0 and len(self.bwd_groups) >= 2 and ring_fits)
-        if self.use_ring_bwd:
-            em(f"constexpr int B2_STAGES = {self.opts.ring_stages};")
-            em("constexpr int B2_CAP = 256;")
-            em("__device__ __forceinline__ void cta_sync_b() { asm volatile(\"bar.sync 1, %0;\" ::\"n\"(32 * NGB) : \"memory\"); }")
-            for gid, ps in enumerate(self.bwd_groups):
-                self._emit_bwd2_group(em, gid, ps)
-        mbf = f", {self.opts.min_blocks_fwd}" if self.opts.min_blocks_fwd else ""
-        mbb = f", {self.opts.min_blocks_bwd}" if self.opts.min_blocks_bwd else ""
+        if self.has_fused:
+            self._emit_fused(em)
+        for bwd in (False, True):
+            for gid, ps in enumerate(self.groups):
+                self._emit_group(em, gid, ps, bwd, ring=False)
+            if self.use_ring_bwd if bwd else self.use_ring:
+                P, NG, sync = _ring_names(bwd)
+                em(f"constexpr int {P}_STAGES = {RING_STAGES};")
+                em(f"constexpr int {P}_CAP = {RING_CAP};")
+                em(f"__device__ __forceinline__ void {sync}() {{ asm volatile(\"bar.sync 1, %0;\" ::\"n\"(32 * {NG}) : \"memory\"); }}")
+                for gid, ps in enumerate(self.groups):
+                    self._emit_group(em, gid, ps, bwd, ring=True)
         # unwritten output chunks (irreps_out entries no instruction writes) must be zero-filled
         unwritten = [io for io in range(len(sig.irreps_out)) if io not in sig.written_outs]
-        # kernels
-        em.block(
-            f"template <typename T> __global__ void __launch_bounds__(32 * NWARP{mbf}) tp_fwd_kernel("
-            "const T* __restrict__ x, const T* __restrict__ y, const T* __restrict__ w, "
-            "const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ perm, "
-            "const int64_t* __restrict__ src, int64_t N, T* __restrict__ out, int grp0)"
-        )
-        em("constexpr int CB = VT<T>::CB, LPE = VT<T>::LPE, CPT = VT<T>::CPT;")
-        em("const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;")
-        em("const int64_t n = (int64_t)blockIdx.x * NWARP + warp;")
-        em("if (n >= N) return;")
-        em("const int grp = grp0 + blockIdx.y / CB, cb = blockIdx.y % CB;")
-        em("const int sub = lane / LPE, cl = lane % LPE;")
-        em("const int ch0 = (cb * LPE + cl) * CPT;")
-        em("const int64_t beg = row_ptr[n], end = row_ptr[n + 1];")
-        em.block("switch (grp)")
-        for gid in range(len(self.fwd_groups)):
-            em(f"case {gid}: fwd_g{gid}<T>(x, y, w, perm, src, n, beg, end, ch0, sub, out); break;")
-        em("default: break;")
-        em.end()
+        self._emit_v1_kernel(em, bwd=False)
         if unwritten:
             em.block("if (grp == 0 && cb == 0)")
             for io in unwritten:
@@ -1026,37 +964,7 @@ class TPGenerator:
         em.end()
         em()
         if self.use_ring:
-            minb = max(1, min(16, 512 // (32 * len(self.fwd_groups))))
-            em.block(
-                f"__global__ void __launch_bounds__(32 * NGF, {minb}) tp_fwd2_kernel("
-                "const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ w, "
-                "const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ perm, "
-                "const int64_t* __restrict__ src, int64_t N, float* __restrict__ out)"
-            )
-            em("extern __shared__ __align__(16) uint8_t f2_smem[];")
-            em("constexpr int LPE = VT<float>::LPE, CPT = VT<float>::CPT, EPW = VT<float>::EPW;")
-            em(f"constexpr size_t RING_FLOATS = (size_t)F2_STAGES * EPW * {sig.weight_numel};")
-            em("float* ring = reinterpret_cast<float*>(f2_smem);")
-            em("uint64_t* full = reinterpret_cast<uint64_t*>(f2_smem + RING_FLOATS * sizeof(float));")
-            em("uint64_t* empty = full + F2_STAGES;")
-            em("int64_t* eids = reinterpret_cast<int64_t*>(empty + F2_STAGES);")
-            em("int64_t* srcs = eids + F2_CAP;")
-            em("const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;")
-            em("const int64_t n = blockIdx.x;")
-            em("const int cb = blockIdx.y;")
-            em("const int sub = lane / LPE, cl = lane % LPE;")
-            em("const int ch0 = (cb * LPE + cl) * CPT;")
-            em("const int64_t beg = row_ptr[n], end = row_ptr[n + 1];")
-            em.block("if (threadIdx.x == 0)")
-            em("for (int s_ = 0; s_ < F2_STAGES; ++s_) { mbar_init(&full[s_], 1); mbar_init(&empty[s_], NGF); }")
-            em("fence_barrier_init();")
-            em.end()
-            em("__syncthreads();")
-            em.block("switch (warp)")
-            for gid in range(len(self.fwd_groups)):
-                em(f"case {gid}: fwd2_g{gid}(x, y, w, perm, src, n, beg, end, ch0, sub, warp, lane, ring, full, empty, eids, srcs, out); break;")
-            em("default: break;")
-            em.end()
+            self._emit_ring_kernel(em, bwd=False)
             if unwritten:
                 em.block("if (blockIdx.y == 0)")
                 for io in unwritten:
@@ -1066,64 +974,10 @@ class TPGenerator:
                 em.end()
             em.end()
             em()
-        em.block(
-            f"template <typename T, bool WANT_GX> __global__ void __launch_bounds__(32 * NWARP{mbb}) tp_bwd_kernel("
-            "const T* __restrict__ x, const T* __restrict__ y, const T* __restrict__ w, "
-            "const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ perm, "
-            "const int64_t* __restrict__ src, const T* __restrict__ gout, int64_t N, "
-            "T* __restrict__ gx, T* __restrict__ gy, T* __restrict__ gw, int det, int64_t gy_slice, int grp0)"
-        )
-        em("constexpr int CB = VT<T>::CB, LPE = VT<T>::LPE, CPT = VT<T>::CPT;")
-        em("const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;")
-        em("const int64_t n = (int64_t)blockIdx.x * NWARP + warp;")
-        em("if (n >= N) return;")
-        em("const int grp = grp0 + blockIdx.y / CB, cb = blockIdx.y % CB;")
-        em("const int sub = lane / LPE, cl = lane % LPE;")
-        em("const int ch0 = (cb * LPE + cl) * CPT;")
-        em("const int64_t beg = row_ptr[n], end = row_ptr[n + 1];")
-        em.block("switch (grp)")
-        for gid in range(len(self.bwd_groups)):
-            em(
-                f"case {gid}: bwd_g{gid}<T, WANT_GX>(x, y, w, perm, src, gout, n, beg, end, ch0, sub, cl, "
-                "gx, gy + (int64_t)(grp * CB + cb) * gy_slice, gw, det != 0); break;"
-            )
-        em("default: break;")
-        em.end()
+        self._emit_v1_kernel(em, bwd=True)
         em.end()
         if self.use_ring_bwd:
-            minb2 = max(1, min(16, 384 // (32 * len(self.bwd_groups))))
-            em.block(
-                f"template <bool WANT_GX> __global__ void __launch_bounds__(32 * NGB, {minb2}) tp_bwd2_kernel("
-                "const float* __restrict__ x, const float* __restrict__ y, const float* __restrict__ w, "
-                "const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ perm, "
-                "const int64_t* __restrict__ src, const float* __restrict__ gout, int64_t N, "
-                "float* __restrict__ gx, float* __restrict__ gy, float* __restrict__ gw, int det, int64_t gy_slice)"
-            )
-            em("extern __shared__ __align__(16) uint8_t b2_smem[];")
-            em("constexpr int LPE = VT<float>::LPE, CPT = VT<float>::CPT, EPW = VT<float>::EPW;")
-            em(f"constexpr size_t RING_FLOATS = (size_t)B2_STAGES * EPW * {sig.weight_numel};")
-            em("float* ring = reinterpret_cast<float*>(b2_smem);")
-            em("uint64_t* full = reinterpret_cast<uint64_t*>(b2_smem + RING_FLOATS * sizeof(float));")
-            em("uint64_t* empty = full + B2_STAGES;")
-            em("int64_t* eids = reinterpret_cast<int64_t*>(empty + B2_STAGES);")
-            em("int64_t* srcs = eids + B2_CAP;")
-            em("const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;")
-            em("const int64_t n = blockIdx.x;")
-            em("const int cb = blockIdx.y;")
-            em("const int sub = lane / LPE, cl = lane % LPE;")
-            em("const int ch0 = (cb * LPE + cl) * CPT;")
-            em("const int64_t beg = row_ptr[n], end = row_ptr[n + 1];")
-            em.block("if (threadIdx.x == 0)")
-            em("for (int s_ = 0; s_ < B2_STAGES; ++s_) { mbar_init(&full[s_], 1); mbar_init(&empty[s_], NGB); }")
-            em("fence_barrier_init();")
-            em.end()
-            em("__syncthreads();")
-            em.block("switch (warp)")
-            for gid in range(len(self.bwd_groups)):
-                em(f"case {gid}: bwd2_g{gid}<WANT_GX>(x, y, w, perm, src, gout, n, beg, end, ch0, sub, cl, warp, lane, "
-                   "ring, full, empty, eids, srcs, gx, gy + (int64_t)(warp * gridDim.y + blockIdx.y) * gy_slice, gw, det != 0); break;")
-            em("default: break;")
-            em.end()
+            self._emit_ring_kernel(em, bwd=True)
             em.end()
         em("}  // namespace")
         em()
@@ -1144,25 +998,17 @@ class TPGenerator:
         em("dim3 block(32 * NWARP);")
         em.block("if (dtype == 0)")
         if self.use_ring:
-            lpe_f2, epw_f2, cb_f2 = self.geometry(2)
-            smem = self.opts.ring_stages * epw_f2 * sig.weight_numel * 4 + 2 * self.opts.ring_stages * 8 + 256 * 16
-            em(f"constexpr int F2_SMEM = {smem};")
-            em("static bool attr_set[64] = {false};  // per device")
-            em("int dev_ = 0; cudaGetDevice(&dev_); dev_ &= 63;")
-            em.block("if (!attr_set[dev_])")
-            em("cudaError_t e_ = cudaFuncSetAttribute(tp_fwd2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, F2_SMEM);")
-            em("if (e_ != cudaSuccess) return (int)e_;")
-            em("attr_set[dev_] = true;")
-            em.end()
+            em(f"constexpr int F2_SMEM = {self.ring_smem_bytes};")
+            _emit_smem_attr(em, ["tp_fwd2_kernel"], "F2_SMEM")
             em("dim3 grid2((unsigned)N, VT<float>::CB), block2(32 * NGF);")
             em("tp_fwd2_kernel<<<grid2, block2, F2_SMEM, st>>>((const float*)x, (const float*)y, (const float*)w, row_ptr, perm, src, N, (float*)out);")
         else:
-            self._emit_v1_launch(em, "NGF", "float", "tp_fwd_kernel<float>",
-                                 "(const float*)x, (const float*)y, (const float*)w, row_ptr, perm, src, N, (float*)out")
+            _emit_v1_launch(em, "NGF", "float", "tp_fwd_kernel<float>",
+                            "(const float*)x, (const float*)y, (const float*)w, row_ptr, perm, src, N, (float*)out")
         em.end()
         em.block("else")
-        self._emit_v1_launch(em, "NGF", "double", "tp_fwd_kernel<double>",
-                             "(const double*)x, (const double*)y, (const double*)w, row_ptr, perm, src, N, (double*)out")
+        _emit_v1_launch(em, "NGF", "double", "tp_fwd_kernel<double>",
+                        "(const double*)x, (const double*)y, (const double*)w, row_ptr, perm, src, N, (double*)out")
         em.end()
         em("return (int)cudaGetLastError();")
         em.end()
@@ -1175,18 +1021,9 @@ class TPGenerator:
         em(f"const int64_t gy_slice = det ? E * {sig.s_dim} : 0;  // deterministic: one grad_Y slice per (path group, channel block)")
         em("dim3 block(32 * NWARP);")
         if self.use_ring_bwd:
-            lpe_f2, epw_f2, cb_f2 = self.geometry(2)
-            smemb = self.opts.ring_stages * epw_f2 * sig.weight_numel * 4 + 2 * self.opts.ring_stages * 8 + 256 * 16
             em.block("if (dtype == 0)")
-            em(f"constexpr int B2_SMEM = {smemb};")
-            em("static bool attr_set[64] = {false};  // per device")
-            em("int dev_ = 0; cudaGetDevice(&dev_); dev_ &= 63;")
-            em.block("if (!attr_set[dev_])")
-            em("cudaError_t e_ = cudaFuncSetAttribute(tp_bwd2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, B2_SMEM);")
-            em("if (e_ == cudaSuccess) e_ = cudaFuncSetAttribute(tp_bwd2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, B2_SMEM);")
-            em("if (e_ != cudaSuccess) return (int)e_;")
-            em("attr_set[dev_] = true;")
-            em.end()
+            em(f"constexpr int B2_SMEM = {self.ring_smem_bytes};")
+            _emit_smem_attr(em, ["tp_bwd2_kernel<true>", "tp_bwd2_kernel<false>"], "B2_SMEM")
             em("dim3 grid2((unsigned)N, VT<float>::CB), block2(32 * NGB);")
             a2 = ("(const float*)x, (const float*)y, (const float*)w, row_ptr, perm, src, (const float*)gout, N, "
                   "(float*)gx, (float*)gy, (float*)gw, det, gy_slice")
@@ -1201,10 +1038,10 @@ class TPGenerator:
                 f"(const {name}*)gout, N, ({name}*)gx, ({name}*)gy, ({name}*)gw, det, gy_slice"
             )
             em.block("if (gx)")
-            self._emit_v1_launch(em, "NGB", name, f"tp_bwd_kernel<{name}, true>", args)
+            _emit_v1_launch(em, "NGB", name, f"tp_bwd_kernel<{name}, true>", args)
             em.end()
             em.block("else")
-            self._emit_v1_launch(em, "NGB", name, f"tp_bwd_kernel<{name}, false>", args)
+            _emit_v1_launch(em, "NGB", name, f"tp_bwd_kernel<{name}, false>", args)
             em.end()
             em.end()
         em("return (int)cudaGetLastError();")
@@ -1229,13 +1066,7 @@ class TPGenerator:
             em("if (N <= 0) return 0;")
             em("if (K <= 0 || K > FT_KMAX || (K % 8) || (ldh % 4) || nctas <= 0) return (int)cudaErrorInvalidValue;")
             em("const size_t smem = ft_smem_bytes<FtSpec>();")
-            em("static bool attr_set[64] = {false};  // per device")
-            em("int dev_ = 0; cudaGetDevice(&dev_); dev_ &= 63;")
-            em.block("if (!attr_set[dev_])")
-            em("cudaError_t e_ = cudaFuncSetAttribute(tp_fused_fwd_kernel<FtSpec>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);")
-            em("if (e_ != cudaSuccess) return (int)e_;")
-            em("attr_set[dev_] = true;")
-            em.end()
+            _emit_smem_attr(em, ["tp_fused_fwd_kernel<FtSpec>"], "(int)smem")
             em("FusedFwdArgs a;")
             em("a.x = x; a.y = y; a.h = h; a.wprep = wprep; a.row_ptr = row_ptr; a.src = src; a.out = out; a.w_out = w_out;")
             em("a.slice_cta0 = slice_cta0; a.N = N; a.E = E; a.ldh = ldh; a.K = K;")

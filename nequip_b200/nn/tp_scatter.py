@@ -20,8 +20,6 @@ find it.  Without nequip the same class stands alone on ``torch.nn.Module``.
 """
 from __future__ import annotations
 
-from typing import Optional
-
 import torch
 
 from .. import ops
@@ -63,7 +61,6 @@ class B200TensorProductScatter(_Base):
         irreps_edge_attr,
         irreps_mid,
         instructions,
-        gen_options: Optional[GenOptions] = None,
         layout: str = "mul_ir",
     ) -> None:
         super().__init__(
@@ -77,9 +74,6 @@ class B200TensorProductScatter(_Base):
         # layout="mul_ir" is the reference's (e3nn) node-feature layout and the drop-in default;
         # "ir_mul" (channel-contiguous, what cuEquivariance uses, nequip/nn/_tp_scatter_cueq.py:107-122)
         # is used between our own kernels
-        import dataclasses
-
-        self._gen_options = dataclasses.replace(gen_options or GenOptions(), layout=layout)
         self.layout = layout
         # the signature is pure host logic; the kernel library is bound on first use, so that constructing a
         # model (e.g. to obtain a state dict for the CPU reference arm of bench.py) loads no native code
@@ -94,7 +88,7 @@ class B200TensorProductScatter(_Base):
     def _plan(self):
         if self._plan_obj is None:
             s = self._sig
-            self._plan_obj = ops.get_plan(s.irreps_in1, s.irreps_in2, s.irreps_out, s.instructions, self._gen_options)
+            self._plan_obj = ops.get_plan(s.irreps_in1, s.irreps_in2, s.irreps_out, s.instructions, GenOptions(layout=self.layout))
         return self._plan_obj
 
     @property
