@@ -107,7 +107,7 @@ int nqb_tp_scatter_gy_slices(const nqb_plan* plan, int dtype);
 int nqb_segment_sum(int dtype, const void* rows /* [R, D] */, int D, const int64_t* perm, const int64_t* seg_ptr /* [N+1] */,
                     int64_t N, void* out /* [N, D] */, nqb_stream_t st);
 
-/* Real spherical harmonics, "component" normalisation, input normalised (lmax <= 3).
+/* Real spherical harmonics, "component" normalisation, input normalised (lmax <= 4).
  *   vec [E,3] f64 -> y [E,(lmax+1)^2] of out_dtype (computed in f64, then cast). */
 int nqb_sh_fwd(int lmax, const double* vec, int64_t E, int out_dtype, void* y, nqb_stream_t st);
 /*   grad_vec [E,3] f64 = J^T grad_y (includes the normalisation Jacobian); overwritten */
@@ -131,7 +131,7 @@ int nqb_tp_fused_fwd(const nqb_plan* plan, const float* x, const float* y, const
                      const float* w2_prepared, const int64_t* row_ptr, const int64_t* src, int64_t N, int64_t E,
                      float* out, float* w_out, const int32_t* slice_cta0, int nctas, nqb_stream_t st);
 
-/* Real spherical harmonics, "component" normalisation, input normalised (lmax <= 3).
+/* Real spherical harmonics, "component" normalisation, input normalised (lmax <= 4).
  *   vec [E,3] f64 -> y [E,(lmax+1)^2] of out_dtype (computed in f64, then cast). */
 int nqb_sh_fwd(int lmax, const double* vec, int64_t E, int out_dtype, void* y, nqb_stream_t st);
 /*   grad_vec [E,3] f64 = J^T grad_y (includes the normalisation Jacobian); overwritten */

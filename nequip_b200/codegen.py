@@ -244,9 +244,9 @@ def _emit_smem_attr(em: _Emitter, kernels: List[str], nbytes: str):
     em.end()
 
 
-def _emit_v1_launch(em: _Emitter, ng: str, tname: str, kernel: str, args: str):
-    """Launch of a register (v1) kernel: all path groups in one grid (blockIdx.y = group, channel block)."""
-    em(f"{{ dim3 grid_((unsigned)((N + NWARP - 1) / NWARP), {ng} * VT<{tname}>::CB); "
+def _emit_v1_launch(em: _Emitter, items: str, kernel: str, args: str):
+    """Launch of a register (v1) kernel: all work items in one grid (blockIdx.y = work item)."""
+    em(f"{{ dim3 grid_((unsigned)((N + NWARP - 1) / NWARP), {items}); "
        f"{kernel}<<<grid_, block, 0, st>>>({args}, 0); }}")
 
 
@@ -300,6 +300,12 @@ class TPGenerator:
         self.opts = opts or GenOptions()
         self.mul_max = max(p.mul for p in sig.paths)
         self.groups = _partition(sig, ACC_CAP)  # the same path groups in the forward and the backward
+        # work items (path group, channel block) per node.  When fp32 has one channel block and every group needs
+        # all fp64 channel blocks (every signature with a single multiplicity <= 64), the work items are
+        # (group, block) in row-major order and the kernels decode blockIdx.y arithmetically, with no table
+        self.items_f, self.items_d = self.work_items("float32"), self.work_items("float64")
+        self.one_block = (self.geometry(2)[2] == 1
+                          and len(self.items_d) == len(self.groups) * self.geometry(1)[2])
         # dynamic shared memory of a ring kernel: weight ring + its full/empty mbarriers + staged edge and source ids
         epw = self.geometry(2)[1]
         self.ring_smem_bytes = RING_STAGES * epw * sig.weight_numel * 4 + 2 * RING_STAGES * 8 + RING_CAP * 16
@@ -309,10 +315,12 @@ class TPGenerator:
         # ... and only when one edge fills the warp (mul >= 64 -> EPW == 1): with two or more edges per warp iteration the
         # ring is EPW x larger per CTA (70-140 KB for the l_max = 3 layers -> 1-3 CTAs per SM) and the register kernels
         # keep more warps resident
+        # (one warp per fp32 work item: the CTA must stay within 1024 threads)
         self.use_ring = (sig.weight_numel % 4 == 0 and len(self.groups) >= 2 and epw == 1
-                         and self.ring_smem_bytes <= 200 * 1024)
+                         and self.ring_smem_bytes <= 200 * 1024 and 32 * len(self.items_f) <= 1024)
         self.use_ring_bwd = self.use_ring  # same groups, same ring: both directions make the same choice
         self.has_fused = self.fused_layout() is not None
+        self._gmul = ""  # extra template argument of the channel accesses of the group being emitted
 
     def out_ir_mul(self, io: int):
         """ir_mul placement of output chunk ``io``: the layout is defined over
@@ -338,6 +346,24 @@ class TPGenerator:
         epw = 32 // lpe
         cb = (pairs + lpe - 1) // lpe
         return lpe, epw, cb
+
+    def work_items(self, dtype) -> List[Tuple[int, int]]:
+        """(path group, channel block) pairs of one node in kernel order, for ``dtype`` "float32" or "float64" (or
+        the torch dtype).  Lanes per edge come from the largest multiplicity of the signature, but each group gets
+        only the channel blocks its own largest multiplicity needs, so every work item owns at least one channel."""
+        cpt = {"float32": 2, "float64": 1}[str(dtype).replace("torch.", "")]
+        lpe = self.geometry(cpt)[0]
+        items = []
+        for g, ps in enumerate(self.groups):
+            pairs = (max(p.mul for p in ps) + cpt - 1) // cpt
+            items += [(g, cb) for cb in range((pairs + lpe - 1) // lpe)]
+        return items
+
+    def _items_expr(self, tname: str, bwd: bool) -> str:
+        """Number of work items per node of the register kernels, as a source expression."""
+        if self.one_block:
+            return f"{'NGB' if bwd else 'NGF'} * VT<{tname}>::CB"
+        return "NWI_F" if tname == "float" else "NWI_D"
 
     # -- per-group helpers ------------------------------------------------------
     @staticmethod
@@ -376,9 +402,9 @@ class TPGenerator:
                 off, stride = irr.offsets()[c], mul
                 al = _aligned(width, off, mul)
             em(f"{ptr} = {base} + {row} * {width} + {off} + ch0;")
-            return f"{mul}, {al}", stride
+            return f"{mul}, {al}{self._gmul}", stride
         em(f"{ptr} = {base} + {row} * {width} + {irr.offsets()[c]} + (int64_t)ch0 * {ir.dim};")
-        return f"{ir.dim}, {mul}", 1
+        return f"{ir.dim}, {mul}{self._gmul}", 1
 
     def _emit_yx_loads(self, em: _Emitter, paths: List[Path], sfx: str, decl: str):
         """Load the harmonics of edge ``e{sfx}`` and gather the x row of its source ``sn{sfx}`` into ``y{j}{sfx}`` and
@@ -409,7 +435,7 @@ class TPGenerator:
         zero = f"valid{sfx}" if mask_w else "true"
         em.block()
         for p in paths:
-            em(f"w{p.idx}{sfx} = vloadw<{p.mul}, {_aligned(W, p.woff)}>(w + e{sfx} * {W} + {p.woff} + ch0, ch0, {zero});")
+            em(f"w{p.idx}{sfx} = vloadw<{p.mul}, {_aligned(W, p.woff)}{self._gmul}>(w + e{sfx} * {W} + {p.woff} + ch0, ch0, {zero});")
         self._emit_yx_loads(em, paths, sfx, "")
         em.end()
 
@@ -487,7 +513,7 @@ class TPGenerator:
         em(f"mbar_wait(&full[st], (gi / {P}_STAGES) & 1);")
         em(f"const float* wrow = ring + (size_t)(st * EPW + (valid ? sub : 0)) * {W};")
         for p in paths:
-            em(f"const V w{p.idx} = vloadws<{p.mul}, {_aligned(W, p.woff)}>(wrow + {p.woff} + ch0, ch0, {'valid' if mask_w else 'true'});")
+            em(f"const V w{p.idx} = vloadws<{p.mul}, {_aligned(W, p.woff)}{self._gmul}>(wrow + {p.woff} + ch0, ch0, {'valid' if mask_w else 'true'});")
         em("__syncwarp();")
         em("if (lane == 0) mbar_arrive(&empty[st]);")
         em.block()
@@ -512,6 +538,8 @@ class TPGenerator:
         args += ([f"{T}* __restrict__ gx", f"{T}* __restrict__ gy", f"{T}* __restrict__ gw", "bool det"] if bwd
                  else [f"{T}* __restrict__ out"])
         name = ("bwd" if bwd else "fwd") + ("2" if ring else "") + f"_g{gid}"
+        # channel accesses are masked only past the blocks this group's work items cover (vfull, nqb_tp_device.cuh)
+        self._gmul = "" if self.one_block else f", {max(p.mul for p in paths)}"
         em.block((f"template <{', '.join(tparams)}> " if tparams else "")
                  + f"__device__ __forceinline__ void {name}(" + ", ".join(args) + ")")
         if ring:
@@ -632,7 +660,7 @@ class TPGenerator:
                     for k in range(1, n1):
                         em(f"r{p.idx} = vfma(x{i1}_{k}, g{p.io}_{k}, r{p.idx});")
                     em(f"const V ky{p.idx} = vmuli(y{yoff}, {_imm(kappa)});")
-                    em(f"if (valid) vstorew<{p.mul}, {_aligned(W, p.woff)}>(gw + e * {W} + {p.woff} + ch0, vmul(ky{p.idx}, r{p.idx}), ch0);")
+                    em(f"if (valid) vstorew<{p.mul}, {_aligned(W, p.woff)}{self._gmul}>(gw + e * {W} + {p.woff} + ch0, vmul(ky{p.idx}, r{p.idx}), ch0);")
                     em(f"q{yoff} = vfma(vmuli(w{p.idx}, {_imm(kappa)}), r{p.idx}, q{yoff});")
                     em.block("if (WANT_GX)")
                     em(f"const V ws = vmul(w{p.idx}, ky{p.idx});")
@@ -675,7 +703,7 @@ class TPGenerator:
                     em(f"V r{p.idx} = vmul(g{p.io}_{ks[0]}, v{p.idx}_{ks[0]});")
                     for k in ks[1:]:
                         em(f"r{p.idx} = vfma(g{p.io}_{k}, v{p.idx}_{k}, r{p.idx});")
-                    em(f"if (valid) vstorew<{p.mul}, {_aligned(W, p.woff)}>(gw + e * {W} + {p.woff} + ch0, r{p.idx}, ch0);")
+                    em(f"if (valid) vstorew<{p.mul}, {_aligned(W, p.woff)}{self._gmul}>(gw + e * {W} + {p.woff} + ch0, r{p.idx}, ch0);")
             em.end()
         # grad_x: atomics into the source row -- or, in deterministic mode, plain stores into the EDGE's own row of a
         # [E, D_in] buffer that nqb_segment_sum reduces over the (source-sorted) edges in a fixed order
@@ -743,6 +771,8 @@ class TPGenerator:
             return None
         if sorted(p.io for p in sig.paths) != list(range(len(sig.irreps_out))):
             return None  # every output chunk must be written by exactly one path
+        if max(p.l3 for p in sig.paths) > 3:
+            return None  # the kernel's per-path accumulators hold 2 l3 + 1 <= FT_N3MAX = 7 components
         pps = 128 // mul
         by_i1: Dict[int, List[Path]] = {}
         for p in sig.paths:
@@ -857,29 +887,33 @@ class TPGenerator:
         em("const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;")
         em("const int64_t n = (int64_t)blockIdx.x * NWARP + warp;")
         em("if (n >= N) return;")
-        em("const int grp = grp0 + blockIdx.y / CB, cb = blockIdx.y % CB;")
+        if self.one_block:
+            em("const int grp = grp0 + blockIdx.y / CB, cb = blockIdx.y % CB;")
+        else:
+            em("const int wi = (sizeof(T) == 4 ? WI_F : WI_D)[blockIdx.y], grp = wi >> 8, cb = wi & 255;")
         em("const int sub = lane / LPE, cl = lane % LPE;")
         em("const int ch0 = (cb * LPE + cl) * CPT;")
         em("const int64_t beg = row_ptr[n], end = row_ptr[n + 1];")
         if bwd:
+            slice_ = "grp * CB + cb" if self.one_block else "blockIdx.y"
             calls = [f"bwd_g{g}<T, WANT_GX>(x, y, w, perm, src, gout, n, beg, end, ch0, sub, cl, "
-                     "gx, gy + (int64_t)(grp * CB + cb) * gy_slice, gw, det != 0)" for g in range(len(self.groups))]
+                     f"gx, gy + (int64_t)({slice_}) * gy_slice, gw, det != 0)" for g in range(len(self.groups))]
         else:
             calls = [f"fwd_g{g}<T>(x, y, w, perm, src, n, beg, end, ch0, sub, out)" for g in range(len(self.groups))]
         _emit_switch(em, "grp", calls)
 
     def _emit_ring_kernel(self, em: _Emitter, bwd: bool):
-        """Ring form: one CTA per (node, channel block), one warp per path group; carves the dynamic shared memory
+        """Ring form: one CTA per node, one warp per fp32 work item; carves the dynamic shared memory
         (weight ring, full/empty mbarriers, staged edge and source ids), initialises the barriers and dispatches the
         warps to their groups; opens the kernel body."""
         P, NG, _ = _ring_names(bwd)
         smem = P.lower() + "_smem"
         if bwd:
-            minb = max(1, min(16, 384 // (32 * len(self.groups))))
+            minb = max(1, min(16, 384 // (32 * len(self.items_f))))
             em.block(f"template <bool WANT_GX> __global__ void __launch_bounds__(32 * NGB, {minb}) tp_bwd2_kernel("
                      + self._kernel_params("float", bwd) + ")")
         else:
-            minb = max(1, min(16, 512 // (32 * len(self.groups))))
+            minb = max(1, min(16, 512 // (32 * len(self.items_f))))
             em.block(f"__global__ void __launch_bounds__(32 * NGF, {minb}) tp_fwd2_kernel(" + self._kernel_params("float", bwd) + ")")
         em(f"extern __shared__ __align__(16) uint8_t {smem}[];")
         em("constexpr int LPE = VT<float>::LPE, CPT = VT<float>::CPT, EPW = VT<float>::EPW;")
@@ -891,7 +925,10 @@ class TPGenerator:
         em(f"int64_t* srcs = eids + {P}_CAP;")
         em("const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;")
         em("const int64_t n = blockIdx.x;")
-        em("const int cb = blockIdx.y;")
+        if self.one_block:
+            em("const int cb = blockIdx.y;")
+        else:
+            em("const int wi = WI_F[warp], grp = wi >> 8, cb = wi & 255;")
         em("const int sub = lane / LPE, cl = lane % LPE;")
         em("const int ch0 = (cb * LPE + cl) * CPT;")
         em("const int64_t beg = row_ptr[n], end = row_ptr[n + 1];")
@@ -901,13 +938,14 @@ class TPGenerator:
         em.end()
         em("__syncthreads();")
         if bwd:
+            slice_ = "warp * gridDim.y + blockIdx.y" if self.one_block else "warp"
             calls = [f"bwd2_g{g}<WANT_GX>(x, y, w, perm, src, gout, n, beg, end, ch0, sub, cl, warp, lane, "
-                     "ring, full, empty, eids, srcs, gx, gy + (int64_t)(warp * gridDim.y + blockIdx.y) * gy_slice, gw, det != 0)"
+                     f"ring, full, empty, eids, srcs, gx, gy + (int64_t)({slice_}) * gy_slice, gw, det != 0)"
                      for g in range(len(self.groups))]
         else:
             calls = [f"fwd2_g{g}(x, y, w, perm, src, n, beg, end, ch0, sub, warp, lane, ring, full, empty, eids, srcs, out)"
                      for g in range(len(self.groups))]
-        _emit_switch(em, "warp", calls)
+        _emit_switch(em, "warp" if self.one_block else "grp", calls)
 
     # -- translation unit ----------------------------------------------------------------
     def source(self) -> str:
@@ -918,6 +956,8 @@ class TPGenerator:
         em(f"// AUTO-GENERATED by nequip_b200/codegen.py (v{CODEGEN_VERSION}) -- do not edit.")
         em(f"// signature: {sig.canonical()}")
         em(f"// layout: {self.opts.layout}  path_groups={len(self.groups)}  ring={int(self.use_ring)}")
+        if not self.one_block:
+            em(f"// work items (path group, channel block): fp32 {self.items_f}, fp64 {self.items_d}")
         em(f"// forward multiply-accumulates per (edge, channel): {sig.fma_count()}")
         em("#include <cuda_runtime.h>")
         em('#include "nqb_tc.cuh"')
@@ -932,8 +972,13 @@ class TPGenerator:
             f"template <> struct VT<double> {{ typedef double V; static constexpr int CPT = 1, LPE = {lpe_d}, "
             f"EPW = {epw_d}, CB = {cb_d}; }};"
         )
-        em(f"constexpr int NGF = {len(self.groups)};")
-        em(f"constexpr int NGB = {len(self.groups)};")
+        # warps of a ring CTA (one per fp32 work item); with one channel block these are the path groups
+        em(f"constexpr int NGF = {len(self.items_f)};")
+        em(f"constexpr int NGB = {len(self.items_f)};")
+        if not self.one_block:
+            em(f"constexpr int NWI_F = {len(self.items_f)}, NWI_D = {len(self.items_d)};  // work items per node")
+            for nm, items in (("WI_F", self.items_f), ("WI_D", self.items_d)):
+                em(f"__constant__ int {nm}[] = {{{', '.join(str(g << 8 | cb) for g, cb in items)}}};  // group << 8 | channel block")
         em("}  // namespace")
         em('#include "nqb_tp_device.cuh"')
         em('#include "nqb_tp_fused.cuh"')
@@ -1000,14 +1045,15 @@ class TPGenerator:
         if self.use_ring:
             em(f"constexpr int F2_SMEM = {self.ring_smem_bytes};")
             _emit_smem_attr(em, ["tp_fwd2_kernel"], "F2_SMEM")
-            em("dim3 grid2((unsigned)N, VT<float>::CB), block2(32 * NGF);")
+            em("dim3 grid2((unsigned)N, VT<float>::CB), block2(32 * NGF);" if self.one_block
+               else "dim3 grid2((unsigned)N), block2(32 * NGF);")
             em("tp_fwd2_kernel<<<grid2, block2, F2_SMEM, st>>>((const float*)x, (const float*)y, (const float*)w, row_ptr, perm, src, N, (float*)out);")
         else:
-            _emit_v1_launch(em, "NGF", "float", "tp_fwd_kernel<float>",
+            _emit_v1_launch(em, self._items_expr("float", False), "tp_fwd_kernel<float>",
                             "(const float*)x, (const float*)y, (const float*)w, row_ptr, perm, src, N, (float*)out")
         em.end()
         em.block("else")
-        _emit_v1_launch(em, "NGF", "double", "tp_fwd_kernel<double>",
+        _emit_v1_launch(em, self._items_expr("double", False), "tp_fwd_kernel<double>",
                         "(const double*)x, (const double*)y, (const double*)w, row_ptr, perm, src, N, (double*)out")
         em.end()
         em("return (int)cudaGetLastError();")
@@ -1024,7 +1070,8 @@ class TPGenerator:
             em.block("if (dtype == 0)")
             em(f"constexpr int B2_SMEM = {self.ring_smem_bytes};")
             _emit_smem_attr(em, ["tp_bwd2_kernel<true>", "tp_bwd2_kernel<false>"], "B2_SMEM")
-            em("dim3 grid2((unsigned)N, VT<float>::CB), block2(32 * NGB);")
+            em("dim3 grid2((unsigned)N, VT<float>::CB), block2(32 * NGB);" if self.one_block
+               else "dim3 grid2((unsigned)N), block2(32 * NGB);")
             a2 = ("(const float*)x, (const float*)y, (const float*)w, row_ptr, perm, src, (const float*)gout, N, "
                   "(float*)gx, (float*)gy, (float*)gw, det, gy_slice")
             em(f"if (gx) tp_bwd2_kernel<true><<<grid2, block2, B2_SMEM, st>>>({a2});")
@@ -1038,19 +1085,22 @@ class TPGenerator:
                 f"(const {name}*)gout, N, ({name}*)gx, ({name}*)gy, ({name}*)gw, det, gy_slice"
             )
             em.block("if (gx)")
-            _emit_v1_launch(em, "NGB", name, f"tp_bwd_kernel<{name}, true>", args)
+            _emit_v1_launch(em, self._items_expr(name, True), f"tp_bwd_kernel<{name}, true>", args)
             em.end()
             em.block("else")
-            _emit_v1_launch(em, "NGB", name, f"tp_bwd_kernel<{name}, false>", args)
+            _emit_v1_launch(em, self._items_expr(name, True), f"tp_bwd_kernel<{name}, false>", args)
             em.end()
             em.end()
         em("return (int)cudaGetLastError();")
         em.end()
-        # deterministic mode: number of grad_Y slices (one per (path group, channel block) writer)
+        # deterministic mode: number of grad_Y slices (one per work item)
         em.block('extern "C" int nqb_spec_gy_slices(int dtype)')
-        if self.use_ring_bwd:
-            em("if (dtype == 0) return NGB * VT<float>::CB;")
-        em("return dtype == 0 ? NGB * VT<float>::CB : NGB * VT<double>::CB;")
+        if not self.one_block:
+            em("return dtype == 0 ? NWI_F : NWI_D;")
+        else:
+            if self.use_ring_bwd:
+                em("if (dtype == 0) return NGB * VT<float>::CB;")
+            em("return dtype == 0 ? NGB * VT<float>::CB : NGB * VT<double>::CB;")
         em.end()
         # fused radial-MLP last layer + TP + scatter forward (SURVEY section 8f-1); -1 = not built for this signature
         em.block('extern "C" int nqb_spec_fused_info(int* nslice, int* nxs, int* xrow)')

@@ -316,9 +316,17 @@ extern "C" int nqb_csr_from_sorted(const int64_t* sorted_keys, int64_t E, int64_
 }
 
 // ------------------------------------------------------------------------------------------
-// spherical harmonics (lmax <= 3), y is the polar axis, m = -l..l, component normalisation
+// spherical harmonics (lmax <= 4), y is the polar axis, m = -l..l, component normalisation
 // ------------------------------------------------------------------------------------------
-#define NQB_MAX_S 16
+#define NQB_MAX_S 25
+
+// degree 4: the block Y_4 = c * C^{4,1,3} : (Y_1, Y_3) of the w3j recursion (SURVEY App. A.3, oracle/sh.py
+// sh_recurrence), multiplied out into quartic polynomials of the unit vector.  Coefficients:
+//   a4 = 3 sqrt(35) / 2, b4 = 3 sqrt(70) / 4, c4 = 3 sqrt(5) / 2, d4 = 3 sqrt(10) / 4, e4 = 3 sqrt(5) / 4,
+//   f4 = 3 sqrt(35) / 8
+#define NQB_SH4_CONSTS                                                                                  \
+  const double a4 = 8.874119674649425, b4 = 6.274950199005566, c4 = 3.3541019662496847;               \
+  const double d4 = 2.3717082451262845, e4 = 1.6770509831248424, f4 = 2.218529918662356;
 
 template <int LMAX>
 __device__ __forceinline__ void sh_eval(double x, double y, double z, double* Y) {
@@ -349,6 +357,19 @@ __device__ __forceinline__ void sh_eval(double x, double y, double z, double* Y)
     Y[13] = b3 * z * (4.0 * y2 - x2 - z2);
     Y[14] = 0.5 * s105 * y * (z2 - x2);
     Y[15] = a3 * z * (z2 - 3.0 * x2);
+  }
+  if (LMAX >= 4) {
+    NQB_SH4_CONSTS
+    const double x2 = x * x, y2 = y * y, z2 = z * z;
+    Y[16] = a4 * x * z * (z2 - x2);
+    Y[17] = b4 * x * y * (3.0 * z2 - x2);
+    Y[18] = c4 * x * z * (6.0 * y2 - x2 - z2);
+    Y[19] = d4 * x * y * (4.0 * y2 - 3.0 * x2 - 3.0 * z2);
+    Y[20] = 0.375 * (3.0 * x2 * x2 - 24.0 * x2 * y2 + 6.0 * x2 * z2 + 8.0 * y2 * y2 - 24.0 * y2 * z2 + 3.0 * z2 * z2);
+    Y[21] = d4 * y * z * (4.0 * y2 - 3.0 * x2 - 3.0 * z2);
+    Y[22] = e4 * (x2 - z2) * (x2 - 6.0 * y2 + z2);
+    Y[23] = b4 * y * z * (z2 - 3.0 * x2);
+    Y[24] = f4 * (x2 * x2 - 6.0 * x2 * z2 + z2 * z2);
   }
 }
 
@@ -385,6 +406,22 @@ __device__ __forceinline__ void sh_vjp(double x, double y, double z, const doubl
     Gz += g[9] * a3 * 6.0 * x * z + g[10] * s105 * x * y + g[11] * b3 * (-2.0 * x * z) + g[12] * c3 * (-6.0 * y * z)
         + g[13] * b3 * (4.0 * y2 - x2 - 3.0 * z2) + g[14] * 0.5 * s105 * 2.0 * y * z + g[15] * a3 * (3.0 * z2 - 3.0 * x2);
     D += 3.0 * (g[9] * Y[9] + g[10] * Y[10] + g[11] * Y[11] + g[12] * Y[12] + g[13] * Y[13] + g[14] * Y[14] + g[15] * Y[15]);
+  }
+  if (LMAX >= 4) {
+    NQB_SH4_CONSTS
+    const double x2 = x * x, y2 = y * y, z2 = z * z, xyz = x * y * z;
+    Gx += g[16] * a4 * z * (z2 - 3.0 * x2) + g[17] * 3.0 * b4 * y * (z2 - x2) + g[18] * c4 * z * (6.0 * y2 - 3.0 * x2 - z2)
+        + g[19] * d4 * y * (4.0 * y2 - 9.0 * x2 - 3.0 * z2) + g[20] * 4.5 * x * (x2 - 4.0 * y2 + z2)
+        - g[21] * 6.0 * d4 * xyz + g[22] * 4.0 * e4 * x * (x2 - 3.0 * y2) - g[23] * 6.0 * b4 * xyz
+        + g[24] * 4.0 * f4 * x * (x2 - 3.0 * z2);
+    Gy += g[17] * b4 * x * (3.0 * z2 - x2) + g[18] * 12.0 * c4 * xyz + g[19] * 3.0 * d4 * x * (4.0 * y2 - x2 - z2)
+        + g[20] * 6.0 * y * (2.0 * y2 - 3.0 * x2 - 3.0 * z2) + g[21] * 3.0 * d4 * z * (4.0 * y2 - x2 - z2)
+        - g[22] * 12.0 * e4 * y * (x2 - z2) + g[23] * b4 * z * (z2 - 3.0 * x2);
+    Gz += g[16] * a4 * x * (3.0 * z2 - x2) + g[17] * 6.0 * b4 * xyz + g[18] * c4 * x * (6.0 * y2 - x2 - 3.0 * z2)
+        - g[19] * 6.0 * d4 * xyz + g[20] * 4.5 * z * (x2 - 4.0 * y2 + z2) + g[21] * d4 * y * (4.0 * y2 - 3.0 * x2 - 9.0 * z2)
+        + g[22] * 4.0 * e4 * z * (3.0 * y2 - z2) + g[23] * 3.0 * b4 * y * (z2 - x2) + g[24] * 4.0 * f4 * z * (z2 - 3.0 * x2);
+    D += 4.0 * (g[16] * Y[16] + g[17] * Y[17] + g[18] * Y[18] + g[19] * Y[19] + g[20] * Y[20] + g[21] * Y[21]
+                + g[22] * Y[22] + g[23] * Y[23] + g[24] * Y[24]);
   }
 }
 
@@ -425,7 +462,7 @@ __global__ void k_sh_bwd(const double* __restrict__ vec, int64_t E, const TO* __
 }
 
 extern "C" int nqb_sh_fwd(int lmax, const double* vec, int64_t E, int out_dtype, void* y, nqb_stream_t st) {
-  if (lmax < 0 || lmax > 3) return fail("nqb_sh_fwd: lmax=%d unsupported (0..3)", lmax);
+  if (lmax < 0 || lmax > 4) return fail("nqb_sh_fwd: lmax=%d unsupported (0..4)", lmax);
   if (out_dtype != NQB_F32 && out_dtype != NQB_F64) return fail("nqb_sh_fwd: bad dtype");
   if (E < 0) return fail("nqb_sh_fwd: negative size");
   if (E == 0) return 0;
@@ -437,14 +474,16 @@ extern "C" int nqb_sh_fwd(int lmax, const double* vec, int64_t E, int out_dtype,
       case 0: k_sh_fwd<0, float><<<blocks, 128, 0, s>>>(vec, E, (float*)y); break;
       case 1: k_sh_fwd<1, float><<<blocks, 128, 0, s>>>(vec, E, (float*)y); break;
       case 2: k_sh_fwd<2, float><<<blocks, 128, 0, s>>>(vec, E, (float*)y); break;
-      default: k_sh_fwd<3, float><<<blocks, 128, 0, s>>>(vec, E, (float*)y); break;
+      case 3: k_sh_fwd<3, float><<<blocks, 128, 0, s>>>(vec, E, (float*)y); break;
+      default: k_sh_fwd<4, float><<<blocks, 128, 0, s>>>(vec, E, (float*)y); break;
     }
   } else {
     switch (lmax) {
       case 0: k_sh_fwd<0, double><<<blocks, 128, 0, s>>>(vec, E, (double*)y); break;
       case 1: k_sh_fwd<1, double><<<blocks, 128, 0, s>>>(vec, E, (double*)y); break;
       case 2: k_sh_fwd<2, double><<<blocks, 128, 0, s>>>(vec, E, (double*)y); break;
-      default: k_sh_fwd<3, double><<<blocks, 128, 0, s>>>(vec, E, (double*)y); break;
+      case 3: k_sh_fwd<3, double><<<blocks, 128, 0, s>>>(vec, E, (double*)y); break;
+      default: k_sh_fwd<4, double><<<blocks, 128, 0, s>>>(vec, E, (double*)y); break;
     }
   }
   NQB_LAUNCH_CHECK("nqb_sh_fwd");
@@ -453,7 +492,7 @@ extern "C" int nqb_sh_fwd(int lmax, const double* vec, int64_t E, int out_dtype,
 
 extern "C" int nqb_sh_bwd(int lmax, const double* vec, int64_t E, int out_dtype, const void* grad_y,
                           double* grad_vec, nqb_stream_t st) {
-  if (lmax < 0 || lmax > 3) return fail("nqb_sh_bwd: lmax=%d unsupported (0..3)", lmax);
+  if (lmax < 0 || lmax > 4) return fail("nqb_sh_bwd: lmax=%d unsupported (0..4)", lmax);
   if (out_dtype != NQB_F32 && out_dtype != NQB_F64) return fail("nqb_sh_bwd: bad dtype");
   if (E < 0) return fail("nqb_sh_bwd: negative size");
   if (E == 0) return 0;
@@ -465,14 +504,16 @@ extern "C" int nqb_sh_bwd(int lmax, const double* vec, int64_t E, int out_dtype,
       case 0: k_sh_bwd<0, float><<<blocks, 128, 0, s>>>(vec, E, (const float*)grad_y, grad_vec); break;
       case 1: k_sh_bwd<1, float><<<blocks, 128, 0, s>>>(vec, E, (const float*)grad_y, grad_vec); break;
       case 2: k_sh_bwd<2, float><<<blocks, 128, 0, s>>>(vec, E, (const float*)grad_y, grad_vec); break;
-      default: k_sh_bwd<3, float><<<blocks, 128, 0, s>>>(vec, E, (const float*)grad_y, grad_vec); break;
+      case 3: k_sh_bwd<3, float><<<blocks, 128, 0, s>>>(vec, E, (const float*)grad_y, grad_vec); break;
+      default: k_sh_bwd<4, float><<<blocks, 128, 0, s>>>(vec, E, (const float*)grad_y, grad_vec); break;
     }
   } else {
     switch (lmax) {
       case 0: k_sh_bwd<0, double><<<blocks, 128, 0, s>>>(vec, E, (const double*)grad_y, grad_vec); break;
       case 1: k_sh_bwd<1, double><<<blocks, 128, 0, s>>>(vec, E, (const double*)grad_y, grad_vec); break;
       case 2: k_sh_bwd<2, double><<<blocks, 128, 0, s>>>(vec, E, (const double*)grad_y, grad_vec); break;
-      default: k_sh_bwd<3, double><<<blocks, 128, 0, s>>>(vec, E, (const double*)grad_y, grad_vec); break;
+      case 3: k_sh_bwd<3, double><<<blocks, 128, 0, s>>>(vec, E, (const double*)grad_y, grad_vec); break;
+      default: k_sh_bwd<4, double><<<blocks, 128, 0, s>>>(vec, E, (const double*)grad_y, grad_vec); break;
     }
   }
   NQB_LAUNCH_CHECK("nqb_sh_bwd");
@@ -591,7 +632,7 @@ extern "C" int nqb_edge_embed_fwd(int lmax, int num_bessel, double r_max, double
                                   const double* cell, int64_t N, int64_t E, int out_dtype, double* vec, void* y,
                                   void* emb, nqb_stream_t st) {
   (void)N;
-  if (lmax < 0 || lmax > 3) return fail("nqb_edge_embed_fwd: lmax=%d unsupported (0..3)", lmax);
+  if (lmax < 0 || lmax > 4) return fail("nqb_edge_embed_fwd: lmax=%d unsupported (0..4)", lmax);
   if (num_bessel < 1 || num_bessel > NQB_MAX_BESSEL) return fail("nqb_edge_embed_fwd: bad num_bessel %d", num_bessel);
   if (out_dtype != NQB_F32 && out_dtype != NQB_F64) return fail("nqb_edge_embed_fwd: bad dtype");
   if (!(r_max > 0.0) || !(poly_p >= 2.0)) return fail("nqb_edge_embed_fwd: need r_max > 0 and p >= 2");
@@ -604,9 +645,9 @@ extern "C" int nqb_edge_embed_fwd(int lmax, int num_bessel, double r_max, double
   cudaStream_t s = (cudaStream_t)st;
 #define EE_FWD(L, TT) k_edge_embed_fwd<L, TT><<<blocks, 128, 0, s>>>(prm, pos, edge_index, shift, cell, E, vec, (TT*)y, (TT*)emb)
   if (out_dtype == NQB_F32) {
-    switch (lmax) { case 0: EE_FWD(0, float); break; case 1: EE_FWD(1, float); break; case 2: EE_FWD(2, float); break; default: EE_FWD(3, float); break; }
+    switch (lmax) { case 0: EE_FWD(0, float); break; case 1: EE_FWD(1, float); break; case 2: EE_FWD(2, float); break; case 3: EE_FWD(3, float); break; default: EE_FWD(4, float); break; }
   } else {
-    switch (lmax) { case 0: EE_FWD(0, double); break; case 1: EE_FWD(1, double); break; case 2: EE_FWD(2, double); break; default: EE_FWD(3, double); break; }
+    switch (lmax) { case 0: EE_FWD(0, double); break; case 1: EE_FWD(1, double); break; case 2: EE_FWD(2, double); break; case 3: EE_FWD(3, double); break; default: EE_FWD(4, double); break; }
   }
 #undef EE_FWD
   NQB_LAUNCH_CHECK("nqb_edge_embed_fwd");
@@ -618,7 +659,7 @@ extern "C" int nqb_edge_embed_bwd(int lmax, int num_bessel, double r_max, double
                                   int out_dtype, const void* grad_y, const void* grad_emb, double* grad_pos,
                                   double* grad_vec, nqb_stream_t st) {
   (void)N;
-  if (lmax < 0 || lmax > 3) return fail("nqb_edge_embed_bwd: lmax=%d unsupported (0..3)", lmax);
+  if (lmax < 0 || lmax > 4) return fail("nqb_edge_embed_bwd: lmax=%d unsupported (0..4)", lmax);
   if (num_bessel < 1 || num_bessel > NQB_MAX_BESSEL) return fail("nqb_edge_embed_bwd: bad num_bessel %d", num_bessel);
   if (out_dtype != NQB_F32 && out_dtype != NQB_F64) return fail("nqb_edge_embed_bwd: bad dtype");
   if (E < 0) return fail("nqb_edge_embed_bwd: negative size");
@@ -630,9 +671,9 @@ extern "C" int nqb_edge_embed_bwd(int lmax, int num_bessel, double r_max, double
   cudaStream_t s = (cudaStream_t)st;
 #define EE_BWD(L, TT) k_edge_embed_bwd<L, TT><<<blocks, 128, 0, s>>>(prm, vec, edge_index, E, (const TT*)grad_y, (const TT*)grad_emb, grad_pos, grad_vec)
   if (out_dtype == NQB_F32) {
-    switch (lmax) { case 0: EE_BWD(0, float); break; case 1: EE_BWD(1, float); break; case 2: EE_BWD(2, float); break; default: EE_BWD(3, float); break; }
+    switch (lmax) { case 0: EE_BWD(0, float); break; case 1: EE_BWD(1, float); break; case 2: EE_BWD(2, float); break; case 3: EE_BWD(3, float); break; default: EE_BWD(4, float); break; }
   } else {
-    switch (lmax) { case 0: EE_BWD(0, double); break; case 1: EE_BWD(1, double); break; case 2: EE_BWD(2, double); break; default: EE_BWD(3, double); break; }
+    switch (lmax) { case 0: EE_BWD(0, double); break; case 1: EE_BWD(1, double); break; case 2: EE_BWD(2, double); break; case 3: EE_BWD(3, double); break; default: EE_BWD(4, double); break; }
   }
 #undef EE_BWD
   NQB_LAUNCH_CHECK("nqb_edge_embed_bwd");

@@ -30,50 +30,59 @@ __device__ __forceinline__ double vfmai(double a, double c, double b) { return f
 __device__ __forceinline__ float vhsum(float2 a) { return a.x + a.y; }
 __device__ __forceinline__ double vhsum(double a) { return a; }
 
+// A chunk of MUL channels is "full" when no lane's channels fall past its end: MUL fills whole channel blocks and
+// reaches every channel block its path group is given.  GMUL is the group's largest multiplicity (its work items
+// cover ceil(GMUL / block) blocks); 0 stands for every channel block of the signature.  Accesses to a chunk that is
+// not full are masked per channel.
+template <typename T, int MUL, int GMUL = 0> __device__ constexpr bool vfull() {
+  constexpr int B = VT<T>::LPE * VT<T>::CPT;
+  return MUL % B == 0 && MUL >= (GMUL > 0 ? (GMUL + B - 1) / B : VT<T>::CB) * B;
+}
+
 // ---- strided channel loads: component i of CPT adjacent channels ---------------------
 // p points at (channel ch0, component i); the next channel is N elements further.
-template <int N, int MUL> __device__ __forceinline__ float2 vload(const float* __restrict__ p, int ch0) {
-  constexpr bool full = (MUL % (VT<float>::LPE * 2)) == 0;
+template <int N, int MUL, int GMUL = 0> __device__ __forceinline__ float2 vload(const float* __restrict__ p, int ch0) {
+  constexpr bool full = vfull<float, MUL, GMUL>();
   if (full) return make_float2(__ldg(p), __ldg(p + N));
   return make_float2(ch0 < MUL ? __ldg(p) : 0.f, ch0 + 1 < MUL ? __ldg(p + N) : 0.f);
 }
-template <int N, int MUL> __device__ __forceinline__ double vload(const double* __restrict__ p, int ch0) {
-  constexpr bool full = (MUL % VT<double>::LPE) == 0;
+template <int N, int MUL, int GMUL = 0> __device__ __forceinline__ double vload(const double* __restrict__ p, int ch0) {
+  constexpr bool full = vfull<double, MUL, GMUL>();
   if (full) return __ldg(p);
   return ch0 < MUL ? __ldg(p) : 0.0;
 }
-template <int N, int MUL> __device__ __forceinline__ void vstore(float* __restrict__ p, float2 v, int ch0) {
-  constexpr bool full = (MUL % (VT<float>::LPE * 2)) == 0;
+template <int N, int MUL, int GMUL = 0> __device__ __forceinline__ void vstore(float* __restrict__ p, float2 v, int ch0) {
+  constexpr bool full = vfull<float, MUL, GMUL>();
   if (full || ch0 < MUL) p[0] = v.x;
   if (full || ch0 + 1 < MUL) p[N] = v.y;
 }
-template <int N, int MUL> __device__ __forceinline__ void vstore(double* __restrict__ p, double v, int ch0) {
-  constexpr bool full = (MUL % VT<double>::LPE) == 0;
+template <int N, int MUL, int GMUL = 0> __device__ __forceinline__ void vstore(double* __restrict__ p, double v, int ch0) {
+  constexpr bool full = vfull<double, MUL, GMUL>();
   if (full || ch0 < MUL) p[0] = v;
 }
-template <int N, int MUL> __device__ __forceinline__ void vatomic(float* p, float2 v, int ch0) {
-  constexpr bool full = (MUL % (VT<float>::LPE * 2)) == 0;
+template <int N, int MUL, int GMUL = 0> __device__ __forceinline__ void vatomic(float* p, float2 v, int ch0) {
+  constexpr bool full = vfull<float, MUL, GMUL>();
   if (full || ch0 < MUL) atomicAdd(p, v.x);
   if (full || ch0 + 1 < MUL) atomicAdd(p + N, v.y);
 }
-template <int N, int MUL> __device__ __forceinline__ void vatomic(double* p, double v, int ch0) {
-  constexpr bool full = (MUL % VT<double>::LPE) == 0;
+template <int N, int MUL, int GMUL = 0> __device__ __forceinline__ void vatomic(double* p, double v, int ch0) {
+  constexpr bool full = vfull<double, MUL, GMUL>();
   if (full || ch0 < MUL) atomicAdd(p, v);
 }
 
 // ---- channel-contiguous (ir_mul) accesses: the CPT channels of one component are adjacent ----------
-template <int MUL, bool AL2> __device__ __forceinline__ float2 vloadc(const float* __restrict__ p, int ch0) {
-  constexpr bool full = (MUL % (VT<float>::LPE * 2)) == 0;
+template <int MUL, bool AL2, int GMUL = 0> __device__ __forceinline__ float2 vloadc(const float* __restrict__ p, int ch0) {
+  constexpr bool full = vfull<float, MUL, GMUL>();
   if (full && AL2) return __ldg(reinterpret_cast<const float2*>(p));
   return make_float2((full || ch0 < MUL) ? __ldg(p) : 0.f, (full || ch0 + 1 < MUL) ? __ldg(p + 1) : 0.f);
 }
-template <int MUL, bool AL2> __device__ __forceinline__ double vloadc(const double* __restrict__ p, int ch0) {
-  constexpr bool full = (MUL % VT<double>::LPE) == 0;
+template <int MUL, bool AL2, int GMUL = 0> __device__ __forceinline__ double vloadc(const double* __restrict__ p, int ch0) {
+  constexpr bool full = vfull<double, MUL, GMUL>();
   return (full || ch0 < MUL) ? __ldg(p) : 0.0;
 }
 __device__ __forceinline__ void red_v2(float* p, float a, float b);
-template <int MUL, bool AL2> __device__ __forceinline__ void vatomicc(float* p, float2 v, int ch0) {
-  constexpr bool full = (MUL % (VT<float>::LPE * 2)) == 0;
+template <int MUL, bool AL2, int GMUL = 0> __device__ __forceinline__ void vatomicc(float* p, float2 v, int ch0) {
+  constexpr bool full = vfull<float, MUL, GMUL>();
   if (full && AL2) {
     red_v2(p, v.x, v.y);
   } else {
@@ -81,8 +90,8 @@ template <int MUL, bool AL2> __device__ __forceinline__ void vatomicc(float* p, 
     if (full || ch0 + 1 < MUL) atomicAdd(p + 1, v.y);
   }
 }
-template <int MUL, bool AL2> __device__ __forceinline__ void vatomicc(double* p, double v, int ch0) {
-  constexpr bool full = (MUL % VT<double>::LPE) == 0;
+template <int MUL, bool AL2, int GMUL = 0> __device__ __forceinline__ void vatomicc(double* p, double v, int ch0) {
+  constexpr bool full = vfull<double, MUL, GMUL>();
   if (full || ch0 < MUL) atomicAdd(p, v);
 }
 
@@ -91,9 +100,9 @@ template <int MUL, bool AL2> __device__ __forceinline__ void vatomicc(double* p,
 __device__ __forceinline__ void red_v2(float* p, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
-template <int N, int MUL, typename... Vs> __device__ __forceinline__ void vatomic_row(float* p, int ch0, Vs... vs) {
+template <int N, int MUL, int GMUL = 0, typename... Vs> __device__ __forceinline__ void vatomic_row(float* p, int ch0, Vs... vs) {
   static_assert(sizeof...(Vs) == N, "one value per component");
-  constexpr bool full = (MUL % (VT<float>::LPE * 2)) == 0;
+  constexpr bool full = vfull<float, MUL, GMUL>();
   const float2 v[N] = {vs...};
   if (full) {
     float flat[2 * N];
@@ -109,8 +118,8 @@ template <int N, int MUL, typename... Vs> __device__ __forceinline__ void vatomi
     }
   }
 }
-template <int N, int MUL, typename... Vs> __device__ __forceinline__ void vatomic_row(double* p, int ch0, Vs... vs) {
-  constexpr bool full = (MUL % VT<double>::LPE) == 0;
+template <int N, int MUL, int GMUL = 0, typename... Vs> __device__ __forceinline__ void vatomic_row(double* p, int ch0, Vs... vs) {
+  constexpr bool full = vfull<double, MUL, GMUL>();
   const double v[N] = {vs...};
 #pragma unroll
   for (int i = 0; i < N; ++i)
@@ -133,8 +142,8 @@ __device__ __forceinline__ double ld_stream(const double* p) {
   asm volatile("ld.global.nc.L1::no_allocate.f64 %0, [%1];" : "=d"(r) : "l"(p));
   return r;
 }
-template <int MUL, bool AL2> __device__ __forceinline__ float2 vloadw(const float* __restrict__ p, int ch0, bool valid) {
-  constexpr bool full = (MUL % (VT<float>::LPE * 2)) == 0;
+template <int MUL, bool AL2, int GMUL = 0> __device__ __forceinline__ float2 vloadw(const float* __restrict__ p, int ch0, bool valid) {
+  constexpr bool full = vfull<float, MUL, GMUL>();
   float2 r;
   if (full && AL2) {
     r = ld_stream2(p);
@@ -145,13 +154,13 @@ template <int MUL, bool AL2> __device__ __forceinline__ float2 vloadw(const floa
   if (!valid) r = make_float2(0.f, 0.f);
   return r;
 }
-template <int MUL, bool AL2> __device__ __forceinline__ double vloadw(const double* __restrict__ p, int ch0, bool valid) {
-  constexpr bool full = (MUL % VT<double>::LPE) == 0;
+template <int MUL, bool AL2, int GMUL = 0> __device__ __forceinline__ double vloadw(const double* __restrict__ p, int ch0, bool valid) {
+  constexpr bool full = vfull<double, MUL, GMUL>();
   double r = (full || ch0 < MUL) ? ld_stream(p) : 0.0;
   return valid ? r : 0.0;
 }
-template <int MUL, bool AL2> __device__ __forceinline__ void vstorew(float* __restrict__ p, float2 v, int ch0) {
-  constexpr bool full = (MUL % (VT<float>::LPE * 2)) == 0;
+template <int MUL, bool AL2, int GMUL = 0> __device__ __forceinline__ void vstorew(float* __restrict__ p, float2 v, int ch0) {
+  constexpr bool full = vfull<float, MUL, GMUL>();
   if (full && AL2) {
     *reinterpret_cast<float2*>(p) = v;
   } else {
@@ -159,8 +168,8 @@ template <int MUL, bool AL2> __device__ __forceinline__ void vstorew(float* __re
     if (full || ch0 + 1 < MUL) p[1] = v.y;
   }
 }
-template <int MUL, bool AL2> __device__ __forceinline__ void vstorew(double* __restrict__ p, double v, int ch0) {
-  constexpr bool full = (MUL % VT<double>::LPE) == 0;
+template <int MUL, bool AL2, int GMUL = 0> __device__ __forceinline__ void vstorew(double* __restrict__ p, double v, int ch0) {
+  constexpr bool full = vfull<double, MUL, GMUL>();
   if (full || ch0 < MUL) p[0] = v;
 }
 
@@ -195,8 +204,8 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 }
 #endif  // NQB_TC_HELPERS
 // weights of the channel pair from the shared-memory ring
-template <int MUL, bool AL2> __device__ __forceinline__ float2 vloadws(const float* p, int ch0, bool valid) {
-  constexpr bool full = (MUL % (VT<float>::LPE * 2)) == 0;
+template <int MUL, bool AL2, int GMUL = 0> __device__ __forceinline__ float2 vloadws(const float* p, int ch0, bool valid) {
+  constexpr bool full = vfull<float, MUL, GMUL>();
   float2 r = make_float2(0.f, 0.f);
   if (valid) {
     if (full && AL2) {

@@ -32,18 +32,32 @@ def reference_test_grid() -> List[TPSignature]:
     return out
 
 
-def nequip_layer_signatures(l_max: int, num_features: int, num_layers: int, parity: bool = True) -> List[TPSignature]:
+def nequip_layer_signatures(l_max: int, num_features, num_layers: int, parity: bool = True,
+                            type_embed_num_features=None) -> List[TPSignature]:
     """Per-layer signatures of ``NequIPGNNModel`` (nequip/model/nequip_models.py:116-210 +
-    nequip/nn/convnetlayer.py:74-114): returns one TPSignature per interaction layer."""
+    nequip/nn/convnetlayer.py:74-114): returns one TPSignature per interaction layer.  ``num_features`` is an int or
+    one width per degree."""
     from .nn.model import layer_irreps  # local import: nn.model imports this package
 
-    return [make_signature(fin, fe, fout) for (fin, fe, fout, _gate) in layer_irreps(l_max, num_features, num_layers, parity)]
+    return [make_signature(fin, fe, fout) for (fin, fe, fout, _gate)
+            in layer_irreps(l_max, num_features, num_layers, parity, type_embed_num_features)]
+
+
+def preset_layer_signatures(name: str) -> List[TPSignature]:
+    """Per-layer signatures of the reference's named architecture ``name`` (S, M, L, XL)."""
+    from .nn.model import preset_kwargs
+
+    kw = preset_kwargs(name)
+    return nequip_layer_signatures(kw["l_max"], kw["num_features"], kw["num_layers"], kw["parity"],
+                                   kw["type_embed_num_features"])
 
 
 def all_known() -> List[TPSignature]:
     sigs = reference_test_grid()
     for (lm, nf, nl) in [(1, 32, 4), (2, 32, 4), (2, 64, 4), (3, 32, 5), (2, 8, 3), (1, 8, 2)]:
         sigs += nequip_layer_signatures(lm, nf, nl)
+    for name in ("S", "M", "L", "XL"):
+        sigs += preset_layer_signatures(name)
     uniq = {}
     for s in sigs:
         uniq[s.canonical()] = s

@@ -21,7 +21,7 @@ Reference files mirrored (under /root/reference):
 from __future__ import annotations
 
 import math
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -55,13 +55,26 @@ NUM_NODES_KEY = "num_atoms"
 # ---------------------------------------------------------------------------------------
 # irreps bookkeeping of the conv stack
 # ---------------------------------------------------------------------------------------
-def hidden_irreps(l_max: int, num_features: int, parity: bool) -> Irreps:
-    """``feature_irreps_hidden`` of NequIPGNNModel (nequip_models.py:176-187)."""
+def feature_widths(l_max: int, num_features) -> List[int]:
+    """One width per degree 0..l_max: an int applies to every degree, a list is taken as is
+    (nequip_models.py:164-169)."""
+    if isinstance(num_features, int):
+        return [num_features] * (l_max + 1)
+    widths = [int(f) for f in num_features]
+    if len(widths) != l_max + 1:
+        raise ValueError(f"num_features: expected an int or l_max + 1 = {l_max + 1} widths, got {list(num_features)}")
+    return widths
+
+
+def hidden_irreps(l_max: int, num_features, parity: bool) -> Irreps:
+    """``feature_irreps_hidden`` of NequIPGNNModel (nequip_models.py:176-187); ``num_features`` is an int or one
+    width per degree."""
+    widths = feature_widths(l_max, num_features)
     items = []
     for l in range(l_max + 1):
         ps = (1, -1) if parity else ((1,) if l % 2 == 0 else (-1,))
         for p in ps:
-            items.append((num_features, Irrep(l, p)))
+            items.append((widths[l], Irrep(l, p)))
     return Irreps(items)
 
 
@@ -79,13 +92,14 @@ def gate_irreps(prev: Irreps, edge_attr: Irreps, hidden: Irreps):
     return scalars, gates, gated, conv_out, layer_out
 
 
-def layer_irreps(l_max: int, num_features: int, num_layers: int, parity: bool = True, type_embed_num_features=None):
+def layer_irreps(l_max: int, num_features, num_layers: int, parity: bool = True, type_embed_num_features=None):
     """[(feature_irreps_in, irreps_edge_attr, conv_irreps_out, (scalars, gates, gated))] per layer."""
-    f0 = type_embed_num_features or num_features
+    widths = feature_widths(l_max, num_features)
+    f0 = type_embed_num_features or widths[0]
     edge_attr = Irreps.spherical_harmonics(l_max)
     prev = Irreps([(f0, Irrep(0, 1))])
-    hid = hidden_irreps(l_max, num_features, parity)
-    hiddens = [hid] * (num_layers - 1) + [Irreps([(num_features, Irrep(0, 1))])]
+    hid = hidden_irreps(l_max, widths, parity)
+    hiddens = [hid] * (num_layers - 1) + [Irreps([(widths[0], Irrep(0, 1))])]
     out = []
     for h in hiddens:
         scalars, gates, gated, conv_out, layer_out = gate_irreps(prev, edge_attr, h)
@@ -502,6 +516,25 @@ class ConvNetLayer(torch.nn.Module):
         return self.equivariant_nonlin(x)
 
 
+# The named architectures of the NequIP foundation potentials: _NEQUIP_GNN_PRESETS (nequip_models.py:30-51) on top
+# of _NEQUIP_GNN_STANDARD_PRESET (nequip_models.py:53-58), combined as PresetNequIPGNNModel does (:98-115).
+NEQUIP_PRESETS: Dict[str, dict] = {
+    "S": dict(num_layers=2, l_max=1, num_features=[128, 64]),
+    "M": dict(num_layers=4, l_max=2, num_features=[128, 64, 32]),
+    "L": dict(num_layers=6, l_max=3, num_features=[128, 64, 32, 32]),
+    "XL": dict(num_layers=6, l_max=4, num_features=[320, 96, 64, 32, 32]),
+}
+NEQUIP_STANDARD_PRESET = dict(parity=False, type_embed_num_features=32, radial_mlp_depth=1, radial_mlp_width=128)
+
+
+def preset_kwargs(name: str, **overrides) -> dict:
+    """Constructor arguments of preset ``name`` (case-insensitive): standard preset < named preset < ``overrides``."""
+    key = name.upper()
+    if key not in NEQUIP_PRESETS:
+        raise ValueError(f"unknown preset {name!r}: expected one of {sorted(NEQUIP_PRESETS)}")
+    return {**NEQUIP_STANDARD_PRESET, **NEQUIP_PRESETS[key], **overrides}
+
+
 class NequIPEnergyModel(torch.nn.Module):
     """``NequIPGNNModel`` (nequip_models.py:116-210) wrapped in the force part of
     ``ForceStressOutput`` (grad_output.py:215-232).  ``forward(data) -> data`` on an
@@ -509,17 +542,25 @@ class NequIPEnergyModel(torch.nn.Module):
     ``atom_types`` [N] i64 and, for periodic systems, ``cell`` [3,3] + ``edge_cell_shift`` [E,3]."""
 
     def __init__(self, *, r_max: float, type_names: Sequence[str], num_layers: int = 4, l_max: int = 1,
-                 parity: bool = True, num_features: int = 32, radial_mlp_depth: int = 1,
+                 parity: bool = True, num_features: Union[int, Sequence[int]] = 32,
+                 type_embed_num_features: Optional[int] = None, radial_mlp_depth: int = 1,
                  radial_mlp_width: int = 128, num_bessels: int = 8, polynomial_cutoff_p: float = 6.0,
                  avg_num_neighbors: float = 1.0, per_type_energy_scales: Optional[Sequence[float]] = None,
                  per_type_energy_shifts: Optional[Sequence[float]] = None, model_dtype=torch.float32,
                  seed: int = 123, node_layout: str = "ir_mul", strict_fast_path: bool = False):
+        """``num_features``: one width for every degree, or a list of l_max + 1 widths (one per degree, e.g.
+        ``[128, 64, 32]`` = 128x0e + 64x1o + 32x2e for l_max = 2 without parity), as in nequip_models.py:164-190.
+        ``type_embed_num_features``: width of the type embedding, which is also the first layer's input and the
+        self-connection's attribute width (nequip_models.py:171-174, 294); defaults to ``num_features[0]``."""
         super().__init__()
+        widths = feature_widths(l_max, num_features)
+        f_embed = int(type_embed_num_features) if type_embed_num_features is not None else widths[0]
         self.r_max, self.l_max, self.num_bessels, self.poly_p = float(r_max), l_max, num_bessels, float(polynomial_cutoff_p)
         self.model_dtype = model_dtype
         self.node_layout = node_layout  # internal layout of node features between the kernels
         self.config = dict(r_max=r_max, type_names=list(type_names), num_layers=num_layers, l_max=l_max, parity=parity,
-                           num_features=num_features, radial_mlp_depth=radial_mlp_depth,
+                           num_features=num_features if isinstance(num_features, int) else widths,
+                           type_embed_num_features=f_embed, radial_mlp_depth=radial_mlp_depth,
                            radial_mlp_width=radial_mlp_width, num_bessels=num_bessels,
                            polynomial_cutoff_p=polynomial_cutoff_p, avg_num_neighbors=avg_num_neighbors)
         prev_default = torch.get_default_dtype()
@@ -536,14 +577,14 @@ class NequIPEnergyModel(torch.nn.Module):
                 if len(avg_num_neighbors) not in (1, ntypes):
                     raise ValueError(f"avg_num_neighbors: expected a scalar or {ntypes} values")
             self.config["avg_num_neighbors"] = avg_num_neighbors
-            self.type_embed = torch.nn.Embedding(ntypes, num_features)
+            self.type_embed = torch.nn.Embedding(ntypes, f_embed)
             edge_attr = Irreps.spherical_harmonics(l_max)
-            prev = Irreps([(num_features, Irrep(0, 1))])
-            hid = hidden_irreps(l_max, num_features, parity)
-            hiddens = [hid] * (num_layers - 1) + [Irreps([(num_features, Irrep(0, 1))])]
+            prev = Irreps([(f_embed, Irrep(0, 1))])
+            hid = hidden_irreps(l_max, widths, parity)
+            hiddens = [hid] * (num_layers - 1) + [Irreps([(widths[0], Irrep(0, 1))])]
             layers = []
             for li, h in enumerate(hiddens):
-                layer = ConvNetLayer(prev, edge_attr, h, num_edge_embed=num_bessels, num_node_attrs=num_features,
+                layer = ConvNetLayer(prev, edge_attr, h, num_edge_embed=num_bessels, num_node_attrs=f_embed,
                                      radial_mlp_depth=radial_mlp_depth, radial_mlp_width=radial_mlp_width,
                                      use_sc=(li != 0), avg_num_neighbors=avg_num_neighbors,
                                      is_first_layer=(li == 0), layout=node_layout)
@@ -568,6 +609,12 @@ class NequIPEnergyModel(torch.nn.Module):
         self.register_buffer("scales", table(per_type_energy_scales, "per_type_energy_scales"))
         self.register_buffer("shifts", table(per_type_energy_shifts, "per_type_energy_shifts"))
         self.set_strict_fast_path(strict_fast_path)
+
+    @classmethod
+    def from_preset(cls, name: str, **kwargs) -> "NequIPEnergyModel":
+        """One of the reference's named architectures ``S``, ``M``, ``L``, ``XL`` (``NEQUIP_PRESETS``); ``kwargs``
+        must include ``r_max`` and ``type_names`` and override any preset value."""
+        return cls(**preset_kwargs(name, **kwargs))
 
     def set_strict_fast_path(self, on: bool = True):
         """Raise instead of warning when an interaction block cannot use the wgmma dense blocks."""
