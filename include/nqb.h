@@ -178,17 +178,10 @@ int nqb_nl_fill(int64_t N, int64_t E, const double* cell_host, const double* inv
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).
  * Together with nqb_gemm_grouped for the second layer this is ScalarMLPFunction (nequip/nn/mlp.py:80-195). */
-/* h_lo (nullable): the part of h the tensor core does not see, h_lo = rna_tf32(h - trunc_tf32(h)).  It can be
- * handed to nqb_gemm_grouped as a_lo_base, but that form doubles the A reads: the product path passes NULL for both. */
 int nqb_mlp_hidden_fwd(const float* emb, const float* W1s, int64_t E, int num_bessel, int hidden, float* h,
-                       float* h_lo, nqb_stream_t st);
+                       nqb_stream_t st);
 int nqb_mlp_hidden_bwd(const float* emb, const float* W1s, const float* grad_h, int64_t E, int num_bessel,
                        int hidden, float* grad_emb, nqb_stream_t st);
-/* Kernel generation of the two calls above: 2 = batched kernels (32 edges per warp, prefetched basis values, float2
- * arithmetic, one 128-byte grad_emb row per four edges), 1 = the round-1 kernels (one edge per warp iteration).  Returns the
- * previous value; 0 only queries.  Default: the library's build-time choice, overridden by the environment variable
- * NQB_HIDDEN_VARIANT=1|2.  Not thread safe -- call between launches (A/B timing, parity tests). */
-int nqb_mlp_hidden_set_variant(int variant);
 
 /* Grouped fp32-accurate GEMM on the tensor cores (wgmma tf32, 3xTF32, segmented fp32
  * accumulation):  C_p[M, N_p] (+)= rowscale_p[m] * A_p[M, K_p] @ B_p[K_p, N_p]  for a list of problems
@@ -204,15 +197,12 @@ int nqb_mlp_hidden_set_variant(int variant);
  * B_p is prepared once (split hi/lo, tiled) with nqb_gemm_prepare into nqb_gemm_prepared_floats(K,N) floats.
  * tile_ctas_dev (nullable): int32 {first CTA, CTAs} per N-tile -- a cost-weighted split of sched_ctas CTAs over
  * the N-tiles computed by the host (problems of one launch differ in K, N and store mode); used when
- * sched_ctas <= #SMs, otherwise the even split is used.
- * a_lo_base (nullable): pre-split low parts of A, same offsets/strides as a_base (see nqb_mlp_hidden_fwd);
- * when null the kernel derives them itself. */
+ * sched_ctas <= #SMs, otherwise the even split is used. */
 int64_t nqb_gemm_prepared_floats(int K, int N);
 int nqb_gemm_prepare(const float* B, int64_t ldb, int K, int N, int transposed, float scale, float* prepared,
                      nqb_stream_t st);
 int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
-                     int sched_ctas, const float* a_base,
-                     const float* a_lo_base, const float* prepared_base, float* c_base,
+                     int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
                      const float* rowscale_base, int64_t rs_ld, int64_t M, nqb_stream_t st);
 
 /* Gate nonlinearity (e3nn nn.Gate with normalize2mom'd SiLU for even / tanh for odd scalars and gates,

@@ -56,14 +56,13 @@ SIGNATURES = {
         _i32, [_i32, _i32, _dbl, _dbl, _dbl, _vp, _vp, _vp, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp]),
     "nqb_edge_embed_bwd": (
         _i32, [_i32, _i32, _dbl, _dbl, _dbl, _vp, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
-    "nqb_mlp_hidden_fwd": (_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
+    "nqb_mlp_hidden_fwd": (_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
-    "nqb_mlp_hidden_set_variant": (_i32, [_i32]),
     "nqb_gemm_prepared_floats": (_i64, [_i32, _i32]),
     "nqb_gemm_prepare": (_i32, [_vp, _i64, _i32, _i32, _i32, C.c_float, _vp, _vp]),
     "nqb_gate_fwd": (_i32, [_i32, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "nqb_gate_bwd": (_i32, [_i32, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
-    "nqb_gemm_grouped": (_i32, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp]),
+    "nqb_gemm_grouped": (_i32, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i64, _i64, _vp]),
 }
 
 
@@ -78,7 +77,7 @@ def lib() -> C.CDLL:
             fn = getattr(L, name)  # AttributeError if the symbol is missing
             fn.restype = res
             fn.argtypes = args
-        if L.nqb_abi_version() != 1:
+        if L.nqb_abi_version() != 2:
             raise RuntimeError("libnqb.so ABI version mismatch")
         _lib = L
     return _lib

@@ -113,9 +113,8 @@ __device__ __forceinline__ void bar_wg(int wg) { asm volatile("bar.sync %0, 128;
 
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const int32_t* __restrict__ tile_ctas,
-         int sched_ctas, const float* __restrict__ a_base,
-         const float* __restrict__ a_lo_base, const float* __restrict__ b_base, float* __restrict__ c_base, const float* __restrict__ rs_base, int64_t rs_ld,
-         int64_t M) {
+         int sched_ctas, const float* __restrict__ a_base, const float* __restrict__ b_base, float* __restrict__ c_base,
+         const float* __restrict__ rs_base, int64_t rs_ld, int64_t M) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& S = *reinterpret_cast<Smem*>(smem_raw);
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
@@ -127,7 +126,6 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
   }
   __syncthreads();
   const Sched sch(blockIdx.x, gridDim.x, ntiles_total, tile_ctas, sched_ctas);
-  const bool presplit = a_lo_base != nullptr;  // caller-supplied low parts: only copied
 
   // ---- A staging: a cursor over this CTA's flat chunk sequence (N-tile q, M-tile pmt, chunk ph_) -------------
   // thread -> rows 16 warp + 8 g + r8 (g < 2) of the warpgroup's 64, k-groups 4 kh + kq (kh < 2): a quarter warp
@@ -137,13 +135,11 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
   int pq = sch.q, ph_ = 0, pnh = 1, pK = 0;
   int64_t pmt = sch.m_start, plda = 0;
   const float* pA = nullptr;
-  const float* pAlo = nullptr;
   bool pvalid = pq < sch.nq_total && sch.m_start < mtiles;
   auto open_q = [&]() {
     WorkQ w;
     decode_q(descs, ndesc, pq, w);
     pA = a_base + w.d->a_off;
-    if (presplit) pAlo = a_lo_base + w.d->a_off;
     plda = w.d->lda;
     pK = w.K;
     pnh = w.kchunks;
@@ -153,7 +149,6 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
   auto issue = [&]() {  // cp.async the cursor's chunk into raw stage n_issued % RAW, advance, commit
     if (pvalid) {
       float* dst = S.araw[wg][n_issued % RAW] + my_off;
-      float* dlo = S.alo[wg][n_issued % NLO] + my_off;
 #pragma unroll
       for (int g = 0; g < 2; ++g) {
         const int64_t m = pmt * TM + wg * MW + warp * 16 + g * 8 + r8;
@@ -163,7 +158,6 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
           const bool in = m < M && k < pK;
           const int64_t off = in ? m * plda + k : 0;
           cp_async16(dst + g * (KC / 4 * 32) + kh * 128, pA + off, in ? 16u : 0u);
-          if (presplit) cp_async16(dlo + g * (KC / 4 * 32) + kh * 128, pAlo + off, in ? 16u : 0u);
         }
       }
       if (++ph_ == pnh) {
@@ -232,17 +226,15 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
         for (int h = seg * SEG; h < h1; ++h, ++i) {
           cp_async_wait<DEPTH - 1>();  // my parts of chunk i have landed
           const float* raw = S.araw[wg][i % RAW] + my_off;
-          if (!presplit) {
-            float* lo = S.alo[wg][i % NLO] + my_off;
+          float* lo = S.alo[wg][i % NLO] + my_off;
 #pragma unroll
-            for (int g = 0; g < 2; ++g)
+          for (int g = 0; g < 2; ++g)
 #pragma unroll
-              for (int kh = 0; kh < 2; ++kh) {
-                const float4 t = *reinterpret_cast<const float4*>(raw + g * (KC / 4 * 32) + kh * 128);
-                *reinterpret_cast<float4*>(lo + g * (KC / 4 * 32) + kh * 128) =
-                    make_float4(tf32_lo(t.x), tf32_lo(t.y), tf32_lo(t.z), tf32_lo(t.w));
-              }
-          }
+            for (int kh = 0; kh < 2; ++kh) {
+              const float4 t = *reinterpret_cast<const float4*>(raw + g * (KC / 4 * 32) + kh * 128);
+              *reinterpret_cast<float4*>(lo + g * (KC / 4 * 32) + kh * 128) =
+                  make_float4(tf32_lo(t.x), tf32_lo(t.y), tf32_lo(t.z), tf32_lo(t.w));
+            }
           fence_proxy_async();  // generic-proxy writes -> visible to the tensor core
           bar_wg(wg);
           uint32_t slot;
@@ -375,8 +367,7 @@ extern "C" int nqb_gemm_prepare(const float* B, int64_t ldb, int K, int N, int t
 }
 
 extern "C" int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
-                                int sched_ctas, const float* a_base,
-                                const float* a_lo_base, const float* prepared_base, float* c_base,
+                                int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
                                 const float* rowscale_base, int64_t rs_ld, int64_t M, nqb_stream_t st) {
   if (ndesc <= 0 || ntiles_total <= 0) return nqb_set_error("nqb_gemm_grouped: empty problem list");
   if (M < 0) return nqb_set_error("nqb_gemm_grouped: negative M");
@@ -393,7 +384,7 @@ extern "C" int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_tot
   int grid = (int)(nwork < gemm_sm_count() ? nwork : gemm_sm_count());
   if (tile_ctas_dev != nullptr && sched_ctas > 0 && sched_ctas <= gemm_sm_count()) grid = sched_ctas;
   else tile_ctas_dev = nullptr;
-  k_gemm3x<<<grid, NTHREADS, sizeof(Smem) + 1024, (cudaStream_t)st>>>((const GemmDesc*)descs_dev, ndesc, ntiles_total, tile_ctas_dev, sched_ctas, a_base, a_lo_base,
+  k_gemm3x<<<grid, NTHREADS, sizeof(Smem) + 1024, (cudaStream_t)st>>>((const GemmDesc*)descs_dev, ndesc, ntiles_total, tile_ctas_dev, sched_ctas, a_base,
                                                                  prepared_base, c_base, rowscale_base, rs_ld, M);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();

@@ -7,7 +7,6 @@
 //     w   =      h   @ (W2 * a2)           [E, H ] x [H, W]    nqb_gemm.cu (unfused) / the fused TP kernels
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "../../include/nqb.h"
 #include "nqb_tc.cuh"
@@ -21,13 +20,16 @@ constexpr int NB = 8;        // Bessel functions
 // first radial layer on CUDA cores (K = 8): h = silu(emb @ W1s)  and its backward
 //   gemb[e, k] = sum_m gh[e, m] * silu'(pre[e, m]) * W1s[k, m],  pre recomputed from emb
 // (feeds / follows the grouped tensor-core GEMM of the second layer, nqb_gemm.cu)
+//   * lane = 4 hidden units whose 8 x 4 first-layer weights live in registers for the whole kernel;
+//   * a warp owns a BATCH of 32 consecutive edges; lane j fetches edge j's 8 basis values with two
+//     coalesced 16-byte loads (1 KB per warp) and the batch after that is already in flight while the
+//     current one is computed; inside the batch the values of edge j are broadcast with warp shuffles,
+//     so no load sits on the critical path of an edge;
+//   * float2 arithmetic on two hidden units at a time, sigmoid from ex2.approx / rcp.approx;
+//   * backward: four edges per inner iteration -- their four grad_h rows are loaded up front and the
+//     4 x 8 partial sums are reduced with one 32-value halving butterfly (31 shuffles) that leaves
+//     element `lane` in lane `lane`: grad_emb is written as one 128-byte row.
 // ---------------------------------------------------------------------------------------------
-// Persistent warps: lane = 4 hidden units whose 8 x 4 first-layer weights live in registers for the whole
-// kernel; a warp walks over edges (grid-stride), reads the 8 basis values of the edge (one broadcast
-// 32-byte load) and writes the edge's 128 activations as one 512-byte row.  (The first version re-staged
-// the 4 KB weight matrix per 8 edges -- as many bytes as it wrote.)
-// both kernel generations use this sigmoid, so that their activations agree bit for bit (h is computed by either,
-// depending on whether the tf32 low part is requested)
 __device__ __forceinline__ float ex2_approx(float x) {
   float r;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
@@ -39,105 +41,7 @@ __device__ __forceinline__ float rcp_approx(float x) {
   return r;
 }
 // 1 / (1 + exp(-p));  p -> -inf gives rcp(inf) = 0, p -> +inf gives rcp(1) = 1
-__device__ __forceinline__ float sigmoid_v2(float p) { return rcp_approx(1.0f + ex2_approx(p * -1.4426950408889634f)); }
-
-__global__ void __launch_bounds__(256) k_hidden_fwd(const float* __restrict__ emb, const float* __restrict__ W1s,
-                                                    int64_t E, float* __restrict__ h, float* __restrict__ h_lo) {
-  const int lane = threadIdx.x & 31, m0 = lane * 4;
-  float w[NB][4];
-#pragma unroll
-  for (int k = 0; k < NB; ++k) {
-    const float4 t = __ldg(reinterpret_cast<const float4*>(W1s + k * H + m0));
-    w[k][0] = t.x; w[k][1] = t.y; w[k][2] = t.z; w[k][3] = t.w;
-  }
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  for (int64_t e = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); e < E; e += nwarps) {
-    const float4 x0 = __ldg(reinterpret_cast<const float4*>(emb + e * NB));
-    const float4 x1 = __ldg(reinterpret_cast<const float4*>(emb + e * NB + 4));
-    const float x[NB] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-    float o[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      float p = 0.f;
-#pragma unroll
-      for (int k = 0; k < NB; ++k) p = fmaf(x[k], w[k][q], p);
-      o[q] = p * sigmoid_v2(p);
-    }
-    __stcs(reinterpret_cast<float4*>(h + e * H + m0), make_float4(o[0], o[1], o[2], o[3]));
-    if (h_lo) __stcs(reinterpret_cast<float4*>(h_lo + e * H + m0), make_float4(tf32_lo(o[0]), tf32_lo(o[1]), tf32_lo(o[2]), tf32_lo(o[3])));
-  }
-}
-
-__global__ void __launch_bounds__(256) k_hidden_bwd(const float* __restrict__ emb, const float* __restrict__ W1s,
-                                                    const float* __restrict__ gh, int64_t E, float* __restrict__ gemb) {
-  const int lane = threadIdx.x & 31, m0 = lane * 4;
-  float w[NB][4];
-#pragma unroll
-  for (int k = 0; k < NB; ++k) {
-    const float4 t = __ldg(reinterpret_cast<const float4*>(W1s + k * H + m0));
-    w[k][0] = t.x; w[k][1] = t.y; w[k][2] = t.z; w[k][3] = t.w;
-  }
-  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
-  for (int64_t e = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); e < E; e += nwarps) {  // warp = edge
-  const float4 x0 = __ldg(reinterpret_cast<const float4*>(emb + e * NB));
-  const float4 x1 = __ldg(reinterpret_cast<const float4*>(emb + e * NB + 4));
-  const float x[NB] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-  const float4 g4 = __ldcs(reinterpret_cast<const float4*>(gh + e * H + m0));
-  const float g[4] = {g4.x, g4.y, g4.z, g4.w};
-  float acc[NB];
-#pragma unroll
-  for (int k = 0; k < NB; ++k) acc[k] = 0.f;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    float p = 0.f;
-#pragma unroll
-    for (int k = 0; k < NB; ++k) p = fmaf(x[k], w[k][q], p);
-    const float sg = sigmoid_v2(p);
-    const float gp = g[q] * (sg * (1.0f + p * (1.0f - sg)));
-#pragma unroll
-    for (int k = 0; k < NB; ++k) acc[k] = fmaf(gp, w[k][q], acc[k]);
-  }
-  // reduce the 8 partial sums over the 32 lanes (halving butterfly: 4 + 2 + 1 + 2 shuffles)
-#pragma unroll
-  for (int o = 16, c = NB; o >= 1; o >>= 1) {
-    if (c > 1) {
-      c >>= 1;
-      const bool up = (lane & o) != 0;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (j < c) {
-          const float mine = up ? acc[j + c] : acc[j];
-          const float theirs = up ? acc[j] : acc[j + c];
-          acc[j] = mine + __shfl_xor_sync(0xffffffffu, theirs, o);
-        }
-      }
-    } else {
-      acc[0] += __shfl_xor_sync(0xffffffffu, acc[0], o);
-    }
-  }
-  // after the three halving steps lane bits (16, 8, 4) select the component: k = 4*b16 + 2*b8 + b4
-  if ((lane & 3) == 0) {
-    const int k = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
-    gemb[e * NB + k] = acc[0];
-  }
-  }  // edge loop
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// v2 of the two kernels.  v1 runs 4 CTAs per SM (55-63 registers) with ONE edge per warp iteration and the
-// edge's basis values fetched by a dependent broadcast load at the top of every iteration: 32 edges in
-// flight per SM, each paying a full DRAM latency before its arithmetic starts.  v2:
-//   * a warp owns a BATCH of 32 consecutive edges; lane j fetches edge j's 8 basis values with two
-//     coalesced 16-byte loads (1 KB per warp) and the batch after that is already in flight while the
-//     current one is computed; inside the batch the values of edge j are broadcast with warp shuffles,
-//     so no load sits on the critical path of an edge;
-//   * float2 arithmetic on two hidden units at a time, sigmoid from ex2.approx / rcp.approx (as v1);
-//   * backward: four edges per inner iteration -- their four grad_h rows are loaded up front and the
-//     4 x 8 partial sums are reduced with one 32-value halving butterfly (31 shuffles instead of
-//     4 x 9) that leaves element `lane` in lane `lane`: grad_emb is written as one 128-byte row.
-// Selected by hidden_variant() below (NQB_HIDDEN_VARIANT / nqb_mlp_hidden_set_variant).
-// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float sigmoid(float p) { return rcp_approx(1.0f + ex2_approx(p * -1.4426950408889634f)); }
 
 struct Basis8 { float4 a, b; };
 __device__ __forceinline__ Basis8 load_basis(const float* __restrict__ emb, int64_t e, int64_t E) {
@@ -158,7 +62,7 @@ __device__ __forceinline__ void bcast_basis(const Basis8& mine, int j, float (&x
   x[4] = __shfl_sync(0xffffffffu, mine.b.x, j); x[5] = __shfl_sync(0xffffffffu, mine.b.y, j);
   x[6] = __shfl_sync(0xffffffffu, mine.b.z, j); x[7] = __shfl_sync(0xffffffffu, mine.b.w, j);
 }
-// pre-activations of this lane's 4 hidden units: p[q] = sum_k x[k] * W1s[k, m0 + q]  (k ascending, as v1)
+// pre-activations of this lane's 4 hidden units: p[q] = sum_k x[k] * W1s[k, m0 + q]  (k ascending)
 __device__ __forceinline__ void preact4(const float (&x)[NB], const float2 (&w01)[NB], const float2 (&w23)[NB],
                                         float2& p01, float2& p23) {
   p01 = make_float2(0.f, 0.f);
@@ -171,8 +75,8 @@ __device__ __forceinline__ void preact4(const float (&x)[NB], const float2 (&w01
   }
 }
 
-__global__ void __launch_bounds__(256) k_hidden_fwd2(const float* __restrict__ emb, const float* __restrict__ W1s,
-                                                     int64_t E, float* __restrict__ h) {
+__global__ void __launch_bounds__(256) k_hidden_fwd(const float* __restrict__ emb, const float* __restrict__ W1s,
+                                                    int64_t E, float* __restrict__ h) {
   const int lane = threadIdx.x & 31, m0 = lane * 4;
   float2 w01[NB], w23[NB];
 #pragma unroll
@@ -198,18 +102,18 @@ __global__ void __launch_bounds__(256) k_hidden_fwd2(const float* __restrict__ e
       float2 p01, p23;
       preact4(x, w01, w23, p01, p23);
       float4 o;
-      o.x = p01.x * sigmoid_v2(p01.x);
-      o.y = p01.y * sigmoid_v2(p01.y);
-      o.z = p23.x * sigmoid_v2(p23.x);
-      o.w = p23.y * sigmoid_v2(p23.y);
+      o.x = p01.x * sigmoid(p01.x);
+      o.y = p01.y * sigmoid(p01.y);
+      o.z = p23.x * sigmoid(p23.x);
+      o.w = p23.y * sigmoid(p23.y);
       __stcs(reinterpret_cast<float4*>(hrow + (int64_t)j * H), o);
     }
     cur = nxt;
   }
 }
 
-__global__ void __launch_bounds__(256) k_hidden_bwd2(const float* __restrict__ emb, const float* __restrict__ W1s,
-                                                     const float* __restrict__ gh, int64_t E, float* __restrict__ gemb) {
+__global__ void __launch_bounds__(256) k_hidden_bwd(const float* __restrict__ emb, const float* __restrict__ W1s,
+                                                    const float* __restrict__ gh, int64_t E, float* __restrict__ gemb) {
   const int lane = threadIdx.x & 31, m0 = lane * 4;
   float2 w01[NB], w23[NB];
 #pragma unroll
@@ -243,7 +147,7 @@ __global__ void __launch_bounds__(256) k_hidden_bwd2(const float* __restrict__ e
         float2 p01, p23;
         preact4(x, w01, w23, p01, p23);
         // gp[q] = grad_h[q] * silu'(p[q]),  silu'(p) = s (1 + p (1 - s))
-        const float s0 = sigmoid_v2(p01.x), s1 = sigmoid_v2(p01.y), s2 = sigmoid_v2(p23.x), s3 = sigmoid_v2(p23.y);
+        const float s0 = sigmoid(p01.x), s1 = sigmoid(p01.y), s2 = sigmoid(p23.x), s3 = sigmoid(p23.y);
         const float2 gp01 = make_float2(g[u].x * (s0 * fmaf(p01.x, 1.0f - s0, 1.0f)), g[u].y * (s1 * fmaf(p01.y, 1.0f - s1, 1.0f)));
         const float2 gp23 = make_float2(g[u].z * (s2 * fmaf(p23.x, 1.0f - s2, 1.0f)), g[u].w * (s3 * fmaf(p23.y, 1.0f - s3, 1.0f)));
 #pragma unroll
@@ -281,45 +185,10 @@ __global__ void __launch_bounds__(256) k_hidden_bwd2(const float* __restrict__ e
 extern "C" int nqb_set_error(const char* msg);  // defined in nqb_runtime.cu
 extern "C" void nqb_count_launch(void);
 
-// persistent grid: 8 CTAs of 256 threads per SM (or fewer when there is less work)
-static unsigned hidden_grid(int64_t threads) {
-  static int sms_dev[64] = {0};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  dev &= 63;
-  if (sms_dev[dev] == 0) {
-    cudaDeviceGetAttribute(&sms_dev[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sms_dev[dev] <= 0) sms_dev[dev] = 132;
-  }
-  const int sms = sms_dev[dev];
-  const int64_t need = (threads + 255) / 256, cap = (int64_t)sms * 8;
-  return (unsigned)(need < cap ? need : cap);
-}
-
-// Kernel generation: 2 = the batched kernels above, 1 = the round-1 kernels (kept for A/B timing and as the
-// reference of the v2 parity test).  Default NQB_HIDDEN_VARIANT_DEFAULT, overridden by the environment variable
-// NQB_HIDDEN_VARIANT or at run time by nqb_mlp_hidden_set_variant().
-#ifndef NQB_HIDDEN_VARIANT_DEFAULT
-#define NQB_HIDDEN_VARIANT_DEFAULT 2
-#endif
-static int g_hidden_variant = 0;  // 0 = not initialised
-static int hidden_variant() {
-  if (g_hidden_variant == 0) {
-    const char* e = getenv("NQB_HIDDEN_VARIANT");
-    g_hidden_variant = (e != nullptr && (e[0] == '1' || e[0] == '2')) ? (e[0] - '0') : NQB_HIDDEN_VARIANT_DEFAULT;
-  }
-  return g_hidden_variant;
-}
-extern "C" int nqb_mlp_hidden_set_variant(int variant) {  // returns the previous one; 0 = query only
-  const int prev = hidden_variant();
-  if (variant == 1 || variant == 2) g_hidden_variant = variant;
-  return prev;
-}
-
-// v2: persistent grid of exactly the resident CTAs (occupancy x SMs), so that a warp sees several batches and
+// persistent grid of exactly the resident CTAs (occupancy x SMs), so that a warp sees several batches and
 // its next batch is always prefetched; fewer CTAs when there are fewer batches than warps
 template <typename K>
-static unsigned hidden_grid2(K kernel, int which, int64_t E) {
+static unsigned hidden_grid(K kernel, int which, int64_t E) {
   static int ctas_dev[2][64] = {{0}, {0}};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -335,16 +204,12 @@ static unsigned hidden_grid2(K kernel, int which, int64_t E) {
 }
 
 extern "C" int nqb_mlp_hidden_fwd(const float* emb, const float* W1s, int64_t E, int num_bessel, int hidden, float* h,
-                                  float* h_lo, nqb_stream_t st) {
+                                  nqb_stream_t st) {
   if (num_bessel != NB || hidden != H) return nqb_set_error("nqb_mlp_hidden_fwd: only num_bessel=8, hidden=128 is built");
   if (E < 0) return nqb_set_error("nqb_mlp_hidden_fwd: negative size");
   if (E == 0) return 0;
   if (!emb || !W1s || !h) return nqb_set_error("nqb_mlp_hidden_fwd: null pointer");
-  const int64_t threads = E * 32;
-  if (hidden_variant() == 2 && h_lo == nullptr)
-    k_hidden_fwd2<<<hidden_grid2(k_hidden_fwd2, 0, E), 256, 0, (cudaStream_t)st>>>(emb, W1s, E, h);
-  else
-    k_hidden_fwd<<<hidden_grid(threads), 256, 0, (cudaStream_t)st>>>(emb, W1s, E, h, h_lo);
+  k_hidden_fwd<<<hidden_grid(k_hidden_fwd, 0, E), 256, 0, (cudaStream_t)st>>>(emb, W1s, E, h);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -357,11 +222,7 @@ extern "C" int nqb_mlp_hidden_bwd(const float* emb, const float* W1s, const floa
   if (E < 0) return nqb_set_error("nqb_mlp_hidden_bwd: negative size");
   if (E == 0) return 0;
   if (!emb || !W1s || !grad_h || !grad_emb) return nqb_set_error("nqb_mlp_hidden_bwd: null pointer");
-  const int64_t threads = E * 32;
-  if (hidden_variant() == 2)
-    k_hidden_bwd2<<<hidden_grid2(k_hidden_bwd2, 1, E), 256, 0, (cudaStream_t)st>>>(emb, W1s, grad_h, E, grad_emb);
-  else
-    k_hidden_bwd<<<hidden_grid(threads), 256, 0, (cudaStream_t)st>>>(emb, W1s, grad_h, E, grad_emb);
+  k_hidden_bwd<<<hidden_grid(k_hidden_bwd, 1, E), 256, 0, (cudaStream_t)st>>>(emb, W1s, grad_h, E, grad_emb);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));

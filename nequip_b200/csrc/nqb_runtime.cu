@@ -50,7 +50,7 @@ static int cuda_fail(cudaError_t e, const char* what) {
     if (e__ != cudaSuccess) return cuda_fail(e__, what);         \
   } while (0)
 
-extern "C" int nqb_abi_version(void) { return 1; }
+extern "C" int nqb_abi_version(void) { return 2; }
 // internal helpers shared with the other translation units of libnqb.so (not part of nqb.h)
 extern "C" int nqb_set_error(const char* msg) { return fail("%s", msg); }
 extern "C" void nqb_count_launch(void) { g_launches.fetch_add(1, std::memory_order_relaxed); }

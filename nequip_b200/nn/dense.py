@@ -146,18 +146,11 @@ class SelfConnectionGemm:
 # ---------------------------------------------------------------------------------------
 class _RadialMLPGemmFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, emb, w1s, fwd: ops.GroupedGemm, bwd: ops.GroupedGemm, W: int):
-        E, hid = emb.shape[0], w1s.shape[1]
-        fast = emb.shape[1] == 8 and hid == 128  # fused CUDA-core kernels for the K = 8 layer
-        if fast:
-            # (no pre-split low part: k_gemm3x computes it from the staged A chunk, which reads A once)
-            h = torch.empty((E, hid), dtype=emb.dtype, device=emb.device)
-            ops.mlp_hidden_fwd(emb, w1s, h, None)
-        else:
-            h = torch.nn.functional.silu(torch.mm(emb, w1s))
-        out = torch.empty((E, W), dtype=emb.dtype, device=emb.device)
-        fwd.run(h, out, E)
-        ctx.bwd, ctx.w1s, ctx.fast = bwd, w1s, fast
+    def forward(ctx, emb, mlp: "RadialMLPGemm"):
+        E = emb.shape[0]
+        out = torch.empty((E, mlp.W), dtype=emb.dtype, device=emb.device)
+        mlp.fwd.run(mlp.hidden(emb), out, E)
+        ctx.mlp = mlp
         ctx.save_for_backward(emb)  # the pre-activation is recomputed in the backward (8 FMAs per value)
         return out
 
@@ -165,16 +158,7 @@ class _RadialMLPGemmFn(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, gw):
         (emb,) = ctx.saved_tensors
-        E, hid = emb.shape[0], ctx.w1s.shape[1]
-        gh = torch.empty((E, hid), dtype=emb.dtype, device=emb.device)
-        ctx.bwd.run(gw.contiguous(), gh, E)
-        if ctx.fast:
-            gemb = torch.empty_like(emb)
-            ops.mlp_hidden_bwd(emb, ctx.w1s, gh, gemb)
-            return gemb, None, None, None, None
-        pre = torch.mm(emb, ctx.w1s)
-        gpre = torch.ops.aten.silu_backward(gh, pre)
-        return torch.mm(gpre, ctx.w1s.t()), None, None, None, None
+        return ctx.mlp.grad_emb(emb, gw), None
 
 
 class RadialMLPGemm:
@@ -185,13 +169,36 @@ class RadialMLPGemm:
         a2 = float(lin2.alpha)
         self.fwd = ops.GroupedGemm([ops.GemmProblem(0, hid, 0, W, lin2.weight.detach(), scale=a2)], device)
         self.bwd = ops.GroupedGemm([ops.GemmProblem(0, W, 0, hid, lin2.weight.detach(), scale=a2, transposed=True)], device)
+        # the CUDA-core hidden-layer kernels are built for [E, 8] x [8, 128] only; other widths run through torch
+        self._hidden_kernel = tuple(self.w1s.shape) == (8, 128)
 
     @staticmethod
     def supported(lin1, lin2, dtype) -> bool:
         return dtype == torch.float32 and lin2.weight.shape[0] % 4 == 0 and lin2.weight.shape[1] % 4 == 0
 
+    def hidden(self, emb):
+        """``h = silu(emb @ w1s)``."""
+        if self._hidden_kernel:
+            h = torch.empty((emb.shape[0], self.w1s.shape[1]), dtype=emb.dtype, device=emb.device)
+            ops.mlp_hidden_fwd(emb, self.w1s, h)
+            return h
+        return torch.nn.functional.silu(torch.mm(emb, self.w1s))
+
+    def grad_emb(self, emb, gw):
+        """Gradient of ``emb`` from the gradient ``gw`` of the edge weights: the transposed second-layer GEMM gives
+        ``grad_h``, then the hidden layer's backward (pre-activation recomputed)."""
+        E = emb.shape[0]
+        gh = torch.empty((E, self.w1s.shape[1]), dtype=emb.dtype, device=emb.device)
+        self.bwd.run(gw.contiguous(), gh, E)
+        if self._hidden_kernel:
+            gemb = torch.empty_like(emb)
+            ops.mlp_hidden_bwd(emb, self.w1s, gh, gemb)
+            return gemb
+        pre = torch.mm(emb, self.w1s)
+        return torch.mm(torch.ops.aten.silu_backward(gh, pre), self.w1s.t())
+
     def __call__(self, emb):
-        return _RadialMLPGemmFn.apply(emb.contiguous(), self.w1s, self.fwd, self.bwd, self.W)
+        return _RadialMLPGemmFn.apply(emb.contiguous(), self)
 
 
 # ---------------------------------------------------------------------------------------
@@ -202,12 +209,7 @@ class _FusedRadialTPFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, emb, x, y, edge_src, mod: "FusedRadialTP", csr):
-        E, hid = emb.shape[0], mod.w1s.shape[1]
-        if emb.shape[1] == 8 and hid == 128:
-            h = torch.empty((E, hid), dtype=emb.dtype, device=emb.device)
-            ops.mlp_hidden_fwd(emb, mod.w1s, h, None)
-        else:
-            h = torch.nn.functional.silu(torch.mm(emb, mod.w1s))
+        h = mod.mlp.hidden(emb)
         need_bwd = any(ctx.needs_input_grad[:3])
         out, w = ops.tp_fused_fwd(mod.fw, x, y, h, edge_src, csr, want_w=need_bwd)
         ctx.mod, ctx.csr = mod, csr
@@ -221,31 +223,20 @@ class _FusedRadialTPFn(torch.autograd.Function):
         emb, x, y, w, edge_src = ctx.saved_tensors
         mod = ctx.mod
         gx, gy, gw = ops.tp_scatter_bwd_raw(mod.plan, x, y, w, edge_src, ctx.csr, gout, need_x=ctx.needs_input_grad[1])
-        gemb = None
-        if ctx.needs_input_grad[0]:
-            E, hid = emb.shape[0], mod.w1s.shape[1]
-            gh = torch.empty((E, hid), dtype=emb.dtype, device=emb.device)
-            mod.bwd.run(gw, gh, E)
-            if emb.shape[1] == 8 and hid == 128:
-                gemb = torch.empty_like(emb)
-                ops.mlp_hidden_bwd(emb, mod.w1s, gh, gemb)
-            else:
-                pre = torch.mm(emb, mod.w1s)
-                gemb = torch.mm(torch.ops.aten.silu_backward(gh, pre), mod.w1s.t())
+        gemb = mod.mlp.grad_emb(emb, gw) if ctx.needs_input_grad[0] else None
         return gemb, gx, (gy if ctx.needs_input_grad[2] else None), None, None, None
 
 
 class FusedRadialTP:
     """Radial MLP (one hidden layer) + TensorProductScatter of one interaction layer as a single forward kernel
-    (``nqb_tp_fused_fwd``); backward = ``nqb_tp_scatter_bwd`` + the grouped GEMM for ``grad_h`` + the hidden layer."""
+    (``nqb_tp_fused_fwd``); backward = ``nqb_tp_scatter_bwd`` + the layer's ``RadialMLPGemm.grad_emb``."""
 
-    def __init__(self, lin1, lin2, plan: ops.TPPlan, device):
+    def __init__(self, mlp: RadialMLPGemm, lin2, plan: ops.TPPlan, device):
+        """``mlp``: the layer's unfused radial MLP (built from the same weights), whose hidden layer and backward GEMM
+        this kernel shares."""
         self.plan = plan
-        self.w1s = (lin1.weight.detach() * lin1.alpha).contiguous()
-        hid, W = lin2.weight.shape
-        a2 = float(lin2.alpha)
-        self.fw = ops.FusedTPWeights(plan, lin2.weight.detach(), a2, device)
-        self.bwd = ops.GroupedGemm([ops.GemmProblem(0, W, 0, hid, lin2.weight.detach(), scale=a2, transposed=True)], device)
+        self.mlp = mlp
+        self.fw = ops.FusedTPWeights(plan, lin2.weight.detach(), float(lin2.alpha), device)
 
     @staticmethod
     def supported(lin1, lin2, plan: ops.TPPlan, dtype) -> bool:

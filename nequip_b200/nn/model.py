@@ -358,7 +358,7 @@ class InteractionBlock(torch.nn.Module):
         if mode is True or mode is False:
             return mode
         if self._fused_choice is None:
-            if torch.cuda.is_current_stream_capturing() or tc["mlp"] is None:
+            if torch.cuda.is_current_stream_capturing():
                 return False
             with torch.no_grad():
                 def t(fn):
@@ -482,12 +482,12 @@ class InteractionBlock(torch.nn.Module):
             return None
         dev = x.device
         lins = [m for m in self.edge_mlp.mlp if isinstance(m, ScalarLinearLayer)]
-        mlp = None
+        mlp = fused = None
         if len(lins) == 2 and dense.RadialMLPGemm.supported(lins[0], lins[1], x.dtype):
             mlp = dense.RadialMLPGemm(lins[0], lins[1], dev)
-        fused = None
-        if len(lins) == 2 and dense.FusedRadialTP.supported(lins[0], lins[1], self.tp_scatter._plan, x.dtype):
-            fused = dense.FusedRadialTP(lins[0], lins[1], self.tp_scatter._plan, dev)
+            # FusedRadialTP.supported implies RadialMLPGemm.supported: the fused block shares the layer's mlp
+            if dense.FusedRadialTP.supported(lins[0], lins[1], self.tp_scatter._plan, x.dtype):
+                fused = dense.FusedRadialTP(mlp, lins[1], self.tp_scatter._plan, dev)
         blocks = dict(
             fused=fused,
             lin1=(dense.IrrepsLinearGemm(self.linear_1, dev, extra_scale=float(self.norm_const.view(-1)[0]))

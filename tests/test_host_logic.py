@@ -85,7 +85,7 @@ def test_generator_emits_packed_fma_source():
         assert len(re.findall(rf"\bw{p.idx}B = vloadw", src)) == 2
 
 
-def test_capi_exports_every_declared_symbol():
+def test_capi_matches_header_and_abi_version():
     header = open(os.path.join(ROOT, "include", "nqb.h")).read()
     header = re.sub(r"/\*.*?\*/", "", header, flags=re.S)
     declared = set(re.findall(r"\b(nqb_[a-z0-9_]+)\s*\(", header))
@@ -94,7 +94,18 @@ def test_capi_exports_every_declared_symbol():
     for name in sorted(declared):
         assert hasattr(lib, name), f"libnqb.so does not export {name}"
     assert declared == set(_capi.SIGNATURES), declared ^ set(_capi.SIGNATURES)
-    assert _capi.lib().nqb_abi_version() == 1
+    assert _capi.lib().nqb_abi_version() == 2
+
+
+def test_hidden_layer_compatibility_arguments():
+    """bench.py calls ``mlp_hidden_fwd(emb, w1s, h, None)`` and reports ``"v%d" % mlp_hidden_variant(0)``."""
+    from nequip_b200 import ops
+
+    assert ops.mlp_hidden_variant(0) == ops.mlp_hidden_variant() == ops.mlp_hidden_variant(2) == 2
+    with pytest.raises(ValueError):
+        ops.mlp_hidden_variant(1)
+    with pytest.raises(ValueError):
+        ops.mlp_hidden_fwd(torch.zeros(1, 8), torch.zeros(8, 128), torch.zeros(1, 128), torch.zeros(1, 128))
 
 
 def test_plan_create_validates_signature():

@@ -23,13 +23,6 @@ def timeit(fn, reps=8, warm=2):
     return e0.elapsed_time(e1) / reps
 
 
-def tf32_lo(a):
-    """rna_tf32(a - trunc_tf32(a)) with integer bit operations (what nqb_mlp_hidden_fwd writes as h_lo)."""
-    hi = (a.view(torch.int32) & -8192).view(torch.float32)
-    lo = a - hi
-    return ((lo.view(torch.int32) + 4096) & -8192).view(torch.float32)
-
-
 def main():
     import argparse
 
@@ -37,7 +30,6 @@ def main():
     ap.add_argument("--scale", type=float, default=1.0)
     ap.add_argument("--cases", default="")
     ap.add_argument("--no-cublas", action="store_true")
-    ap.add_argument("--presplit", action="store_true", help="also hand the kernel pre-split low parts of A")
     args = ap.parse_args()
     torch.backends.cuda.matmul.allow_tf32 = False
     E, Nat = int(588616 * args.scale), int(10648 * args.scale)
@@ -51,14 +43,10 @@ def main():
         C = torch.empty(M, N, device="cuda")
         gg = ops.GroupedGemm([ops.GemmProblem(0, K, 0, N, B)], "cuda")
         ms = timeit(lambda: gg.run(A, C, M))
-        ms0 = ms
-        if args.presplit:
-            A_lo = tf32_lo(A)
-            ms = timeit(lambda: gg.run(A, C, M, a_lo=A_lo))
         ref = A[:4096].double() @ B.double()
         err = float((C[:4096].double() - ref).abs().max() / ref.abs().max())
         ms_t = 0.0 if args.no_cublas else timeit(lambda: torch.mm(A, B, out=C), reps=3, warm=1)
-        print(json.dumps({"case": name, "M": M, "K": K, "N": N, "ms": round(ms, 4), "ms_computed_lo": (round(ms0, 4) if args.presplit else None), "cublas_fp32_ms": round(ms_t, 4),
+        print(json.dumps({"case": name, "M": M, "K": K, "N": N, "ms": round(ms, 4), "cublas_fp32_ms": round(ms_t, 4),
                           "TFLOPs_fp32_equiv": round(2.0 * M * K * N / ms / 1e9, 1),
                           "io_GBps": round((M * K + M * N) * 4 / ms / 1e6, 1), "rel_err": err}), flush=True)
         del A, B, C
