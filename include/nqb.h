@@ -73,15 +73,19 @@ int nqb_plan_signature(const nqb_plan* plan, char* buf, int buflen);
 
 /* Destination-CSR helpers.  edge_dst must be non-decreasing for
  * nqb_csr_from_sorted (the reference's neighbour lists are grouped by centre atom);
- * nqb_csr_check_sorted writes 1/0 into *flag_dev.  For unsorted edges the caller
- * supplies perm (stable argsort of edge_dst) and the sorted keys. */
+ * nqb_csr_check_sorted writes 1/0 into *flag_dev (fully written).  For unsorted edges the caller
+ * supplies perm (stable argsort of edge_dst) and the sorted keys.
+ * row_ptr [N+1] is fully written (row_ptr[n] = first slot whose key >= n; E = 0 gives all zeros). */
 int nqb_csr_check_sorted(const int64_t* keys, int64_t E, int32_t* flag_dev, nqb_stream_t st);
 int nqb_csr_from_sorted(const int64_t* sorted_keys, int64_t E, int64_t N, int64_t* row_ptr /* [N+1] */,
                         nqb_stream_t st);
 
 /* out[N, D_mid] = scatter_dst( TP_uvu( x[src], y, w ) ).  Every element of out is
  * written exactly once (no pre-zeroing needed, deterministic).
- *   x [N, D_in], y [E, S], w [E, W], out [N, D_mid]: dtype NQB_F32/NQB_F64, row-major, mul_ir layout
+ *   x [N, D_in], y [E, S], w [E, W], out [N, D_mid]: dtype NQB_F32/NQB_F64, row-major, in the layout the plan's
+ *   kernel library was generated for (mul_ir or ir_mul, nequip_b200/codegen.py GenOptions.layout).
+ *   out is fully written, also for nodes without edges (E = 0 included) and in irreps_out chunks no instruction
+ *   writes (zeros).
  *   row_ptr [N+1]: CSR over edges ordered by destination; perm [E] or NULL (identity):
  *   slot s of the CSR refers to edge perm[s]; src [E]: source node of each edge (original order). */
 int nqb_tp_scatter_fwd(const nqb_plan* plan, int dtype, const void* x, const void* y, const void* w,
@@ -90,7 +94,8 @@ int nqb_tp_scatter_fwd(const nqb_plan* plan, int dtype, const void* x, const voi
 
 /* Gradients of the above.  grad_w [E, W] is fully written.  grad_y [E, S] and
  * grad_x [N, D_in] are ACCUMULATED INTO (caller zero-fills); grad_x may be NULL
- * (skips the source-row reduction, e.g. first layer at inference). */
+ * (skips the source-row reduction, e.g. first layer at inference; grad_y and grad_w are the same as with it).
+ * E = 0 writes nothing (grad_w has no rows). */
 int nqb_tp_scatter_bwd(const nqb_plan* plan, int dtype, const void* x, const void* y, const void* w,
                        const int64_t* row_ptr, const int64_t* perm, const int64_t* src,
                        const void* grad_out, int64_t N, int64_t E, void* grad_x, void* grad_y,
@@ -98,19 +103,21 @@ int nqb_tp_scatter_bwd(const nqb_plan* plan, int dtype, const void* x, const voi
                        nqb_stream_t st);
 /* deterministic != 0 (bitwise-repeatable backward; the default accumulates grad_x / grad_Y with red.global.add in
  * whatever order the edges retire, as the reference's OpenEquivariance back-end does, nequip/nn/_tp_scatter_oeq.py:46):
- *   grad_x is then an [E, D_in] buffer -- every edge stores its contribution to its SOURCE atom in its own row -- to be
+ *   grad_x is then an [E, D_in] buffer, FULLY WRITTEN -- every edge stores its contribution to its SOURCE atom in its
+ *   own row, zeros in the columns of irreps_in1 chunks no instruction reads -- to be
  *   reduced over the source-sorted edges with nqb_segment_sum (perm = stable argsort of edge_src, the
  *   edge_transpose_perm of nequip/data/transforms/neighborlist.py:150-155; seg_ptr = CSR over the sorted sources);
- *   grad_y is [nqb_tp_scatter_gy_slices(plan, dtype), E, S], zero-initialised by the caller: each writer owns a slice,
- *   the caller sums the slices in index order. */
+ *   grad_y is [nqb_tp_scatter_gy_slices(plan, dtype), E, S], ACCUMULATED INTO (zero-initialised by the caller): each
+ *   writer owns a slice, the caller sums the slices in index order.
+ * nqb_segment_sum: out [N, D] is fully written (a segment without rows gives 0). */
 int nqb_tp_scatter_gy_slices(const nqb_plan* plan, int dtype);
 int nqb_segment_sum(int dtype, const void* rows /* [R, D] */, int D, const int64_t* perm, const int64_t* seg_ptr /* [N+1] */,
                     int64_t N, void* out /* [N, D] */, nqb_stream_t st);
 
 /* Real spherical harmonics, "component" normalisation, input normalised (lmax <= 4).
- *   vec [E,3] f64 -> y [E,(lmax+1)^2] of out_dtype (computed in f64, then cast). */
+ *   vec [E,3] f64 -> y [E,(lmax+1)^2] of out_dtype (computed in f64, then cast); y is fully written. */
 int nqb_sh_fwd(int lmax, const double* vec, int64_t E, int out_dtype, void* y, nqb_stream_t st);
-/*   grad_vec [E,3] f64 = J^T grad_y (includes the normalisation Jacobian); overwritten */
+/*   grad_vec [E,3] f64 = J^T grad_y (includes the normalisation Jacobian); fully written */
 int nqb_sh_bwd(int lmax, const double* vec, int64_t E, int out_dtype, const void* grad_y,
                double* grad_vec, nqb_stream_t st);
 
@@ -119,6 +126,8 @@ int nqb_sh_bwd(int lmax, const double* vec, int64_t E, int out_dtype, const void
  * i.e. nequip/nn/mlp.py:262-268 (the last ScalarLinearLayer built at nequip/nn/interaction_block.py:119-127)
  * composed with TensorProductScatter.forward (nequip/nn/_tp_scatter_base.py:35-38) so that the [E, W] weight
  * tensor is never written (w_out == NULL) -- or is written once on the side for an unfused backward.
+ * out [N, D_mid] is fully written (nodes without edges and E = 0 included); w_out [E, W], when given, is fully
+ * written.  h [E, ldh] is read in its first K columns only; h must be 16-byte aligned.
  * float32, ir_mul node layout, edges grouped by destination (row_ptr; no permutation), K <= 128, K % 8 == 0.
  * nqb_tp_fused_slices(plan): number of 128-row weight slices of the signature, 0 = no fused kernel built.
  * w2_prepared: per slice, the tf32 hi and lo parts of the [128 x 128] block W2^T (rows = the slice's columns of the
@@ -131,25 +140,18 @@ int nqb_tp_fused_fwd(const nqb_plan* plan, const float* x, const float* y, const
                      const float* w2_prepared, const int64_t* row_ptr, const int64_t* src, int64_t N, int64_t E,
                      float* out, float* w_out, const int32_t* slice_cta0, int nctas, nqb_stream_t st);
 
-/* Real spherical harmonics, "component" normalisation, input normalised (lmax <= 4).
- *   vec [E,3] f64 -> y [E,(lmax+1)^2] of out_dtype (computed in f64, then cast). */
-int nqb_sh_fwd(int lmax, const double* vec, int64_t E, int out_dtype, void* y, nqb_stream_t st);
-/*   grad_vec [E,3] f64 = J^T grad_y (includes the normalisation Jacobian); overwritten */
-int nqb_sh_bwd(int lmax, const double* vec, int64_t E, int out_dtype, const void* grad_y,
-               double* grad_vec, nqb_stream_t st);
-
 /* Fused edge geometry + embeddings:
  *   r_ij = pos[idx1] - pos[idx0] + shift @ cell ; Y = SH(r_ij) ;
  *   emb[:, n] = sinc(n x) n * f_cut(x) * prefactor , x = |r|/r_max, n = 1..num_bessel
  * edge_index [2,E] i64; shift [E,3] f64 or NULL; cell [3,3] f64 (rows = lattice vectors) or NULL.
- * Outputs: vec [E,3] f64 (kept for backward), y [E,S], emb [E,num_bessel] (out_dtype). */
+ * Outputs, each fully written: vec [E,3] f64 (kept for backward), y [E,S], emb [E,num_bessel] (out_dtype). */
 int nqb_edge_embed_fwd(int lmax, int num_bessel, double r_max, double poly_p, double prefactor,
                        const double* pos, const int64_t* edge_index, const double* shift,
                        const double* cell, int64_t N, int64_t E, int out_dtype, double* vec, void* y,
                        void* emb, nqb_stream_t st);
 /* grad_pos [N,3] f64 is ACCUMULATED INTO (caller zero-fills):
  *   g = J_Y^T grad_y + J_emb^T grad_emb ;  grad_pos[idx1] += g ; grad_pos[idx0] -= g.
- * grad_vec [E,3] f64 (may be NULL) receives g itself (per-edge forces / virial assembly). */
+ * grad_vec [E,3] f64 (may be NULL) receives g itself (per-edge forces / virial assembly); fully written. */
 int nqb_edge_embed_bwd(int lmax, int num_bessel, double r_max, double poly_p, double prefactor,
                        const double* vec, const int64_t* edge_index, int64_t N, int64_t E,
                        int out_dtype, const void* grad_y, const void* grad_emb, double* grad_pos,
@@ -177,7 +179,8 @@ int nqb_nl_fill(int64_t N, int64_t E, const double* cell_host, const double* inv
 
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).
- * Together with nqb_gemm_grouped for the second layer this is ScalarMLPFunction (nequip/nn/mlp.py:80-195). */
+ * Together with nqb_gemm_grouped for the second layer this is ScalarMLPFunction (nequip/nn/mlp.py:80-195).
+ * h [E, hidden] and grad_emb [E, num_bessel] are fully written. */
 int nqb_mlp_hidden_fwd(const float* emb, const float* W1s, int64_t E, int num_bessel, int hidden, float* h,
                        nqb_stream_t st);
 int nqb_mlp_hidden_bwd(const float* emb, const float* W1s, const float* grad_h, int64_t E, int num_bessel,
@@ -191,10 +194,14 @@ int nqb_mlp_hidden_bwd(const float* emb, const float* W1s, const float* grad_h, 
  * descs_dev: device array of ndesc records of 12 int64:
  *   {a_off, c_off, b_off, rs_off (row of the [R, rs_ld] row-scale matrix, -1 = none), lda, ldc, K, N, kchunks=ceil(K/32), ntiles=ceil(N/128),
  *    tile0 (prefix sum of ntiles), flags};  offsets in floats from the bases.
- *   flags: bit0 C += (one writer per element within the launch), bit1 rows whose row scale is 0 are left
- *   untouched (disjoint row-masked writers), bit2 C += with red.global.add (several problems add into the same C).
- * Requirements: K, N, lda, ldc, a_off, c_off multiples of 4; bases 16-byte aligned.
- * B_p is prepared once (split hi/lo, tiled) with nqb_gemm_prepare into nqb_gemm_prepared_floats(K,N) floats.
+ *   flags: none: C is fully written (rows < M, columns < N_p); bit0 C is ACCUMULATED INTO (one writer per element
+ *   within the launch); bit1 rows whose row scale is 0 are left untouched (disjoint row-masked writers); bit2 C is
+ *   ACCUMULATED INTO with red.global.add (several problems add into the same C).  Nothing outside rows < M,
+ *   columns [c_off + m * ldc, + N_p) is written; A is read in rows < M, columns < K_p only.  M = 0 writes nothing.
+ * Requirements: K, N, lda, ldc, a_off, c_off multiples of 4; a_base, prepared_base, c_base 16-byte aligned
+ * (checked: an error, no launch).
+ * B_p is prepared once (split hi/lo, tiled) with nqb_gemm_prepare into nqb_gemm_prepared_floats(K,N) floats
+ * (fully written).
  * tile_ctas_dev (nullable): int32 {first CTA, CTAs} per N-tile -- a cost-weighted split of sched_ctas CTAs over
  * the N-tiles computed by the host (problems of one launch differ in K, N and store mode); used when
  * sched_ctas <= #SMs, otherwise the even split is used. */
@@ -212,7 +219,8 @@ int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_total, const i
  *     out[n,j] = gate[j] < 0 ? act(x[n,src[j]]) : x[n,src[j]] * act(x[n,gate[j]])
  *   backward, per INPUT column i: tab[6*i..] = {role, a, b, c, d, kind}
  *     role 0 scalar (a = output column); role 1 gated value (a = output column, b = gate input column);
- *     role 2 gate (a = first output column, b = first gated input column, c = component stride, d = 2l+1). */
+ *     role 2 gate (a = first output column, b = first gated input column, c = component stride, d = 2l+1).
+ * out [N, d_out] and grad_x [N, d_in] are fully written. */
 int nqb_gate_fwd(int dtype, const void* x, int64_t N, int d_in, int d_out, const int32_t* src,
                  const int32_t* gate, const int32_t* kind, void* out, nqb_stream_t st);
 int nqb_gate_bwd(int dtype, const void* x, const void* grad_out, int64_t N, int d_in, int d_out,

@@ -373,6 +373,9 @@ extern "C" int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_tot
   if (M < 0) return nqb_set_error("nqb_gemm_grouped: negative M");
   if (M == 0) return 0;
   if (!descs_dev || !a_base || !prepared_base || !c_base) return nqb_set_error("nqb_gemm_grouped: null pointer");
+  // A is staged with 16-byte cp.async, the weights with bulk copies, C is stored in float2 pairs
+  if (((uintptr_t)a_base | (uintptr_t)prepared_base | (uintptr_t)c_base) & 15)
+    return nqb_set_error("nqb_gemm_grouped: a_base, prepared_base and c_base must be 16-byte aligned");
   static bool attr_set[64] = {false};
   const int dev = gemm_device();
   if (!attr_set[dev]) {

@@ -24,6 +24,7 @@
 
 #include <atomic>
 #include <string>
+#include <vector>
 
 #include "../../include/nqb.h"
 
@@ -82,6 +83,9 @@ struct nqb_plan {
   spec_fused_fwd_fn fused_fwd = nullptr;  // null: the signature has no fused radial-MLP + TP kernel
   int fused_nslice = 0;
   int d_in, s_dim, w_numel, d_out;
+  // {first column, columns} of the irreps_in1 chunks no instruction reads: the kernels never touch them, so the
+  // deterministic backward zero-fills them in its per-edge grad_x buffer
+  std::vector<std::pair<int, int>> unread_in1;
 };
 
 static void append_irreps(std::string& s, const nqb_irrep* ir, int n) {
@@ -142,6 +146,11 @@ extern "C" int nqb_plan_create(const nqb_irrep* in1, int n_in1, const nqb_irrep*
   p->fwd = ffwd;
   p->bwd = fbwd;
   fdims(&p->d_in, &p->s_dim, &p->w_numel, &p->d_out);
+  for (int i = 0, off = 0; i < n_in1; off += in1[i].mul * (2 * in1[i].l + 1), ++i) {
+    bool read = false;
+    for (int k = 0; k < n_ins; ++k) read |= ins[k].i_in1 == i;
+    if (!read) p->unread_in1.push_back({off, in1[i].mul * (2 * in1[i].l + 1)});
+  }
   p->gy_slices = (spec_gy_slices_fn)dlsym(lib, "nqb_spec_gy_slices");
   spec_fused_info_fn finfo = (spec_fused_info_fn)dlsym(lib, "nqb_spec_fused_info");
   spec_fused_fwd_fn ffused = (spec_fused_fwd_fn)dlsym(lib, "nqb_spec_fused_fwd");
@@ -203,6 +212,15 @@ extern "C" int nqb_tp_scatter_bwd(const nqb_plan* plan, int dtype, const void* x
   if (!row_ptr || !x || !y || !w || !src || !grad_out || !grad_y || !grad_w)
     return fail("nqb_tp_scatter_bwd: null pointer argument");
   if (deterministic && !plan->gy_slices) return fail("nqb_tp_scatter_bwd: kernel library has no deterministic mode");
+  if (deterministic && grad_x) {
+    // the per-edge grad_x buffer is fully written: zeros in the columns of chunks no instruction reads
+    const size_t esz = dtype == NQB_F32 ? sizeof(float) : sizeof(double);
+    for (const auto& c : plan->unread_in1) {
+      cudaError_t e = cudaMemset2DAsync((char*)grad_x + c.first * esz, plan->d_in * esz, 0, c.second * esz, (size_t)E,
+                                        (cudaStream_t)st);
+      if (e != cudaSuccess) return cuda_fail(e, "nqb_tp_scatter_bwd: zero fill of unread grad_x columns");
+    }
+  }
   int rc = plan->bwd(dtype, x, y, w, row_ptr, perm, src, grad_out, N, E, grad_x, grad_y, grad_w, deterministic ? 1 : 0,
                      (cudaStream_t)st);
   g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -259,6 +277,8 @@ extern "C" int nqb_tp_fused_fwd(const nqb_plan* plan, const float* x, const floa
   if (!row_ptr || !out || !w2_prepared || !slice_cta0 || (E > 0 && (!x || !y || !h || !src)))
     return fail("nqb_tp_fused_fwd: null pointer argument");
   if (K <= 0 || K > 128 || (K % 8) || (ldh % 4) || ldh < K) return fail("nqb_tp_fused_fwd: needs 0 < K <= 128, K %% 8 == 0, ldh %% 4 == 0");
+  // h rows are staged with 16-byte cp.async
+  if (E > 0 && ((uintptr_t)h & 15)) return fail("nqb_tp_fused_fwd: h must be 16-byte aligned");
   if (nctas <= 0) return fail("nqb_tp_fused_fwd: empty grid");
   int rc = plan->fused_fwd(x, y, h, ldh, K, w2_prepared, row_ptr, src, N, E, out, w_out, slice_cta0, nctas, (cudaStream_t)st);
   g_launches.fetch_add(1, std::memory_order_relaxed);
