@@ -176,6 +176,24 @@ int nqb_nl_fill(int64_t N, int64_t E, const double* cell_host, const double* inv
                 const int* search, double r_max, const double* wpos, const int32_t* cidx, const int32_t* base,
                 const int64_t* order, const int64_t* bin_start, const int64_t* row_ptr /* [N+1] */,
                 int64_t* edge_index /* [2,E] */, double* shifts /* [E,3] */, nqb_stream_t st);
+/* Capacity mode: a list of fixed length `capacity` whatever the frame's edge count E, so positions -> list -> model
+ * is capturable in one CUDA graph (no host read of E).  Unused slots hold null edges (i, i, pad_shift): a self-edge
+ * to a periodic image at least r_max + one lattice vector away, which contributes exactly zero energy and force.
+ * nqb_nl_pad runs after the exclusive scan (row_ptr [N+1] of the exact list, N > 0):
+ *   row_ptr_pad [N+1] fully written: row_ptr[i] + floor((capacity - E) * i / N), row_ptr_pad[N] = capacity, so
+ *   every row gets floor or ceil of (capacity - E) / N null edges; when E > capacity, floor(capacity * i / N);
+ *   num_edges [1] fully written: the true E (also on overflow); overflow [1] fully written: 1 if E > capacity, else 0. */
+int nqb_nl_pad(int64_t N, int64_t capacity, const int64_t* row_ptr, int64_t* row_ptr_pad, int64_t* num_edges,
+               int32_t* overflow, nqb_stream_t st);
+/* edge_index [2,capacity] and shifts [capacity,3] fully written, nothing past capacity: row i holds
+ * [row_ptr_pad[i], row_ptr_pad[i+1]), its real edges first (order and shifts as nqb_nl_fill; none on overflow), then
+ * null edges (i, i, pad_shift).  pad_shift: 3 integer-valued doubles on the HOST; overflow: device flag of nqb_nl_pad. */
+int nqb_nl_fill_capacity(int64_t N, int64_t capacity, const double* cell_host, const double* inv_host, const int* pbc,
+                         const int* nbins, const int* search, double r_max, const double* wpos, const int32_t* cidx,
+                         const int32_t* base, const int64_t* order, const int64_t* bin_start,
+                         const int64_t* row_ptr_pad /* [N+1] */, const int32_t* overflow /* [1] */,
+                         const double* pad_shift_host, int64_t* edge_index /* [2,capacity] */,
+                         double* shifts /* [capacity,3] */, nqb_stream_t st);
 
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).

@@ -50,6 +50,9 @@ SIGNATURES = {
     "nqb_nl_bin": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp]),
     "nqb_nl_count": (_i32, [_i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nqb_nl_fill": (_i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nl_pad": (_i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nl_fill_capacity": (
+        _i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nqb_sh_fwd": (_i32, [_i32, _vp, _i64, _i32, _vp, _vp]),
     "nqb_sh_bwd": (_i32, [_i32, _vp, _i64, _i32, _vp, _vp, _vp]),
     "nqb_edge_embed_fwd": (

@@ -136,30 +136,63 @@ __device__ __forceinline__ bool nl_less(int64_t ja, const double* sa, int64_t jb
   return sa[2] < sb[2];
 }
 
+// kCapacity = false: the row's edges go to [row_ptr[i], row_ptr[i + 1]) of an exactly sized list (nqb_nl_fill).
+// kCapacity = true (nqb_nl_fill_capacity): the row owns [row_ptr_pad[i], row_ptr_pad[i + 1]) of a list of E = capacity
+// slots; its real edges come first (same order and shifts as above, none when *overflow is set) and the remaining slots
+// hold null edges (i, i, pad_shift).  The trailing parameters are appended so the unpadded variant's code is unchanged.
+template <bool kCapacity>
 __global__ void k_nl_fill(NlParams p, int64_t N, const double* __restrict__ wpos, const int32_t* __restrict__ cidx,
                           const int32_t* __restrict__ base, const int64_t* __restrict__ order,
                           const int64_t* __restrict__ bin_start, const int64_t* __restrict__ row_ptr, int64_t E,
-                          int64_t* __restrict__ edge_index, double* __restrict__ shifts) {
+                          int64_t* __restrict__ edge_index, double* __restrict__ shifts,
+                          const int32_t* __restrict__ overflow, double3 pad_shift) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   const int64_t beg = row_ptr[i];
   int64_t n = 0;
   int64_t* ej = edge_index + E;  // neighbours (row 1)
-  nl_visit(p, i, wpos, cidx, order, bin_start, [&](int64_t j, int ix, int iy, int iz) {
-    // insertion into the sorted prefix of the row (rows hold a few dozen neighbours)
-    double s[3] = {(double)(ix + base[3 * j] - base[3 * i]), (double)(iy + base[3 * j + 1] - base[3 * i + 1]),
-                   (double)(iz + base[3 * j + 2] - base[3 * i + 2])};
-    int64_t q = beg + n;
-    while (q > beg && nl_less(j, s, ej[q - 1], shifts + 3 * (q - 1))) {
-      ej[q] = ej[q - 1];
-      shifts[3 * q] = shifts[3 * (q - 1)]; shifts[3 * q + 1] = shifts[3 * (q - 1) + 1]; shifts[3 * q + 2] = shifts[3 * (q - 1) + 2];
-      --q;
+  if (!kCapacity || *overflow == 0) {
+    nl_visit(p, i, wpos, cidx, order, bin_start, [&](int64_t j, int ix, int iy, int iz) {
+      // insertion into the sorted prefix of the row (rows hold a few dozen neighbours)
+      double s[3] = {(double)(ix + base[3 * j] - base[3 * i]), (double)(iy + base[3 * j + 1] - base[3 * i + 1]),
+                     (double)(iz + base[3 * j + 2] - base[3 * i + 2])};
+      int64_t q = beg + n;
+      while (q > beg && nl_less(j, s, ej[q - 1], shifts + 3 * (q - 1))) {
+        ej[q] = ej[q - 1];
+        shifts[3 * q] = shifts[3 * (q - 1)]; shifts[3 * q + 1] = shifts[3 * (q - 1) + 1]; shifts[3 * q + 2] = shifts[3 * (q - 1) + 2];
+        --q;
+      }
+      ej[q] = j;
+      shifts[3 * q] = s[0]; shifts[3 * q + 1] = s[1]; shifts[3 * q + 2] = s[2];
+      edge_index[beg + n] = i;
+      ++n;
+    });
+  }
+  if (kCapacity) {
+    const int64_t end = row_ptr[i + 1];
+    for (int64_t q = beg + n; q < end; ++q) {
+      edge_index[q] = i;
+      ej[q] = i;
+      shifts[3 * q] = pad_shift.x; shifts[3 * q + 1] = pad_shift.y; shifts[3 * q + 2] = pad_shift.z;
     }
-    ej[q] = j;
-    shifts[3 * q] = s[0]; shifts[3 * q + 1] = s[1]; shifts[3 * q + 2] = s[2];
-    edge_index[beg + n] = i;
-    ++n;
-  });
+  }
+}
+
+// Padded row pointer of the capacity mode (one thread per entry of [0, N]).  E = row_ptr[N] real edges; each row gets
+// floor or ceil of (capacity - E) / N null edges: row_ptr_pad[i] = row_ptr[i] + floor((capacity - E) i / N).  When
+// E > capacity, every row holds only null edges: row_ptr_pad[i] = floor(capacity i / N).
+__global__ void k_nl_pad(int64_t N, int64_t capacity, const int64_t* __restrict__ row_ptr,
+                         int64_t* __restrict__ row_ptr_pad, int64_t* __restrict__ num_edges,
+                         int32_t* __restrict__ overflow) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > N) return;
+  const int64_t E = row_ptr[N];
+  const bool over = E > capacity;
+  row_ptr_pad[i] = over ? capacity * i / N : row_ptr[i] + (capacity - E) * i / N;
+  if (i == 0) {
+    *num_edges = E;
+    *overflow = over ? 1 : 0;
+  }
 }
 
 }  // namespace
@@ -227,8 +260,45 @@ extern "C" int nqb_nl_fill(int64_t N, int64_t E, const double* cell_host, const 
     return nqb_set_error("nqb_nl_fill: null pointer");
   NlParams p;
   nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
-  k_nl_fill<<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(p, N, wpos, cidx, base, order, bin_start, row_ptr, E,
-                                                                    edge_index, shifts);
+  k_nl_fill<false><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(p, N, wpos, cidx, base, order, bin_start,
+                                                                           row_ptr, E, edge_index, shifts, nullptr,
+                                                                           make_double3(0.0, 0.0, 0.0));
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+// Capacity mode, step 3a: padded row pointer, true edge count and overflow flag from the exact row pointer.
+extern "C" int nqb_nl_pad(int64_t N, int64_t capacity, const int64_t* row_ptr, int64_t* row_ptr_pad, int64_t* num_edges,
+                          int32_t* overflow, nqb_stream_t st) {
+  if (N <= 0 || capacity < 0) return nqb_set_error("nqb_nl_pad: needs N > 0 and capacity >= 0");
+  if (!row_ptr || !row_ptr_pad || !num_edges || !overflow) return nqb_set_error("nqb_nl_pad: null pointer");
+  k_nl_pad<<<(unsigned)((N + 1 + 127) / 128), 128, 0, (cudaStream_t)st>>>(N, capacity, row_ptr, row_ptr_pad, num_edges,
+                                                                          overflow);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+// Capacity mode, step 3b: fill a [2, capacity] list along row_ptr_pad (from nqb_nl_pad); pad_shift: 3 doubles on the HOST.
+extern "C" int nqb_nl_fill_capacity(int64_t N, int64_t capacity, const double* cell_host, const double* inv_host,
+                                    const int* pbc, const int* nbins, const int* search, double r_max, const double* wpos,
+                                    const int32_t* cidx, const int32_t* base, const int64_t* order,
+                                    const int64_t* bin_start, const int64_t* row_ptr_pad, const int32_t* overflow,
+                                    const double* pad_shift_host, int64_t* edge_index, double* shifts, nqb_stream_t st) {
+  if (N <= 0 || capacity < 0) return nqb_set_error("nqb_nl_fill_capacity: needs N > 0 and capacity >= 0");
+  if (capacity == 0) return 0;
+  if (!wpos || !cidx || !base || !order || !bin_start || !row_ptr_pad || !overflow || !pad_shift_host || !edge_index ||
+      !shifts)
+    return nqb_set_error("nqb_nl_fill_capacity: null pointer");
+  NlParams p;
+  nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
+  const double3 ps = make_double3(pad_shift_host[0], pad_shift_host[1], pad_shift_host[2]);
+  k_nl_fill<true><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(p, N, wpos, cidx, base, order, bin_start,
+                                                                          row_ptr_pad, capacity, edge_index, shifts,
+                                                                          overflow, ps);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));

@@ -204,5 +204,14 @@ def replicate_frame(data: Dict[str, torch.Tensor], copies: int, r_max: float = 5
     }
 
 
+def oscillating_positions(pos0: torch.Tensor, t: int, period: int = 50, amplitude: float = 0.2, seed: int = 0) -> torch.Tensor:
+    """Step ``t`` of a bounded MD-like trajectory: ``pos0 + amplitude * sin(2 pi t / period + phi)``, one seeded phase
+    per atom and direction.  Edges cross the cutoff at most steps, and unlike a trajectory integrated with a
+    random-weight model's forces, it stays physical for any number of steps."""
+    g = torch.Generator().manual_seed(seed)
+    phi = (2 * np.pi) * torch.rand(tuple(pos0.shape), generator=g, dtype=torch.float64).to(pos0.device)
+    return pos0 + amplitude * torch.sin(2 * np.pi * t / period + phi)
+
+
 def to_device(data: Dict, device) -> Dict:
     return {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in data.items()}

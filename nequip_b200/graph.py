@@ -12,9 +12,15 @@ A graph is valid for one (num_atoms, num_edges) pair and for edge lists grouped 
 reference's neighbour lists produce, nequip/data/transforms/neighborlist.py:120-157); the sortedness flag
 is computed inside the graph and verified when the results are read.  Anything else: use the eager
 ``model(data)`` call (same kernels, more launch overhead).
+
+``GraphedMDStep`` lifts the shape restriction for molecular dynamics in a fixed periodic cell: the device neighbour
+list (``ops.NeighborListPlan``) is part of the graph and writes a list of fixed length ``capacity`` whose unused
+slots hold null edges, which contribute exactly zero (DESIGN.md section 4.8).  So one graph replays every step
+whatever the step's edge count, and a step that needs more than ``capacity`` edges is re-captured.
 """
 from __future__ import annotations
 
+import math
 from typing import Dict, Optional
 
 import torch
@@ -132,3 +138,84 @@ class GraphedShardedEnergyForces(GraphedEnergyForces):
         d.update(self.static)
         e, f = P.sharded_energy_forces(self.model, d, self.plan, self.halo, reduce_forces="owner")
         return {"total_energy": e, "forces": f}
+
+
+#: default edge capacity of GraphedMDStep: E0 * (1 + CAPACITY_SLACK), E0 = the example frame's edge count
+CAPACITY_SLACK = 0.02
+
+
+class GraphedMDStep(GraphedEnergyForces):
+    """One CUDA graph for a whole MD step in a fixed periodic cell: positions -> device neighbour list -> energy ->
+    forces.  ``g = GraphedMDStep(model, example); out = g(pos)``.
+
+    ``example`` holds CUDA tensors ``pos`` [N,3], ``atom_types`` [N] and ``cell`` [3,3] (all three directions periodic;
+    the cell is captured, so NVE / NVT).  ``capacity`` is the length of the edge buffer, by default
+    ``E0 + ceil(CAPACITY_SLACK * E0)`` with E0 the example's edge count; unused slots hold null edges.
+
+    ``g(pos)`` takes host (pinned) or device positions and returns ``total_energy`` [1,1], ``atomic_energy`` [N,1],
+    ``forces`` [N,3] and ``num_edges`` [1] -- views of static buffers that the next call overwrites.  Every call
+    reads the step's edge count and overflow flag back (12 bytes, one event wait) and checks that the list was grouped
+    by destination.  If the step needed more than ``capacity`` edges, the graph is re-captured with
+    ``capacity = ceil(1.02 * needed)`` and the same positions are computed again, so a returned result never comes
+    from a truncated list; ``capacity`` only grows and ``recaptures`` counts the re-captures."""
+
+    def __init__(self, model, example: Dict[str, torch.Tensor], capacity: Optional[int] = None, warmup: int = 3):
+        if example["pos"].device.type != "cuda":
+            raise RuntimeError("GraphedMDStep needs CUDA tensors (there is no CPU path)")
+        if example.get("cell") is None:
+            raise ValueError("GraphedMDStep needs a periodic cell")
+        if capacity is None:
+            e0 = int(ops.neighbor_list(example["pos"], example["cell"], True, model.r_max)["edge_index"].shape[1])
+            capacity = e0 + math.ceil(CAPACITY_SLACK * e0)
+        self.recaptures = 0
+        self._warmup = warmup
+        self._num_edges_host = torch.zeros(1, dtype=torch.int64).pin_memory()
+        self._overflow_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+        self._capture(model, {k: example[k] for k in ("pos", "atom_types", "cell")}, int(capacity))
+
+    def _capture(self, model, example: Dict[str, torch.Tensor], capacity: int) -> None:
+        self.capacity = capacity
+        self.plan = ops.NeighborListPlan(example["pos"].shape[0], example["cell"], True, model.r_max, capacity,
+                                         device=example["pos"].device)
+        super().__init__(model, example, warmup=self._warmup)
+        ops.src_csr_cache.clear()  # like csr_cache: an entry made during the capture lives in the graph's pool
+        out, self._out = self._out, None
+        self.atomic_energy, self.num_edges, self.overflow = out["atomic_energy"], out["num_edges"], out["overflow"]
+
+    def _run(self):
+        nl = self.plan.run(self.static["pos"])
+        d = dict(self.extra)
+        d.update(self.static)
+        d["edge_index"], d["edge_cell_shift"] = nl["edge_index"], nl["edge_cell_shift"]
+        out = self.model(d)
+        self._out = {"atomic_energy": out["atomic_energy"], "num_edges": nl["num_edges"], "overflow": nl["overflow"]}
+        return out
+
+    def _recapture(self, capacity: int) -> None:
+        example = {k: v.clone() for k, v in self.static.items()}  # the positions that overflowed
+        replays = self.replays
+        # drop every reference into the old graph's memory pool so that it is released with the graph
+        self.graph = self.plan = None
+        self.energy = self.forces = self.atomic_energy = self.num_edges = self.overflow = self.sorted_flag = None
+        self._sorted_flags = []
+        self._flag_event = None
+        self._capture(self.model, example, capacity)
+        self.replays = replays
+        self.recaptures += 1
+
+    def __call__(self, pos: torch.Tensor) -> Dict[str, torch.Tensor]:
+        self.static["pos"].copy_(pos, non_blocking=True)
+        while True:
+            self.replay()
+            self._num_edges_host.copy_(self.num_edges, non_blocking=True)
+            self._overflow_host.copy_(self.overflow, non_blocking=True)
+            done = torch.cuda.Event()
+            done.record()
+            done.synchronize()
+            self._verify_previous()
+            if int(self._overflow_host[0]) == 0:
+                break
+            needed = int(self._num_edges_host[0])
+            self._recapture(max(self.capacity + 1, math.ceil(1.02 * needed)))
+        return {"total_energy": self.energy, "atomic_energy": self.atomic_energy, "forces": self.forces,
+                "num_edges": self.num_edges}

@@ -128,6 +128,10 @@ def build_csr(edge_dst: torch.Tensor, num_nodes: int, assume_sorted: Optional[bo
     st = _stream()
     is_sorted = assume_sorted
     deferred = getattr(_sorted_tls, "flags", None)
+    if deferred is None and _capture_flags and torch.cuda.is_current_stream_capturing():
+        # the backward of a captured step runs in autograd's device thread, which has no thread-local context:
+        # use the innermost deferred_sorted_check that is open in some thread
+        deferred = _capture_flags[-1]
     if is_sorted is None and deferred is not None:
         # CUDA-graph capture (nequip_b200/graph.py): no host sync allowed -- run the check kernel, keep its
         # flag for the caller to verify after the replay, and build the CSR as if sorted
@@ -151,6 +155,7 @@ def build_csr(edge_dst: torch.Tensor, num_nodes: int, assume_sorted: Optional[bo
 
 
 _sorted_tls = threading.local()
+_capture_flags: List[List[torch.Tensor]] = []  # flag lists of the open deferred_sorted_check contexts, any thread
 
 
 class deferred_sorted_check:
@@ -161,10 +166,15 @@ class deferred_sorted_check:
         self.flags: List[torch.Tensor] = []
         self._prev = getattr(_sorted_tls, "flags", None)
         _sorted_tls.flags = self.flags
+        _capture_flags.append(self.flags)
         return self
 
     def __exit__(self, *exc):
         _sorted_tls.flags = self._prev
+        for k in range(len(_capture_flags) - 1, -1, -1):
+            if _capture_flags[k] is self.flags:
+                del _capture_flags[k]
+                break
         return False
 
 
@@ -756,23 +766,10 @@ def gate(x: torch.Tensor, tabs: GateTables) -> torch.Tensor:
 # ---------------------------------------------------------------------------------------
 # neighbour list on the device -- nqb_nl_bin / nqb_nl_count / nqb_nl_fill   (SURVEY 8f-2)
 # ---------------------------------------------------------------------------------------
-def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, transpose_perm: bool = False):
-    """Full neighbour list within ``r_max`` built on the GPU (cell list), in the layout the convolution wants.
-
-    ``pos`` [N,3] float64 CUDA; ``cell`` [3,3] (rows = lattice vectors; host or device) or None; ``pbc`` bool or 3
-    bools.  Returns a dict with ``edge_index`` [2,E] int64 (row 0 = centre / scatter destination, row 1 =
-    neighbour), ``edge_cell_shift`` [E,3] float64 (edge vector = pos[j] - pos[i] + shift @ cell), ``row_ptr``
-    [N+1] int64 (destination CSR: edges are sorted by (centre, neighbour)) and, on request,
-    ``edge_transpose_perm`` [E] (argsort by (neighbour, centre), nequip/data/transforms/neighborlist.py:150-155).
-    Same contract as the reference's host backends (nequip/data/_nl.py:60-152): both directions, no self edge in
-    the home image.  One host synchronisation (the edge count)."""
+def _nl_cell(cell, pbc):
+    """Host copies of the periodicity (3 bools), the cell (rows = lattice vectors) and its inverse."""
     import numpy as np
 
-    _require_cuda(pos)
-    L = _capi.lib()
-    pos = pos.detach().double().contiguous()
-    N = pos.shape[0]
-    dev = pos.device
     if isinstance(pbc, bool):
         pbc = (pbc,) * 3
     pbc = [bool(b) for b in (pbc.tolist() if torch.is_tensor(pbc) else pbc)]
@@ -782,9 +779,82 @@ def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, tr
         cell_np = np.eye(3)
     else:
         cell_np = (cell.detach().cpu().double().reshape(3, 3).numpy() if torch.is_tensor(cell) else np.asarray(cell, dtype=np.float64).reshape(3, 3)).copy()
-    inv_np = np.linalg.inv(cell_np)
-    # distance between opposite faces along each lattice direction = 1 / |column d of the inverse|
-    perp = 1.0 / np.linalg.norm(inv_np, axis=0)
+    return pbc, cell_np, np.linalg.inv(cell_np)
+
+
+class _NlArgs:
+    """Host-side arguments of the nqb_nl_* calls: cell, inverse, periodicity, bin grid and search range."""
+
+    def __init__(self, N: int, cell_np, inv_np, pbc, r_max: float, lo, width):
+        import numpy as np
+
+        # distance between opposite faces along each lattice direction = 1 / |column d of the inverse|
+        perp = 1.0 / np.linalg.norm(inv_np, axis=0)
+        nb, sr = [1, 1, 1], [1, 1, 1]
+        cap = max(1, int(round((4 * max(N, 1)) ** (1.0 / 3.0))))
+        for d in range(3):
+            extent = perp[d] * (1.0 if pbc[d] else width[d])
+            nb[d] = int(min(cap, max(1, np.floor(extent / r_max))))
+            sr[d] = int(np.ceil(r_max / (extent / nb[d]) - 1e-12)) if pbc[d] else 1
+            sr[d] = max(sr[d], 1)
+        I3 = C.c_int * 3
+        D9, D3 = C.c_double * 9, C.c_double * 3
+        self.cell, self.inv = D9(*cell_np.reshape(-1)), D9(*inv_np.reshape(-1))
+        self.pbc, self.nb, self.sr = I3(*[int(b) for b in pbc]), I3(*nb), I3(*sr)
+        self.lo, self.width = D3(*lo), D3(*width)
+        self.r_max = float(r_max)
+        self.nbins = nb[0] * nb[1] * nb[2]
+
+
+def _nl_scratch(N: int, nbins: int, dev) -> Dict[str, torch.Tensor]:
+    """Buffers of the bin / sort / count / scan steps (``row_ptr`` is the exact list's destination CSR)."""
+    return {
+        "wpos": torch.empty((N, 3), dtype=torch.float64, device=dev),
+        "base": torch.empty((N, 3), dtype=torch.int32, device=dev),
+        "cidx": torch.empty((N, 3), dtype=torch.int32, device=dev),
+        "binid": torch.empty((N,), dtype=torch.int64, device=dev),
+        "sorted_bin": torch.empty((N,), dtype=torch.int64, device=dev),
+        "order": torch.empty((N,), dtype=torch.int64, device=dev),
+        "bins": torch.arange(nbins + 1, device=dev, dtype=torch.int64),
+        "bin_start": torch.empty((nbins + 1,), dtype=torch.int64, device=dev),
+        "counts": torch.zeros((N,), dtype=torch.int64, device=dev),
+        "row_ptr": torch.zeros((N + 1,), dtype=torch.int64, device=dev),
+    }
+
+
+def _nl_rows(pos: torch.Tensor, a: _NlArgs, s: Dict[str, torch.Tensor]) -> None:
+    """Bins, atoms sorted by bin, neighbours per atom and their exclusive scan into ``s["row_ptr"]``; all on the
+    device, no host synchronisation."""
+    L = _capi.lib()
+    N = pos.shape[0]
+    st = _stream()
+    _capi.check(L.nqb_nl_bin(_ptr(pos), N, a.cell, a.inv, a.pbc, a.nb, a.sr, a.lo, a.width, a.r_max, _ptr(s["wpos"]),
+                             _ptr(s["base"]), _ptr(s["binid"]), _ptr(s["cidx"]), st), "nqb_nl_bin")
+    torch.sort(s["binid"], stable=True, out=(s["sorted_bin"], s["order"]))
+    torch.searchsorted(s["sorted_bin"], s["bins"], out=s["bin_start"])
+    _capi.check(L.nqb_nl_count(N, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, _ptr(s["wpos"]), _ptr(s["cidx"]),
+                               _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(s["counts"]), st), "nqb_nl_count")
+    torch.cumsum(s["counts"], 0, out=s["row_ptr"][1:])
+
+
+def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, transpose_perm: bool = False):
+    """Full neighbour list within ``r_max`` built on the GPU (cell list), in the layout the convolution wants.
+
+    ``pos`` [N,3] float64 CUDA; ``cell`` [3,3] (rows = lattice vectors; host or device) or None; ``pbc`` bool or 3
+    bools.  Returns a dict with ``edge_index`` [2,E] int64 (row 0 = centre / scatter destination, row 1 =
+    neighbour), ``edge_cell_shift`` [E,3] float64 (edge vector = pos[j] - pos[i] + shift @ cell), ``row_ptr``
+    [N+1] int64 (destination CSR: edges are sorted by (centre, neighbour)) and, on request,
+    ``edge_transpose_perm`` [E] (argsort by (neighbour, centre), nequip/data/transforms/neighborlist.py:150-155).
+    Same contract as the reference's host backends (nequip/data/_nl.py:60-152): both directions, no self edge in
+    the home image.  One host synchronisation (the edge count); ``NeighborListPlan`` has none."""
+    import numpy as np
+
+    _require_cuda(pos)
+    L = _capi.lib()
+    pos = pos.detach().double().contiguous()
+    N = pos.shape[0]
+    dev = pos.device
+    pbc, cell_np, inv_np = _nl_cell(cell, pbc)
     lo = np.zeros(3)
     width = np.ones(3)
     if not all(pbc) and N > 0:
@@ -793,39 +863,101 @@ def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, tr
         for d in range(3):
             if not pbc[d]:
                 lo[d], width[d] = fmin[d], max(fmax[d] - fmin[d], 1e-9) * (1 + 1e-9)
-    nb, sr = [1, 1, 1], [1, 1, 1]
-    cap = max(1, int(round((4 * max(N, 1)) ** (1.0 / 3.0))))
-    for d in range(3):
-        extent = perp[d] * (1.0 if pbc[d] else width[d])
-        nb[d] = int(min(cap, max(1, np.floor(extent / r_max))))
-        sr[d] = int(np.ceil(r_max / (extent / nb[d]) - 1e-12)) if pbc[d] else 1
-        sr[d] = max(sr[d], 1)
-    I3 = C.c_int * 3
-    D9, D3 = C.c_double * 9, C.c_double * 3
-    cell_c, inv_c = D9(*cell_np.reshape(-1)), D9(*inv_np.reshape(-1))
-    pbc_c, nb_c, sr_c = I3(*[int(b) for b in pbc]), I3(*nb), I3(*sr)
-    lo_c, wd_c = D3(*lo), D3(*width)
-    st = _stream()
-    wpos = torch.empty((N, 3), dtype=torch.float64, device=dev)
-    base = torch.empty((N, 3), dtype=torch.int32, device=dev)
-    cidx = torch.empty((N, 3), dtype=torch.int32, device=dev)
-    binid = torch.empty((N,), dtype=torch.int64, device=dev)
-    _capi.check(L.nqb_nl_bin(_ptr(pos), N, cell_c, inv_c, pbc_c, nb_c, sr_c, lo_c, wd_c, float(r_max), _ptr(wpos), _ptr(base),
-                             _ptr(binid), _ptr(cidx), st), "nqb_nl_bin")
-    nbins = nb[0] * nb[1] * nb[2]
-    sorted_bin, order = torch.sort(binid, stable=True)
-    bin_start = torch.searchsorted(sorted_bin, torch.arange(nbins + 1, device=dev, dtype=torch.int64)).contiguous()
-    counts = torch.zeros((N,), dtype=torch.int64, device=dev)
-    _capi.check(L.nqb_nl_count(N, cell_c, inv_c, pbc_c, nb_c, sr_c, float(r_max), _ptr(wpos), _ptr(cidx), _ptr(order),
-                               _ptr(bin_start), _ptr(counts), st), "nqb_nl_count")
-    row_ptr = torch.zeros((N + 1,), dtype=torch.int64, device=dev)
-    torch.cumsum(counts, 0, out=row_ptr[1:])
+    a = _NlArgs(N, cell_np, inv_np, pbc, r_max, lo, width)
+    s = _nl_scratch(N, a.nbins, dev)
+    _nl_rows(pos, a, s)
+    row_ptr = s["row_ptr"]
     E = int(row_ptr[-1].item())
     edge_index = torch.empty((2, E), dtype=torch.int64, device=dev)
     shifts = torch.empty((E, 3), dtype=torch.float64, device=dev)
-    _capi.check(L.nqb_nl_fill(N, E, cell_c, inv_c, pbc_c, nb_c, sr_c, float(r_max), _ptr(wpos), _ptr(cidx), _ptr(base),
-                              _ptr(order), _ptr(bin_start), _ptr(row_ptr), _ptr(edge_index), _ptr(shifts), st), "nqb_nl_fill")
+    _capi.check(L.nqb_nl_fill(N, E, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, _ptr(s["wpos"]), _ptr(s["cidx"]),
+                              _ptr(s["base"]), _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(row_ptr), _ptr(edge_index),
+                              _ptr(shifts), _stream()), "nqb_nl_fill")
     out = {"edge_index": edge_index, "edge_cell_shift": shifts, "row_ptr": row_ptr}
     if transpose_perm:
         out["edge_transpose_perm"] = torch.argsort(edge_index[1] * N + edge_index[0], stable=True)
     return out
+
+
+def null_edge_shift(cell, r_max: float):
+    """Cell shift [3] (integer-valued float64, host) of the null edges of ``NeighborListPlan``: ``k e_d`` along the
+    longest lattice vector ``a_d``, ``k = floor(r_max / |a_d|) + 2``, so the edge (i, i, k e_d) is at least
+    ``r_max + |a_d|`` long.  Its cutoff envelope and the envelope's derivative are exactly 0 there, and the radial MLP
+    has no bias with silu(0) = 0, so such an edge adds exact zeros to the energy, the forces and the virial."""
+    import numpy as np
+
+    cell_np = (cell.detach().cpu().double().reshape(3, 3).numpy() if torch.is_tensor(cell)
+               else np.asarray(cell, dtype=np.float64).reshape(3, 3))
+    lengths = np.linalg.norm(cell_np, axis=1)
+    d = int(np.argmax(lengths))
+    shift = np.zeros(3)
+    shift[d] = np.floor(r_max / lengths[d]) + 2
+    return shift
+
+
+class NeighborListPlan:
+    """Device neighbour list of a fixed length ``capacity`` for one cell: positions in, list out, without a host
+    synchronisation, so it can be captured in a CUDA graph (``graph.GraphedMDStep``).
+
+    All host work (inverse cell, bin grid, search range, the null-edge shift) and every allocation happen here; the
+    cell is fixed for the plan's lifetime.  The cell must be given and periodic in all three directions: a
+    non-periodic direction needs the positions' bounding box on the host at every call.  A molecule in vacuum can use
+    a large periodic box.
+
+    ``run(pos)`` returns ``edge_index`` [2, capacity], ``edge_cell_shift`` [capacity, 3], ``row_ptr`` [N+1] (the
+    padded destination CSR), ``num_edges`` [1] int64 (the true edge count E) and ``overflow`` [1] int32, all on the
+    device and all overwritten by the next ``run``.  Row i holds its real edges in the order of ``neighbor_list``,
+    then null edges (i, i, ``pad_shift``); each row gets floor or ceil of (capacity - E) / N of them.  When
+    E > capacity, ``overflow`` is 1 and every row holds only null edges: the list must not be used."""
+
+    def __init__(self, num_atoms: int, cell, pbc, r_max: float, capacity: int, device=None):
+        import numpy as np
+
+        if cell is None:
+            raise ValueError("NeighborListPlan needs a cell")
+        if isinstance(pbc, bool):
+            pbc = (pbc,) * 3
+        pbc = [bool(b) for b in (pbc.tolist() if torch.is_tensor(pbc) else pbc)]
+        if len(pbc) != 3 or not all(pbc):
+            raise ValueError("NeighborListPlan needs all three directions periodic (the bounding box of a "
+                             "non-periodic direction is found on the host at every call); use a large periodic box")
+        if int(num_atoms) < 1 or int(capacity) < 0:
+            raise ValueError("NeighborListPlan needs num_atoms >= 1 and capacity >= 0")
+        self.num_atoms, self.capacity, self.r_max = int(num_atoms), int(capacity), float(r_max)
+        pbc, cell_np, inv_np = _nl_cell(cell, pbc)
+        self.pad_shift = null_edge_shift(cell_np, r_max)
+        self._pad_shift_c = (C.c_double * 3)(*self.pad_shift)
+        dev = torch.device(device) if device is not None else (
+            cell.device if torch.is_tensor(cell) and cell.is_cuda else torch.device("cuda"))
+        self.device = dev
+        self._a = _NlArgs(self.num_atoms, cell_np, inv_np, pbc, r_max, np.zeros(3), np.ones(3))
+        self._s = _nl_scratch(self.num_atoms, self._a.nbins, dev)
+        N, cap = self.num_atoms, self.capacity
+        self.edge_index = torch.empty((2, cap), dtype=torch.int64, device=dev)
+        self.edge_cell_shift = torch.empty((cap, 3), dtype=torch.float64, device=dev)
+        self.row_ptr = torch.empty((N + 1,), dtype=torch.int64, device=dev)
+        self.num_edges = torch.empty((1,), dtype=torch.int64, device=dev)
+        self.overflow = torch.empty((1,), dtype=torch.int32, device=dev)
+
+    def run(self, pos: torch.Tensor) -> Dict[str, torch.Tensor]:
+        _require_cuda(pos)
+        if tuple(pos.shape) != (self.num_atoms, 3):
+            raise ValueError(f"NeighborListPlan: pos must be [{self.num_atoms}, 3], got {tuple(pos.shape)}")
+        pos = pos.detach().double().contiguous()
+        L = _capi.lib()
+        a, s = self._a, self._s
+        _nl_rows(pos, a, s)
+        st = _stream()
+        _capi.check(L.nqb_nl_pad(self.num_atoms, self.capacity, _ptr(s["row_ptr"]), _ptr(self.row_ptr),
+                                 _ptr(self.num_edges), _ptr(self.overflow), st), "nqb_nl_pad")
+        _capi.check(L.nqb_nl_fill_capacity(self.num_atoms, self.capacity, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max,
+                                           _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["base"]), _ptr(s["order"]),
+                                           _ptr(s["bin_start"]), _ptr(self.row_ptr), _ptr(self.overflow),
+                                           self._pad_shift_c, _ptr(self.edge_index), _ptr(self.edge_cell_shift), st),
+                    "nqb_nl_fill_capacity")
+        # the kernels write through raw pointers: bump the version counters so that the CSRs cached against these
+        # buffers (csr_cache, src_csr_cache) are rebuilt for the new list
+        for t in (self.edge_index, self.edge_cell_shift, self.row_ptr, self.num_edges, self.overflow):
+            torch.autograd.graph.increment_version(t)
+        return {"edge_index": self.edge_index, "edge_cell_shift": self.edge_cell_shift, "row_ptr": self.row_ptr,
+                "num_edges": self.num_edges, "overflow": self.overflow}

@@ -1,0 +1,186 @@
+#!/usr/bin/env python
+"""MD step: eager neighbour list + model against the graphed step (``graph.GraphedMDStep``) on a moving frame.
+
+Each workload follows the bounded trajectory ``data.oscillating_positions`` (0.2 A amplitude, period 50 steps), whose
+edge count changes at most steps.  Positions start on the device; each step ends with the forces on the host, as in
+a host-driven MD loop.
+  A: ``ops.neighbor_list`` + ``model(d)`` (eager launches, one host synchronisation for the edge count), forces D2H;
+  B: ``GraphedMDStep`` (one graph replay, 12-byte read-back of the edge count / overflow flag), forces D2H.
+Arms are timed A, B, A, B in one process; every 10th step B's energy and forces are compared with A's at the same
+positions.  ``pad`` lines time B on the frozen first frame with capacity E, 1.02 E and 1.05 E (the cost of the null
+edges).  The first line names the GPU, its power limit and its maximum SM clock.
+
+    python tools/bench_md.py [--workloads water_1k_l2_f32,li3po4_10k_l2_f64,S_li3po4_10k] [--steps 100]
+                             [--warmup 10] [--out FILE]
+"""
+import argparse
+import json
+import math
+import os
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+R_MAX = 5.0
+PERIOD, AMPLITUDE = 50, 0.2
+# name: (structure kind, n_side, model kwargs or a preset name) -- the first two are bench.py's workloads
+WORKLOADS = {
+    "water_1k_l2_f32": ("water", 10, dict(l_max=2, num_layers=4, num_features=32, radial_mlp_depth=1,
+                                          radial_mlp_width=128)),
+    "li3po4_10k_l2_f64": ("li3po4", 22, dict(l_max=2, num_layers=4, num_features=64, radial_mlp_depth=1,
+                                             radial_mlp_width=128)),
+    "S_li3po4_10k": ("li3po4", 22, "S"),
+}
+
+
+def emit(line, sink):
+    print(json.dumps(line), flush=True)
+    sink.append(line)
+
+
+def gpu_info():
+    import torch
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=index,name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    dev = torch.cuda.current_device()
+    rows = [r.split(", ") for r in q.stdout.strip().splitlines()] if q.returncode == 0 else []
+    row = next((r for r in rows if r and r[0] == str(dev)), None)
+    return {"kind": "gpu", "name": torch.cuda.get_device_name(dev),
+            "power_limit": row[2] if row else "not read", "max_sm_clock": row[3] if row else "not read"}
+
+
+def build(workload):
+    import torch
+
+    from nequip_b200 import data as D
+    from nequip_b200.nn.model import NequIPEnergyModel
+
+    kind, n_side, mk = WORKLOADS[workload]
+    sysd = D.make_system(kind, n_side, r_max=R_MAX, seed=0)
+    meta = sysd.pop("_meta")
+    kw = dict(r_max=R_MAX, type_names=meta["type_names"], avg_num_neighbors=meta["avg_num_neighbors"],
+              strict_fast_path=True)
+    model = (NequIPEnergyModel.from_preset(mk, **kw) if isinstance(mk, str)
+             else NequIPEnergyModel(parity=True, **mk, **kw)).cuda()
+    for p in model.parameters():
+        p.requires_grad_(False)
+    dev = D.to_device({k: sysd[k] for k in ("pos", "atom_types", "cell")}, "cuda")
+    return model, dev, int(sysd["edge_index"].shape[1])
+
+
+def arm_eager(model, dev, positions, keep):
+    from nequip_b200 import ops
+
+    kept, counts = {}, []
+    for t, pos in enumerate(positions):
+        nl = ops.neighbor_list(pos, dev["cell"], True, R_MAX)
+        out = model(dict(dev, pos=pos, edge_index=nl["edge_index"], edge_cell_shift=nl["edge_cell_shift"]))
+        f = out["forces"].cpu()
+        counts.append(int(nl["edge_index"].shape[1]))
+        if keep and t % 10 == 0:
+            kept[t] = (float(out["total_energy"]), f)
+    return kept, counts
+
+
+def arm_graph(g, positions, keep):
+    kept, counts = {}, []
+    for t, pos in enumerate(positions):
+        out = g(pos)
+        f = out["forces"].cpu()
+        counts.append(int(g._num_edges_host[0]))  # read back by the call itself
+        if keep and t % 10 == 0:
+            kept[t] = (float(out["total_energy"]), f)
+    return kept, counts
+
+
+def timed(fn, warm_positions, positions):
+    import torch
+
+    fn(warm_positions, False)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    kept, counts = fn(positions, True)
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) * 1e3 / len(positions), kept, counts
+
+
+def run_workload(workload, steps, warmup, sink):
+    import torch
+
+    from nequip_b200 import data as D
+    from nequip_b200.graph import GraphedMDStep
+
+    model, dev, E0 = build(workload)
+    N = dev["pos"].shape[0]
+    pos0 = dev["pos"].clone()
+    positions = [D.oscillating_positions(pos0, t, PERIOD, AMPLITUDE, seed=1) for t in range(steps)]
+    warm = [D.oscillating_positions(pos0, -1 - t, PERIOD, AMPLITUDE, seed=1) for t in range(warmup)]
+    g = GraphedMDStep(model, dev)
+    cap0 = g.capacity
+    ms = {"A": [], "B": []}
+    ref, got, counts = None, None, None
+    for rep in range(2):
+        t_a, ref, counts = timed(lambda p, k: arm_eager(model, dev, p, k), warm, positions)
+        t_b, got, counts_b = timed(lambda p, k: arm_graph(g, p, k), warm, positions)
+        if counts_b != counts:
+            raise RuntimeError(f"{workload}: graphed edge counts differ from the eager list's")
+        ms["A"].append(t_a)
+        ms["B"].append(t_b)
+        emit({"kind": "md_rep", "workload": workload, "rep": rep, "A_eager_ms_per_step": round(t_a, 4),
+              "B_graph_ms_per_step": round(t_b, 4)}, sink)
+    de, df = 0.0, 0.0
+    for t, (e_a, f_a) in ref.items():
+        e_b, f_b = got[t]
+        de = max(de, abs(e_b - e_a) / abs(e_a))
+        df = max(df, float((f_b - f_a).abs().max()) / float(f_a.abs().max()))
+    changed = sum(a != b for a, b in zip(counts, counts[1:]))
+    emit({"kind": "md", "workload": workload, "atoms": N, "E0": E0, "steps": steps, "period": PERIOD,
+          "amplitude_A": AMPLITUDE, "A_eager_ms_per_step": [round(x, 4) for x in ms["A"]],
+          "B_graph_ms_per_step": [round(x, 4) for x in ms["B"]],
+          "speedup_B_over_A": round(min(ms["A"]) / min(ms["B"]), 3),
+          "edge_count_changed_fraction": round(changed / (steps - 1), 4),
+          "E_over_E0_min": round(min(counts) / E0, 5), "E_over_E0_max": round(max(counts) / E0, 5),
+          "capacity_initial": cap0, "capacity_final": g.capacity, "recaptures": g.recaptures,
+          "launches_per_replay": g.launches_per_replay, "checked_steps": len(ref),
+          "max_rel_energy_dev_B_vs_A": de, "max_force_dev_B_vs_A_over_max_F": df}, sink)
+    del g
+    torch.cuda.empty_cache()
+    # cost of the padding: B on the frozen first frame
+    frozen = [pos0] * steps
+    for slack in (0.0, 0.02, 0.05):
+        cap = E0 + math.ceil(slack * E0)
+        g = GraphedMDStep(model, dev, capacity=cap)
+        t_pad, _, _ = timed(lambda p, k: arm_graph(g, p, False), [pos0] * warmup, frozen)
+        emit({"kind": "pad", "workload": workload, "E": E0, "capacity": cap, "slack": slack,
+              "B_graph_ms_per_step": round(t_pad, 4), "recaptures": g.recaptures}, sink)
+        del g
+        torch.cuda.empty_cache()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workloads", default=",".join(WORKLOADS))
+    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--out", default=None, help="also write the JSON lines to this file")
+    args = ap.parse_args()
+    import torch
+
+    torch.backends.cuda.matmul.allow_tf32 = False
+    sink = []
+    emit(gpu_info(), sink)
+    for w in args.workloads.split(","):
+        run_workload(w, args.steps, args.warmup, sink)
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, "w") as fh:
+            for line in sink:
+                fh.write(json.dumps(line) + "\n")
+
+
+if __name__ == "__main__":
+    main()
