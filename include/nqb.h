@@ -194,6 +194,27 @@ int nqb_nl_fill_capacity(int64_t N, int64_t capacity, const double* cell_host, c
                          const int64_t* row_ptr_pad /* [N+1] */, const int32_t* overflow /* [1] */,
                          const double* pad_shift_host, int64_t* edge_index /* [2,capacity] */,
                          double* shifts /* [capacity,3] */, nqb_stream_t st);
+/* Variable cell: the cell-dependent arguments (cell, inverse, periodicity, bin grid, search range, r_max and the
+ * null-edge shift) live in a parameter block in DEVICE memory, so one captured graph follows a cell that changes between
+ * replays.  The block's layout is private to the library: nqb_nl_params_bytes() is its size, and
+ * nqb_nl_params_pack fills out_host [nqb_nl_params_bytes()] on the HOST with exactly the values the by-value calls
+ * derive from the same arguments (host only, no CUDA call; every direction must be periodic).  The caller copies the
+ * block to the device, stream-ordered before the calls that read it.
+ * nqb_nl_bin_dp, nqb_nl_count_dp and nqb_nl_fill_capacity_dp have the write contracts of nqb_nl_bin (wpos, base, bin,
+ * cidx fully written), nqb_nl_count (counts fully written) and nqb_nl_fill_capacity (edge_index, shifts fully written,
+ * nothing past capacity; null edges carry the block's pad_shift). */
+int64_t nqb_nl_params_bytes(void);
+int nqb_nl_params_pack(const double* cell_host, const double* inv_host, const int* pbc, const int* nbins,
+                       const int* search, double r_max, const double* pad_shift_host, void* out_host);
+int nqb_nl_bin_dp(const double* pos, int64_t N, const void* params_dev, double* wpos /* [N,3] */,
+                  int32_t* base /* [N,3] */, int64_t* bin /* [N] */, int32_t* cidx /* [N,3] */, nqb_stream_t st);
+int nqb_nl_count_dp(int64_t N, const void* params_dev, const double* wpos, const int32_t* cidx, const int64_t* order,
+                    const int64_t* bin_start, int64_t* counts /* [N] */, nqb_stream_t st);
+int nqb_nl_fill_capacity_dp(int64_t N, int64_t capacity, const void* params_dev, const double* wpos,
+                            const int32_t* cidx, const int32_t* base, const int64_t* order, const int64_t* bin_start,
+                            const int64_t* row_ptr_pad /* [N+1] */, const int32_t* overflow /* [1] */,
+                            int64_t* edge_index /* [2,capacity] */, double* shifts /* [capacity,3] */,
+                            nqb_stream_t st);
 
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).

@@ -53,6 +53,11 @@ SIGNATURES = {
     "nqb_nl_pad": (_i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp]),
     "nqb_nl_fill_capacity": (
         _i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nl_params_bytes": (_i64, []),
+    "nqb_nl_params_pack": (_i32, [_vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp]),
+    "nqb_nl_bin_dp": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nl_count_dp": (_i32, [_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nl_fill_capacity_dp": (_i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nqb_sh_fwd": (_i32, [_i32, _vp, _i64, _i32, _vp, _vp]),
     "nqb_sh_bwd": (_i32, [_i32, _vp, _i64, _i32, _vp, _vp, _vp]),
     "nqb_edge_embed_fwd": (

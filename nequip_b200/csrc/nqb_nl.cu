@@ -15,6 +15,7 @@
 // explicitly rounded operations (no FMA contraction), so the edge set is bit-identical.
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/nqb.h"
 
@@ -35,14 +36,33 @@ struct NlParams {
   double r2;
 };
 
+// Where the kernels read NlParams from (template argument PS): the by-value kernel parameter NlParams (host-built
+// per launch) or a block in device memory, NlBlock* (variable cell: nqb_nl_params_pack fills it on the host and the
+// caller copies it in before a launch or a graph replay).  The block also holds the null-edge shift of the capacity
+// fill, which follows the cell.  One kernel body per kernel reads its parameters through nl_p / nl_pad_shift.
+struct NlBlock {
+  NlParams p;
+  double pad_shift[3];
+};
+typedef const NlBlock* __restrict__ NlBlockPtr;
+
+__device__ __forceinline__ const NlParams& nl_p(const NlParams& p) { return p; }
+__device__ __forceinline__ const NlParams& nl_p(NlBlockPtr b) { return b->p; }
+__device__ __forceinline__ double3 nl_pad_shift(const NlParams&, double3 pad_shift) { return pad_shift; }
+__device__ __forceinline__ double3 nl_pad_shift(NlBlockPtr b, double3) {
+  return make_double3(b->pad_shift[0], b->pad_shift[1], b->pad_shift[2]);
+}
+
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
 
 // wrapped cartesian position, integer base shift (pos + base @ cell is the wrapped position) and bin of one atom
-__global__ void k_nl_bin(NlParams p, const double* __restrict__ pos, int64_t N, double* __restrict__ wpos,
+template <class PS>
+__global__ void k_nl_bin(PS ps, const double* __restrict__ pos, int64_t N, double* __restrict__ wpos,
                          int32_t* __restrict__ base, int64_t* __restrict__ bin, int32_t* __restrict__ cidx) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
+  const NlParams& p = nl_p(ps);
   const double x = pos[3 * i], y = pos[3 * i + 1], z = pos[3 * i + 2];
   double f[3];
   if (p.orthorhombic) {
@@ -119,13 +139,14 @@ __device__ __forceinline__ void nl_visit(const NlParams& p, int64_t i, const dou
   }
 }
 
-__global__ void k_nl_count(NlParams p, int64_t N, const double* __restrict__ wpos, const int32_t* __restrict__ cidx,
+template <class PS>
+__global__ void k_nl_count(PS ps, int64_t N, const double* __restrict__ wpos, const int32_t* __restrict__ cidx,
                            const int64_t* __restrict__ order, const int64_t* __restrict__ bin_start,
                            int64_t* __restrict__ counts) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   int64_t n = 0;
-  nl_visit(p, i, wpos, cidx, order, bin_start, [&](int64_t, int, int, int) { ++n; });
+  nl_visit(nl_p(ps), i, wpos, cidx, order, bin_start, [&](int64_t, int, int, int) { ++n; });
   counts[i] = n;
 }
 
@@ -140,8 +161,10 @@ __device__ __forceinline__ bool nl_less(int64_t ja, const double* sa, int64_t jb
 // kCapacity = true (nqb_nl_fill_capacity): the row owns [row_ptr_pad[i], row_ptr_pad[i + 1]) of a list of E = capacity
 // slots; its real edges come first (same order and shifts as above, none when *overflow is set) and the remaining slots
 // hold null edges (i, i, pad_shift).  The trailing parameters are appended so the unpadded variant's code is unchanged.
-template <bool kCapacity>
-__global__ void k_nl_fill(NlParams p, int64_t N, const double* __restrict__ wpos, const int32_t* __restrict__ cidx,
+// With PS = NlBlockPtr (only with kCapacity) the null-edge shift comes from the block and the pad_shift argument is
+// not read.
+template <bool kCapacity, class PS>
+__global__ void k_nl_fill(PS ps, int64_t N, const double* __restrict__ wpos, const int32_t* __restrict__ cidx,
                           const int32_t* __restrict__ base, const int64_t* __restrict__ order,
                           const int64_t* __restrict__ bin_start, const int64_t* __restrict__ row_ptr, int64_t E,
                           int64_t* __restrict__ edge_index, double* __restrict__ shifts,
@@ -152,7 +175,7 @@ __global__ void k_nl_fill(NlParams p, int64_t N, const double* __restrict__ wpos
   int64_t n = 0;
   int64_t* ej = edge_index + E;  // neighbours (row 1)
   if (!kCapacity || *overflow == 0) {
-    nl_visit(p, i, wpos, cidx, order, bin_start, [&](int64_t j, int ix, int iy, int iz) {
+    nl_visit(nl_p(ps), i, wpos, cidx, order, bin_start, [&](int64_t j, int ix, int iy, int iz) {
       // insertion into the sorted prefix of the row (rows hold a few dozen neighbours)
       double s[3] = {(double)(ix + base[3 * j] - base[3 * i]), (double)(iy + base[3 * j + 1] - base[3 * i + 1]),
                      (double)(iz + base[3 * j + 2] - base[3 * i + 2])};
@@ -170,10 +193,11 @@ __global__ void k_nl_fill(NlParams p, int64_t N, const double* __restrict__ wpos
   }
   if (kCapacity) {
     const int64_t end = row_ptr[i + 1];
+    const double3 ps3 = nl_pad_shift(ps, pad_shift);
     for (int64_t q = beg + n; q < end; ++q) {
       edge_index[q] = i;
       ej[q] = i;
-      shifts[3 * q] = pad_shift.x; shifts[3 * q + 1] = pad_shift.y; shifts[3 * q + 2] = pad_shift.z;
+      shifts[3 * q] = ps3.x; shifts[3 * q + 1] = ps3.y; shifts[3 * q + 2] = ps3.z;
     }
   }
 }
@@ -215,7 +239,7 @@ extern "C" int nqb_nl_bin(const double* pos, int64_t N, const double* cell_host,
     if (nbins[d] < 1 || search[d] < 0) return nqb_set_error("nqb_nl_bin: bad bin grid");
   }
   p.r2 = r_max * r_max;
-  k_nl_bin<<<(unsigned)((N + 127) / 128), 128, 0, (cudaStream_t)st>>>(p, pos, N, wpos, base, bin, cidx);
+  k_nl_bin<NlParams><<<(unsigned)((N + 127) / 128), 128, 0, (cudaStream_t)st>>>(p, pos, N, wpos, base, bin, cidx);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -242,7 +266,7 @@ extern "C" int nqb_nl_count(int64_t N, const double* cell_host, const double* in
   if (!wpos || !cidx || !order || !bin_start || !counts) return nqb_set_error("nqb_nl_count: null pointer");
   NlParams p;
   nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
-  k_nl_count<<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(p, N, wpos, cidx, order, bin_start, counts);
+  k_nl_count<NlParams><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(p, N, wpos, cidx, order, bin_start, counts);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -260,9 +284,8 @@ extern "C" int nqb_nl_fill(int64_t N, int64_t E, const double* cell_host, const 
     return nqb_set_error("nqb_nl_fill: null pointer");
   NlParams p;
   nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
-  k_nl_fill<false><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(p, N, wpos, cidx, base, order, bin_start,
-                                                                           row_ptr, E, edge_index, shifts, nullptr,
-                                                                           make_double3(0.0, 0.0, 0.0));
+  k_nl_fill<false, NlParams><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
+      p, N, wpos, cidx, base, order, bin_start, row_ptr, E, edge_index, shifts, nullptr, make_double3(0.0, 0.0, 0.0));
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -296,9 +319,73 @@ extern "C" int nqb_nl_fill_capacity(int64_t N, int64_t capacity, const double* c
   NlParams p;
   nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
   const double3 ps = make_double3(pad_shift_host[0], pad_shift_host[1], pad_shift_host[2]);
-  k_nl_fill<true><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(p, N, wpos, cidx, base, order, bin_start,
-                                                                          row_ptr_pad, capacity, edge_index, shifts,
-                                                                          overflow, ps);
+  k_nl_fill<true, NlParams><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
+      p, N, wpos, cidx, base, order, bin_start, row_ptr_pad, capacity, edge_index, shifts, overflow, ps);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+// Variable cell: the same three kernels reading their parameters from a block in device memory, so that a captured
+// graph follows a cell that changes between replays.  The block is built on the host by nqb_nl_params_pack (the
+// helper above, so the orthorhombic test and every field match the by-value path) and copied in by the caller.
+extern "C" int64_t nqb_nl_params_bytes(void) { return (int64_t)sizeof(NlBlock); }
+
+extern "C" int nqb_nl_params_pack(const double* cell_host, const double* inv_host, const int* pbc, const int* nbins,
+                                  const int* search, double r_max, const double* pad_shift_host, void* out_host) {
+  if (!cell_host || !inv_host || !pbc || !nbins || !search || !pad_shift_host || !out_host)
+    return nqb_set_error("nqb_nl_params_pack: null pointer");
+  for (int d = 0; d < 3; ++d) {
+    if (!pbc[d]) return nqb_set_error("nqb_nl_params_pack: every direction must be periodic");
+    if (nbins[d] < 1 || search[d] < 0) return nqb_set_error("nqb_nl_params_pack: bad bin grid");
+  }
+  NlBlock b;
+  memset(&b, 0, sizeof(b));
+  nl_params(cell_host, inv_host, pbc, nbins, search, r_max, b.p);
+  for (int d = 0; d < 3; ++d) b.pad_shift[d] = pad_shift_host[d];
+  memcpy(out_host, &b, sizeof(b));
+  return 0;
+}
+
+extern "C" int nqb_nl_bin_dp(const double* pos, int64_t N, const void* params_dev, double* wpos, int32_t* base,
+                             int64_t* bin, int32_t* cidx, nqb_stream_t st) {
+  if (N < 0) return nqb_set_error("nqb_nl_bin_dp: negative size");
+  if (N == 0) return 0;
+  if (!pos || !params_dev || !wpos || !base || !bin || !cidx) return nqb_set_error("nqb_nl_bin_dp: null pointer");
+  k_nl_bin<NlBlockPtr><<<(unsigned)((N + 127) / 128), 128, 0, (cudaStream_t)st>>>(
+      (const NlBlock*)params_dev, pos, N, wpos, base, bin, cidx);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int nqb_nl_count_dp(int64_t N, const void* params_dev, const double* wpos, const int32_t* cidx,
+                               const int64_t* order, const int64_t* bin_start, int64_t* counts, nqb_stream_t st) {
+  if (N <= 0) return 0;
+  if (!params_dev || !wpos || !cidx || !order || !bin_start || !counts)
+    return nqb_set_error("nqb_nl_count_dp: null pointer");
+  k_nl_count<NlBlockPtr><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
+      (const NlBlock*)params_dev, N, wpos, cidx, order, bin_start, counts);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int nqb_nl_fill_capacity_dp(int64_t N, int64_t capacity, const void* params_dev, const double* wpos,
+                                       const int32_t* cidx, const int32_t* base, const int64_t* order,
+                                       const int64_t* bin_start, const int64_t* row_ptr_pad, const int32_t* overflow,
+                                       int64_t* edge_index, double* shifts, nqb_stream_t st) {
+  if (N <= 0 || capacity < 0) return nqb_set_error("nqb_nl_fill_capacity_dp: needs N > 0 and capacity >= 0");
+  if (capacity == 0) return 0;
+  if (!params_dev || !wpos || !cidx || !base || !order || !bin_start || !row_ptr_pad || !overflow || !edge_index ||
+      !shifts)
+    return nqb_set_error("nqb_nl_fill_capacity_dp: null pointer");
+  k_nl_fill<true, NlBlockPtr><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
+      (const NlBlock*)params_dev, N, wpos, cidx, base, order, bin_start, row_ptr_pad, capacity, edge_index, shifts,
+      overflow, make_double3(0.0, 0.0, 0.0));
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));

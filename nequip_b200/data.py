@@ -213,5 +213,20 @@ def oscillating_positions(pos0: torch.Tensor, t: int, period: int = 50, amplitud
     return pos0 + amplitude * torch.sin(2 * np.pi * t / period + phi)
 
 
+def oscillating_strain(t: int, period: int = 50, diagonal: float = 0.02, shear: float = 0.03) -> torch.Tensor:
+    """``I + eps(t)`` [3,3] float64 of a bounded variable-cell trajectory: ``eps`` is symmetric, its diagonal
+    oscillates with amplitude ``diagonal`` and its off-diagonal pairs with amplitude ``shear``, each with its own fixed
+    phase.  Step t of the trajectory is ``cell0 @ S`` and ``oscillating_positions(pos0, t) @ S`` (rows = vectors), so
+    the cell is triclinic at most steps.  The diagonal phases are pi/3 apart, so the trace of eps swings by
+    2 * diagonal: the volume swings by about +-4 % for diagonal = 0.02 (phases 2 pi/3 apart would keep it fixed)."""
+    w = 2 * np.pi * t / period
+    eps = np.zeros((3, 3))
+    for d in range(3):
+        eps[d, d] = diagonal * np.sin(w + np.pi * d / 3)
+    for k, (a, b) in enumerate(((0, 1), (0, 2), (1, 2))):
+        eps[a, b] = eps[b, a] = shear * np.sin(w + np.pi / 4 + 2 * np.pi * k / 3)
+    return torch.from_numpy(np.eye(3) + eps)
+
+
 def to_device(data: Dict, device) -> Dict:
     return {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in data.items()}

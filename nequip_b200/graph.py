@@ -16,7 +16,9 @@ is computed inside the graph and verified when the results are read.  Anything e
 ``GraphedMDStep`` lifts the shape restriction for molecular dynamics in a fixed periodic cell: the device neighbour
 list (``ops.NeighborListPlan``) is part of the graph and writes a list of fixed length ``capacity`` whose unused
 slots hold null edges, which contribute exactly zero (DESIGN.md section 4.8).  So one graph replays every step
-whatever the step's edge count, and a step that needs more than ``capacity`` edges is re-captured.
+whatever the step's edge count, and a step that needs more than ``capacity`` edges is re-captured.  With
+``variable_cell=True`` the cell is an input of every step as well (constant-pressure MD): the neighbour list reads it
+from a device parameter block that is refreshed before each replay, and the step also returns stress and virial.
 """
 from __future__ import annotations
 
@@ -145,11 +147,11 @@ CAPACITY_SLACK = 0.02
 
 
 class GraphedMDStep(GraphedEnergyForces):
-    """One CUDA graph for a whole MD step in a fixed periodic cell: positions -> device neighbour list -> energy ->
-    forces.  ``g = GraphedMDStep(model, example); out = g(pos)``.
+    """One CUDA graph for a whole MD step in a periodic cell: positions -> device neighbour list -> energy -> forces.
+    ``g = GraphedMDStep(model, example); out = g(pos)``.
 
-    ``example`` holds CUDA tensors ``pos`` [N,3], ``atom_types`` [N] and ``cell`` [3,3] (all three directions periodic;
-    the cell is captured, so NVE / NVT).  ``capacity`` is the length of the edge buffer, by default
+    ``example`` holds CUDA tensors ``pos`` [N,3], ``atom_types`` [N] and ``cell`` [3,3] (all three directions periodic).
+    By default the cell is captured (NVE / NVT).  ``capacity`` is the length of the edge buffer, by default
     ``E0 + ceil(CAPACITY_SLACK * E0)`` with E0 the example's edge count; unused slots hold null edges.
 
     ``g(pos)`` takes host (pinned) or device positions and returns ``total_energy`` [1,1], ``atomic_energy`` [N,1],
@@ -157,9 +159,16 @@ class GraphedMDStep(GraphedEnergyForces):
     reads the step's edge count and overflow flag back (12 bytes, one event wait) and checks that the list was grouped
     by destination.  If the step needed more than ``capacity`` edges, the graph is re-captured with
     ``capacity = ceil(1.02 * needed)`` and the same positions are computed again, so a returned result never comes
-    from a truncated list; ``capacity`` only grows and ``recaptures`` counts the re-captures."""
+    from a truncated list; ``capacity`` only grows and ``recaptures`` counts the re-captures.
 
-    def __init__(self, model, example: Dict[str, torch.Tensor], capacity: Optional[int] = None, warmup: int = 3):
+    ``variable_cell=True`` (NPT): ``g(pos, cell)`` also takes the step's cell ([3,3], host or device; a device cell
+    costs one device-to-host read).  It is copied into the static ``cell`` input the model reads and handed to the
+    neighbour list (``ops.NeighborListPlan.set_cell``) before the replay.  The captured call is
+    ``model(d, compute_stress=True)``, so the outputs also hold ``stress`` and ``virial`` [1,3,3].  A re-capture
+    happens at the current cell, with a bin grid chosen for it."""
+
+    def __init__(self, model, example: Dict[str, torch.Tensor], capacity: Optional[int] = None, warmup: int = 3,
+                 variable_cell: bool = False):
         if example["pos"].device.type != "cuda":
             raise RuntimeError("GraphedMDStep needs CUDA tensors (there is no CPU path)")
         if example.get("cell") is None:
@@ -167,6 +176,7 @@ class GraphedMDStep(GraphedEnergyForces):
         if capacity is None:
             e0 = int(ops.neighbor_list(example["pos"], example["cell"], True, model.r_max)["edge_index"].shape[1])
             capacity = e0 + math.ceil(CAPACITY_SLACK * e0)
+        self.variable_cell = bool(variable_cell)
         self.recaptures = 0
         self._warmup = warmup
         self._num_edges_host = torch.zeros(1, dtype=torch.int64).pin_memory()
@@ -176,19 +186,22 @@ class GraphedMDStep(GraphedEnergyForces):
     def _capture(self, model, example: Dict[str, torch.Tensor], capacity: int) -> None:
         self.capacity = capacity
         self.plan = ops.NeighborListPlan(example["pos"].shape[0], example["cell"], True, model.r_max, capacity,
-                                         device=example["pos"].device)
+                                         device=example["pos"].device, variable_cell=self.variable_cell)
         super().__init__(model, example, warmup=self._warmup)
         ops.src_csr_cache.clear()  # like csr_cache: an entry made during the capture lives in the graph's pool
         out, self._out = self._out, None
         self.atomic_energy, self.num_edges, self.overflow = out["atomic_energy"], out["num_edges"], out["overflow"]
+        self.stress, self.virial = out.get("stress"), out.get("virial")
 
     def _run(self):
         nl = self.plan.run(self.static["pos"])
         d = dict(self.extra)
         d.update(self.static)
         d["edge_index"], d["edge_cell_shift"] = nl["edge_index"], nl["edge_cell_shift"]
-        out = self.model(d)
+        out = self.model(d, compute_stress=True) if self.variable_cell else self.model(d)
         self._out = {"atomic_energy": out["atomic_energy"], "num_edges": nl["num_edges"], "overflow": nl["overflow"]}
+        if self.variable_cell:
+            self._out.update(stress=out["stress"], virial=out["virial"])
         return out
 
     def _recapture(self, capacity: int) -> None:
@@ -197,13 +210,21 @@ class GraphedMDStep(GraphedEnergyForces):
         # drop every reference into the old graph's memory pool so that it is released with the graph
         self.graph = self.plan = None
         self.energy = self.forces = self.atomic_energy = self.num_edges = self.overflow = self.sorted_flag = None
+        self.stress = self.virial = None
         self._sorted_flags = []
         self._flag_event = None
         self._capture(self.model, example, capacity)
         self.replays = replays
         self.recaptures += 1
 
-    def __call__(self, pos: torch.Tensor) -> Dict[str, torch.Tensor]:
+    def __call__(self, pos: torch.Tensor, cell: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
+        if self.variable_cell:
+            if cell is None:
+                raise ValueError("GraphedMDStep(variable_cell=True) needs the step's cell: g(pos, cell)")
+            self.plan.set_cell(cell)  # checks the cell before anything is copied
+            self.static["cell"].copy_(torch.as_tensor(cell).reshape(self.static["cell"].shape), non_blocking=True)
+        elif cell is not None:
+            raise ValueError("this GraphedMDStep was captured for a fixed cell; build it with variable_cell=True")
         self.static["pos"].copy_(pos, non_blocking=True)
         while True:
             self.replay()
@@ -217,5 +238,8 @@ class GraphedMDStep(GraphedEnergyForces):
                 break
             needed = int(self._num_edges_host[0])
             self._recapture(max(self.capacity + 1, math.ceil(1.02 * needed)))
-        return {"total_energy": self.energy, "atomic_energy": self.atomic_energy, "forces": self.forces,
-                "num_edges": self.num_edges}
+        out = {"total_energy": self.energy, "atomic_energy": self.atomic_energy, "forces": self.forces,
+               "num_edges": self.num_edges}
+        if self.variable_cell:
+            out.update(stress=self.stress, virial=self.virial)
+        return out

@@ -783,18 +783,23 @@ def _nl_cell(cell, pbc):
 
 
 class _NlArgs:
-    """Host-side arguments of the nqb_nl_* calls: cell, inverse, periodicity, bin grid and search range."""
+    """Host-side arguments of the nqb_nl_* calls: cell, inverse, periodicity, bin grid and search range.
 
-    def __init__(self, N: int, cell_np, inv_np, pbc, r_max: float, lo, width):
+    ``nb`` (3 ints) fixes the bin grid instead of deriving it from the cell; the search range is still the one this
+    cell needs with that grid (a variable-cell ``NeighborListPlan`` keeps its grid, and so its scratch sizes)."""
+
+    def __init__(self, N: int, cell_np, inv_np, pbc, r_max: float, lo, width, nb=None):
         import numpy as np
 
         # distance between opposite faces along each lattice direction = 1 / |column d of the inverse|
         perp = 1.0 / np.linalg.norm(inv_np, axis=0)
-        nb, sr = [1, 1, 1], [1, 1, 1]
+        fixed = nb is not None
+        nb, sr = ([int(n) for n in nb] if fixed else [1, 1, 1]), [1, 1, 1]
         cap = max(1, int(round((4 * max(N, 1)) ** (1.0 / 3.0))))
         for d in range(3):
             extent = perp[d] * (1.0 if pbc[d] else width[d])
-            nb[d] = int(min(cap, max(1, np.floor(extent / r_max))))
+            if not fixed:
+                nb[d] = int(min(cap, max(1, np.floor(extent / r_max))))
             sr[d] = int(np.ceil(r_max / (extent / nb[d]) - 1e-12)) if pbc[d] else 1
             sr[d] = max(sr[d], 1)
         I3 = C.c_int * 3
@@ -822,18 +827,28 @@ def _nl_scratch(N: int, nbins: int, dev) -> Dict[str, torch.Tensor]:
     }
 
 
-def _nl_rows(pos: torch.Tensor, a: _NlArgs, s: Dict[str, torch.Tensor]) -> None:
+def _nl_rows(pos: torch.Tensor, a: _NlArgs, s: Dict[str, torch.Tensor],
+             params_dev: Optional[torch.Tensor] = None) -> None:
     """Bins, atoms sorted by bin, neighbours per atom and their exclusive scan into ``s["row_ptr"]``; all on the
-    device, no host synchronisation."""
+    device, no host synchronisation.  ``params_dev``: read the cell-dependent arguments from this device parameter
+    block (``nqb_nl_params_pack``) instead of passing ``a``'s by value."""
     L = _capi.lib()
     N = pos.shape[0]
     st = _stream()
-    _capi.check(L.nqb_nl_bin(_ptr(pos), N, a.cell, a.inv, a.pbc, a.nb, a.sr, a.lo, a.width, a.r_max, _ptr(s["wpos"]),
-                             _ptr(s["base"]), _ptr(s["binid"]), _ptr(s["cidx"]), st), "nqb_nl_bin")
+    if params_dev is None:
+        _capi.check(L.nqb_nl_bin(_ptr(pos), N, a.cell, a.inv, a.pbc, a.nb, a.sr, a.lo, a.width, a.r_max,
+                                 _ptr(s["wpos"]), _ptr(s["base"]), _ptr(s["binid"]), _ptr(s["cidx"]), st), "nqb_nl_bin")
+    else:
+        _capi.check(L.nqb_nl_bin_dp(_ptr(pos), N, _ptr(params_dev), _ptr(s["wpos"]), _ptr(s["base"]), _ptr(s["binid"]),
+                                    _ptr(s["cidx"]), st), "nqb_nl_bin_dp")
     torch.sort(s["binid"], stable=True, out=(s["sorted_bin"], s["order"]))
     torch.searchsorted(s["sorted_bin"], s["bins"], out=s["bin_start"])
-    _capi.check(L.nqb_nl_count(N, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, _ptr(s["wpos"]), _ptr(s["cidx"]),
-                               _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(s["counts"]), st), "nqb_nl_count")
+    if params_dev is None:
+        _capi.check(L.nqb_nl_count(N, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, _ptr(s["wpos"]), _ptr(s["cidx"]),
+                                   _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(s["counts"]), st), "nqb_nl_count")
+    else:
+        _capi.check(L.nqb_nl_count_dp(N, _ptr(params_dev), _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["order"]),
+                                      _ptr(s["bin_start"]), _ptr(s["counts"]), st), "nqb_nl_count_dp")
     torch.cumsum(s["counts"], 0, out=s["row_ptr"][1:])
 
 
@@ -895,14 +910,45 @@ def null_edge_shift(cell, r_max: float):
     return shift
 
 
+def _nl_cell_block(cell, r_max: float, nb, num_atoms: int):
+    """Host part of ``NeighborListPlan.set_cell``: checks ``cell`` ([3,3] or [1,3,3], finite, non-singular) and returns
+    the ``_NlArgs`` of this cell on the fixed bin grid ``nb`` (inverse as in ``neighbor_list``, search range for this
+    cell), its null-edge shift and the packed device parameter block (``nqb_nl_params_pack``, ctypes buffer)."""
+    import numpy as np
+
+    c = cell.detach().cpu().double().numpy() if torch.is_tensor(cell) else np.asarray(cell, dtype=np.float64)
+    if c.shape not in ((3, 3), (1, 3, 3)):
+        raise ValueError(f"set_cell: cell must be [3, 3] or [1, 3, 3], got {tuple(c.shape)}")
+    c = c.reshape(3, 3)
+    if not np.all(np.isfinite(c)):
+        raise ValueError("set_cell: cell is not finite")
+    vol = abs(float(np.linalg.det(c)))
+    if not vol > 1e-12 * float(np.prod(np.linalg.norm(c, axis=1))):
+        raise ValueError("set_cell: cell is singular")
+    pbc, cell_np, inv_np = _nl_cell(c, True)
+    a = _NlArgs(num_atoms, cell_np, inv_np, pbc, r_max, np.zeros(3), np.ones(3), nb=nb)
+    pad_shift = null_edge_shift(cell_np, r_max)
+    L = _capi.lib()
+    block = C.create_string_buffer(int(L.nqb_nl_params_bytes()))
+    _capi.check(L.nqb_nl_params_pack(a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, (C.c_double * 3)(*pad_shift), block),
+                "nqb_nl_params_pack")
+    return a, pad_shift, block
+
+
 class NeighborListPlan:
     """Device neighbour list of a fixed length ``capacity`` for one cell: positions in, list out, without a host
     synchronisation, so it can be captured in a CUDA graph (``graph.GraphedMDStep``).
 
     All host work (inverse cell, bin grid, search range, the null-edge shift) and every allocation happen here; the
-    cell is fixed for the plan's lifetime.  The cell must be given and periodic in all three directions: a
+    cell is fixed for the plan's lifetime unless ``variable_cell``.  The cell must be given and periodic in all three directions: a
     non-periodic direction needs the positions' bounding box on the host at every call.  A molecule in vacuum can use
     a large periodic box.
+
+    ``variable_cell=True`` (constant-pressure MD): the kernels read the cell-dependent arguments from a parameter
+    block in device memory, and ``set_cell(cell)`` replaces them between runs (or graph replays) without touching
+    the captured launches.  The bin grid chosen for the construction cell is kept for the plan's lifetime (the
+    scratch sizes depend on it); each cell gets the search range it needs on that grid, so any cell gives the exact
+    list and a cell far from the first one only costs more or less bin visits.  The null-edge shift follows the cell.
 
     ``run(pos)`` returns ``edge_index`` [2, capacity], ``edge_cell_shift`` [capacity, 3], ``row_ptr`` [N+1] (the
     padded destination CSR), ``num_edges`` [1] int64 (the true edge count E) and ``overflow`` [1] int32, all on the
@@ -910,7 +956,8 @@ class NeighborListPlan:
     then null edges (i, i, ``pad_shift``); each row gets floor or ceil of (capacity - E) / N of them.  When
     E > capacity, ``overflow`` is 1 and every row holds only null edges: the list must not be used."""
 
-    def __init__(self, num_atoms: int, cell, pbc, r_max: float, capacity: int, device=None):
+    def __init__(self, num_atoms: int, cell, pbc, r_max: float, capacity: int, device=None,
+                 variable_cell: bool = False):
         import numpy as np
 
         if cell is None:
@@ -938,6 +985,35 @@ class NeighborListPlan:
         self.row_ptr = torch.empty((N + 1,), dtype=torch.int64, device=dev)
         self.num_edges = torch.empty((1,), dtype=torch.int64, device=dev)
         self.overflow = torch.empty((1,), dtype=torch.int32, device=dev)
+        self.variable_cell = bool(variable_cell)
+        self._params_dev = None
+        if self.variable_cell:
+            self.nbins = tuple(self._a.nb)
+            nbytes = int(_capi.lib().nqb_nl_params_bytes())
+            self._params_dev = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+            self._params_host = torch.empty((nbytes,), dtype=torch.uint8).pin_memory()
+            self._params_event: Optional[torch.cuda.Event] = None
+            self.set_cell(cell)
+
+    def set_cell(self, cell) -> None:
+        """Make the following ``run`` calls (and replays of graphs that captured them) use ``cell`` ([3,3] or
+        [1,3,3], rows = lattice vectors).  A host call, not captured: it computes the inverse (as ``neighbor_list``
+        does), the search range on the plan's bin grid and the null-edge shift of this cell, packs them and copies the
+        block to the device asynchronously on the current stream, after the previous copy out of the staging block
+        has finished.  A CUDA ``cell`` costs one device-to-host read.  After ``set_cell(c)``, ``run(pos)`` holds the
+        rows of ``neighbor_list(pos, c)`` bit for bit.  Raises ``ValueError`` for a wrong shape, a non-finite or
+        singular cell and on a plan built without ``variable_cell``."""
+        if not self.variable_cell:
+            raise ValueError("NeighborListPlan.set_cell needs a plan built with variable_cell=True")
+        a, pad_shift, block = _nl_cell_block(cell, self.r_max, self.nbins, self.num_atoms)
+        if self._params_event is not None:
+            self._params_event.synchronize()
+        C.memmove(self._params_host.data_ptr(), block, len(block))
+        with torch.cuda.device(self.device):
+            self._params_dev.copy_(self._params_host, non_blocking=True)
+            self._params_event = torch.cuda.Event()
+            self._params_event.record()
+        self._a, self.pad_shift = a, pad_shift
 
     def run(self, pos: torch.Tensor) -> Dict[str, torch.Tensor]:
         _require_cuda(pos)
@@ -946,15 +1022,23 @@ class NeighborListPlan:
         pos = pos.detach().double().contiguous()
         L = _capi.lib()
         a, s = self._a, self._s
-        _nl_rows(pos, a, s)
+        _nl_rows(pos, a, s, self._params_dev)
         st = _stream()
         _capi.check(L.nqb_nl_pad(self.num_atoms, self.capacity, _ptr(s["row_ptr"]), _ptr(self.row_ptr),
                                  _ptr(self.num_edges), _ptr(self.overflow), st), "nqb_nl_pad")
-        _capi.check(L.nqb_nl_fill_capacity(self.num_atoms, self.capacity, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max,
-                                           _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["base"]), _ptr(s["order"]),
-                                           _ptr(s["bin_start"]), _ptr(self.row_ptr), _ptr(self.overflow),
-                                           self._pad_shift_c, _ptr(self.edge_index), _ptr(self.edge_cell_shift), st),
-                    "nqb_nl_fill_capacity")
+        if self.variable_cell:
+            _capi.check(L.nqb_nl_fill_capacity_dp(self.num_atoms, self.capacity, _ptr(self._params_dev),
+                                                  _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["base"]), _ptr(s["order"]),
+                                                  _ptr(s["bin_start"]), _ptr(self.row_ptr), _ptr(self.overflow),
+                                                  _ptr(self.edge_index), _ptr(self.edge_cell_shift), st),
+                        "nqb_nl_fill_capacity_dp")
+        else:
+            _capi.check(L.nqb_nl_fill_capacity(self.num_atoms, self.capacity, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max,
+                                               _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["base"]), _ptr(s["order"]),
+                                               _ptr(s["bin_start"]), _ptr(self.row_ptr), _ptr(self.overflow),
+                                               self._pad_shift_c, _ptr(self.edge_index), _ptr(self.edge_cell_shift),
+                                               st),
+                        "nqb_nl_fill_capacity")
         # the kernels write through raw pointers: bump the version counters so that the CSRs cached against these
         # buffers (csr_cache, src_csr_cache) are rebuilt for the new list
         for t in (self.edge_index, self.edge_cell_shift, self.row_ptr, self.num_edges, self.overflow):

@@ -10,8 +10,18 @@ Arms are timed A, B, A, B in one process; every 10th step B's energy and forces 
 positions.  ``pad`` lines time B on the frozen first frame with capacity E, 1.02 E and 1.05 E (the cost of the null
 edges).  The first line names the GPU, its power limit and its maximum SM clock.
 
+``--cell npt`` runs the same workloads with a cell that changes every step: ``cell(t) = cell0 @ S(t)`` and positions
+``oscillating_positions(pos0, t) @ S(t)`` with ``S = data.oscillating_strain`` (I + eps, eps symmetric, 2 % diagonal and
+3 % shear amplitude, period 50).  Positions and cells start on the device; each step ends with forces and stress on
+the host.
+  A: ``ops.neighbor_list`` + ``model(d, compute_stress=True)``;
+  B: ``GraphedMDStep(variable_cell=True)``, ``g(pos, cell)``.
+Timed A, B, A, B; every 10th step B's energy, forces and stress are compared with A's.  ``npt_overhead`` lines time the
+fixed-cell graph against the variable-cell graph on the frozen first frame, alternated (the cost of the device
+parameter block plus the stress).
+
     python tools/bench_md.py [--workloads water_1k_l2_f32,li3po4_10k_l2_f64,S_li3po4_10k] [--steps 100]
-                             [--warmup 10] [--out FILE]
+                             [--warmup 10] [--cell fixed|npt] [--out FILE]
 """
 import argparse
 import json
@@ -161,11 +171,106 @@ def run_workload(workload, steps, warmup, sink):
         torch.cuda.empty_cache()
 
 
+def arm_eager_npt(model, dev, frames, keep):
+    from nequip_b200 import ops
+
+    kept, counts = {}, []
+    for t, (pos, cell) in enumerate(frames):
+        nl = ops.neighbor_list(pos, cell, True, R_MAX)
+        out = model(dict(dev, pos=pos, cell=cell, edge_index=nl["edge_index"], edge_cell_shift=nl["edge_cell_shift"]),
+                    compute_stress=True)
+        f, s = out["forces"].cpu(), out["stress"].cpu()
+        counts.append(int(nl["edge_index"].shape[1]))
+        if keep and t % 10 == 0:
+            kept[t] = (float(out["total_energy"]), f, s)
+    return kept, counts
+
+
+def arm_graph_npt(g, frames, keep):
+    kept, counts = {}, []
+    for t, (pos, cell) in enumerate(frames):
+        out = g(pos, cell)
+        f, s = out["forces"].cpu(), out["stress"].cpu()
+        counts.append(int(g._num_edges_host[0]))  # read back by the call itself
+        if keep and t % 10 == 0:
+            kept[t] = (float(out["total_energy"]), f, s)
+    return kept, counts
+
+
+def run_workload_npt(workload, steps, warmup, sink):
+    import torch
+
+    from nequip_b200 import data as D
+    from nequip_b200.graph import GraphedMDStep
+
+    model, dev, E0 = build(workload)
+    N = dev["pos"].shape[0]
+    pos0, cell0 = dev["pos"].clone(), dev["cell"].clone()
+
+    def frame(t):
+        S = D.oscillating_strain(t, PERIOD).cuda()
+        return D.oscillating_positions(pos0, t, PERIOD, AMPLITUDE, seed=1) @ S, cell0 @ S
+
+    frames = [frame(t) for t in range(steps)]
+    warm = [frame(-1 - t) for t in range(warmup)]
+    g = GraphedMDStep(model, dev, variable_cell=True)
+    cap0 = g.capacity
+    ms = {"A": [], "B": []}
+    ref, got, counts = None, None, None
+    for rep in range(2):
+        t_a, ref, counts = timed(lambda p, k: arm_eager_npt(model, dev, p, k), warm, frames)
+        t_b, got, counts_b = timed(lambda p, k: arm_graph_npt(g, p, k), warm, frames)
+        if counts_b != counts:
+            raise RuntimeError(f"{workload}: graphed edge counts differ from the eager list's")
+        ms["A"].append(t_a)
+        ms["B"].append(t_b)
+        emit({"kind": "npt_rep", "workload": workload, "rep": rep, "A_eager_ms_per_step": round(t_a, 4),
+              "B_graph_ms_per_step": round(t_b, 4)}, sink)
+    de, df, ds = 0.0, 0.0, 0.0
+    for t, (e_a, f_a, s_a) in ref.items():
+        e_b, f_b, s_b = got[t]
+        de = max(de, abs(e_b - e_a) / abs(e_a))
+        df = max(df, float((f_b - f_a).abs().max()) / float(f_a.abs().max()))
+        ds = max(ds, float((s_b - s_a).abs().max()) / float(s_a.abs().max()))
+    vols = [abs(float(torch.linalg.det(c))) for _p, c in frames]
+    emit({"kind": "npt", "workload": workload, "atoms": N, "E0": E0, "steps": steps, "period": PERIOD,
+          "amplitude_A": AMPLITUDE, "strain_diagonal": 0.02, "strain_shear": 0.03,
+          "volume_over_V0_min": round(min(vols) / vols[0], 5), "volume_over_V0_max": round(max(vols) / vols[0], 5),
+          "A_eager_ms_per_step": [round(x, 4) for x in ms["A"]],
+          "B_graph_ms_per_step": [round(x, 4) for x in ms["B"]],
+          "speedup_B_over_A": round(min(ms["A"]) / min(ms["B"]), 3),
+          "E_over_E0_min": round(min(counts) / E0, 5), "E_over_E0_max": round(max(counts) / E0, 5),
+          "capacity_initial": cap0, "capacity_final": g.capacity, "recaptures": g.recaptures,
+          "launches_per_replay": g.launches_per_replay, "checked_steps": len(ref),
+          "max_rel_energy_dev_B_vs_A": de, "max_force_dev_B_vs_A_over_max_F": df,
+          "max_stress_dev_B_vs_A_over_max_stress": ds}, sink)
+    del g
+    torch.cuda.empty_cache()
+    # cost of the variable cell: fixed-cell graph against variable-cell graph on the frozen first frame, alternated
+    g_fixed = GraphedMDStep(model, dev)
+    g_var = GraphedMDStep(model, dev, variable_cell=True)
+    frozen = [(pos0, cell0)] * steps
+    fixed_ms, var_ms = [], []
+    for _rep in range(2):
+        t_f, _, _ = timed(lambda p, k: arm_graph(g_fixed, [q for q, _c in p], False), frozen[:warmup], frozen)
+        t_v, _, _ = timed(lambda p, k: arm_graph_npt(g_var, p, False), frozen[:warmup], frozen)
+        fixed_ms.append(round(t_f, 4))
+        var_ms.append(round(t_v, 4))
+    emit({"kind": "npt_overhead", "workload": workload, "capacity_fixed": g_fixed.capacity,
+          "capacity_variable": g_var.capacity, "fixed_cell_graph_ms_per_step": fixed_ms,
+          "variable_cell_graph_ms_per_step": var_ms,
+          "variable_over_fixed": round(min(var_ms) / min(fixed_ms), 3)}, sink)
+    del g_fixed, g_var
+    torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workloads", default=",".join(WORKLOADS))
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--cell", choices=("fixed", "npt"), default="fixed",
+                    help="fixed: the cell of the first frame throughout; npt: a cell that changes every step")
     ap.add_argument("--out", default=None, help="also write the JSON lines to this file")
     args = ap.parse_args()
     import torch
@@ -174,7 +279,7 @@ def main():
     sink = []
     emit(gpu_info(), sink)
     for w in args.workloads.split(","):
-        run_workload(w, args.steps, args.warmup, sink)
+        (run_workload_npt if args.cell == "npt" else run_workload)(w, args.steps, args.warmup, sink)
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         with open(args.out, "w") as fh:
