@@ -250,6 +250,22 @@ int nqb_gemm_prepare(const float* B, int64_t ldb, int K, int N, int transposed, 
 int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
                      int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
                      const float* rowscale_base, int64_t rs_ld, int64_t M, nqb_stream_t st);
+/* The same GEMM with an activation epilogue (the radial MLP's hidden layers, SiLU).  With v the finished value
+ * (after the row scale), three more flag bits apply per problem:
+ *   bit3  C = silu(v) instead of v;
+ *   bit4  also aux = v (the pre-activation);
+ *   bit5  C = v * silu'(aux)  with  silu'(p) = s(p) (1 + p (1 - s(p))),  s = sigmoid  (the gradient through the
+ *         activation whose pre-activation was saved with bit4).
+ * aux is addressed like C: element (m, n) of problem p is aux_base[c_off + m * ldc + n].  Bits 3-5 are never
+ * combined with bit0 or bit2 (the host rejects it).  Problems without bits 3-5 behave as in nqb_gemm_grouped.
+ * Write contract: with bit3 or bit4, C (and with bit4 aux) is fully written in rows < M, columns < N_p, and nothing
+ * else of C or aux is written; with bit5, aux is read in rows < M, columns < N_p only, and C is fully written there.
+ * aux_base must be non-null and 16-byte aligned (checked: an error, no launch; the entry point cannot see the
+ * device descriptors, so it requires aux even when only bit3 is used, in which case aux is never touched and
+ * c_base may be passed). */
+int nqb_gemm_grouped_act(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
+                         int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
+                         const float* rowscale_base, int64_t rs_ld, int64_t M, float* aux_base, nqb_stream_t st);
 
 /* Gate nonlinearity (e3nn nn.Gate with normalize2mom'd SiLU for even / tanh for odd scalars and gates,
  * nequip/nn/convnetlayer.py:42-56,104-112), one kernel per direction.  Column tables (device, int32) are

@@ -71,6 +71,7 @@ SIGNATURES = {
     "nqb_gate_fwd": (_i32, [_i32, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "nqb_gate_bwd": (_i32, [_i32, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
     "nqb_gemm_grouped": (_i32, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i64, _i64, _vp]),
+    "nqb_gemm_grouped_act": (_i32, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
 }
 
 

@@ -25,6 +25,7 @@
 // slots (mbarrier complete_tx); a problem with K <= 128 keeps its chunks resident for all of the CTA's M-tiles.
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdio.h>
 
 #include "../../include/nqb.h"
 #include "nqb_tc.cuh"
@@ -111,10 +112,13 @@ __device__ __forceinline__ void decode_q(const GemmDesc* descs, int ndesc, int q
 
 __device__ __forceinline__ void bar_wg(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
+// ACT = false: the plain GEMM.  ACT = true also honours the activation bits 3-5 of a problem's flags in the
+// epilogue, with the auxiliary matrix at aux_base (addressed with C's c_off and ldc); see nqb.h.
+template <bool ACT>
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const int32_t* __restrict__ tile_ctas,
          int sched_ctas, const float* __restrict__ a_base, const float* __restrict__ b_base, float* __restrict__ c_base,
-         const float* __restrict__ rs_base, int64_t rs_ld, int64_t M) {
+         const float* __restrict__ rs_base, int64_t rs_ld, int64_t M, float* __restrict__ aux_base) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& S = *reinterpret_cast<Smem*>(smem_raw);
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
@@ -216,9 +220,12 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
     //        bit1 rows whose row scale is zero are not touched (disjoint row-masked writers),
     //        bit2 accumulate with red.global.add (several problems of this launch add into the same C)
     // both accumulate modes add with red.global (performed at L2)
+    // ACT only (never with bit0 / bit2): bit3 store silu(v), bit4 also store v to aux, bit5 store v * silu'(aux)
     const bool reduce = (d->flags & 5) != 0, skipz = (d->flags & 2) != 0;
     const int64_t ldc = d->ldc;
     float* C = c_base + d->c_off + (int64_t)w.nt * TN;
+    [[maybe_unused]] const int act = ACT ? (int)(d->flags >> 3) & 7 : 0;
+    [[maybe_unused]] float* X = ACT && (act & 6) ? aux_base + d->c_off + (int64_t)w.nt * TN : nullptr;
     bool first_mt = true;
     for (int64_t mt = sch.m_start; mt < mtiles; mt += sch.m_step) {
       for (int seg = 0; seg < nseg; ++seg) {
@@ -287,7 +294,24 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
 #pragma unroll
         for (int j = 0; j < TN / 8; ++j) {
           if (j * 8 + c0 < w.ncols) {
-            const float v0 = hh[4 * j + 2 * half] * rs, v1 = hh[4 * j + 2 * half + 1] * rs;
+            float v0 = hh[4 * j + 2 * half] * rs, v1 = hh[4 * j + 2 * half + 1] * rs;
+            if constexpr (ACT) {
+              if (act != 0) {
+                float* xp = X + m * ldc + c0 + j * 8;
+                if (act & 4) {  // gradient through the activation: silu'(p) = s (1 + p (1 - s))
+                  const float2 p = *reinterpret_cast<const float2*>(xp);
+                  const float s0 = sigmoid(p.x), s1 = sigmoid(p.y);
+                  v0 *= s0 * fmaf(p.x, 1.0f - s0, 1.0f);
+                  v1 *= s1 * fmaf(p.y, 1.0f - s1, 1.0f);
+                } else {
+                  if (act & 2) *reinterpret_cast<float2*>(xp) = make_float2(v0, v1);
+                  if (act & 1) {
+                    v0 *= sigmoid(v0);
+                    v1 *= sigmoid(v1);
+                  }
+                }
+              }
+            }
             if (reduce)
               asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(crow + j * 8), "f"(v0), "f"(v1) : "memory");
             else
@@ -366,20 +390,31 @@ extern "C" int nqb_gemm_prepare(const float* B, int64_t ldb, int K, int N, int t
   return 0;
 }
 
-extern "C" int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
-                                int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
-                                const float* rowscale_base, int64_t rs_ld, int64_t M, nqb_stream_t st) {
-  if (ndesc <= 0 || ntiles_total <= 0) return nqb_set_error("nqb_gemm_grouped: empty problem list");
-  if (M < 0) return nqb_set_error("nqb_gemm_grouped: negative M");
+// the launcher of both entry points; errors are reported under the entry point's name
+template <bool ACT>
+static int gemm_grouped_launch(const char* who, const void* descs_dev, int ndesc, int ntiles_total,
+                               const int32_t* tile_ctas_dev, int sched_ctas, const float* a_base,
+                               const float* prepared_base, float* c_base, float* aux_base, const float* rowscale_base,
+                               int64_t rs_ld, int64_t M, nqb_stream_t st) {
+  auto fail = [&](const char* what) {
+    char msg[160];  // nqb_set_error copies it
+    snprintf(msg, sizeof(msg), "%s: %s", who, what);
+    return nqb_set_error(msg);
+  };
+  if (ndesc <= 0 || ntiles_total <= 0) return fail("empty problem list");
+  if (M < 0) return fail("negative M");
   if (M == 0) return 0;
-  if (!descs_dev || !a_base || !prepared_base || !c_base) return nqb_set_error("nqb_gemm_grouped: null pointer");
-  // A is staged with 16-byte cp.async, the weights with bulk copies, C is stored in float2 pairs
-  if (((uintptr_t)a_base | (uintptr_t)prepared_base | (uintptr_t)c_base) & 15)
-    return nqb_set_error("nqb_gemm_grouped: a_base, prepared_base and c_base must be 16-byte aligned");
+  if (!descs_dev || !a_base || !prepared_base || !c_base) return fail("null pointer");
+  // the device descriptors cannot be read here: an activation launch always takes an aux matrix
+  if (ACT && !aux_base) return fail("aux_base is null (bit4 / bit5 problems store to or read from it)");
+  // A is staged with 16-byte cp.async, the weights with bulk copies, C and aux are stored in float2 pairs
+  if (((uintptr_t)a_base | (uintptr_t)prepared_base | (uintptr_t)c_base | (uintptr_t)aux_base) & 15)
+    return fail(ACT ? "a_base, prepared_base, c_base and aux_base must be 16-byte aligned"
+                    : "a_base, prepared_base and c_base must be 16-byte aligned");
   static bool attr_set[64] = {false};
   const int dev = gemm_device();
   if (!attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(k_gemm3x, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem) + 1024);
+    cudaError_t e = cudaFuncSetAttribute(k_gemm3x<ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem) + 1024);
     if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
     attr_set[dev] = true;
   }
@@ -387,10 +422,26 @@ extern "C" int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_tot
   int grid = (int)(nwork < gemm_sm_count() ? nwork : gemm_sm_count());
   if (tile_ctas_dev != nullptr && sched_ctas > 0 && sched_ctas <= gemm_sm_count()) grid = sched_ctas;
   else tile_ctas_dev = nullptr;
-  k_gemm3x<<<grid, NTHREADS, sizeof(Smem) + 1024, (cudaStream_t)st>>>((const GemmDesc*)descs_dev, ndesc, ntiles_total, tile_ctas_dev, sched_ctas, a_base,
-                                                                 prepared_base, c_base, rowscale_base, rs_ld, M);
+  k_gemm3x<ACT><<<grid, NTHREADS, sizeof(Smem) + 1024, (cudaStream_t)st>>>(
+      (const GemmDesc*)descs_dev, ndesc, ntiles_total, tile_ctas_dev, sched_ctas, a_base, prepared_base, c_base,
+      rowscale_base, rs_ld, M, aux_base);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
   return 0;
+}
+
+extern "C" int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
+                                int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
+                                const float* rowscale_base, int64_t rs_ld, int64_t M, nqb_stream_t st) {
+  return gemm_grouped_launch<false>("nqb_gemm_grouped", descs_dev, ndesc, ntiles_total, tile_ctas_dev, sched_ctas,
+                                    a_base, prepared_base, c_base, nullptr, rowscale_base, rs_ld, M, st);
+}
+
+extern "C" int nqb_gemm_grouped_act(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
+                                    int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
+                                    const float* rowscale_base, int64_t rs_ld, int64_t M, float* aux_base,
+                                    nqb_stream_t st) {
+  return gemm_grouped_launch<true>("nqb_gemm_grouped_act", descs_dev, ndesc, ntiles_total, tile_ctas_dev, sched_ctas,
+                                   a_base, prepared_base, c_base, aux_base, rowscale_base, rs_ld, M, st);
 }

@@ -30,19 +30,6 @@ constexpr int NB = 8;        // Bessel functions
 //     4 x 8 partial sums are reduced with one 32-value halving butterfly (31 shuffles) that leaves
 //     element `lane` in lane `lane`: grad_emb is written as one 128-byte row.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float ex2_approx(float x) {
-  float r;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-__device__ __forceinline__ float rcp_approx(float x) {
-  float r;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-// 1 / (1 + exp(-p));  p -> -inf gives rcp(inf) = 0, p -> +inf gives rcp(1) = 1
-__device__ __forceinline__ float sigmoid(float p) { return rcp_approx(1.0f + ex2_approx(p * -1.4426950408889634f)); }
-
 struct Basis8 { float4 a, b; };
 __device__ __forceinline__ Basis8 load_basis(const float* __restrict__ emb, int64_t e, int64_t E) {
   Basis8 r;

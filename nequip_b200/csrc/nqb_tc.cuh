@@ -140,6 +140,20 @@ __device__ __forceinline__ float2 fmul2_rn(float2 a, float2 b) { return make_flo
 
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x)); }
 
+// sigmoid from the SFU: ex2.approx / rcp.approx (the radial-MLP hidden layers, nqb_mlp.cu and nqb_gemm.cu)
+__device__ __forceinline__ float ex2_approx(float x) {
+  float r;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+  return r;
+}
+__device__ __forceinline__ float rcp_approx(float x) {
+  float r;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+  return r;
+}
+// 1 / (1 + exp(-p));  p -> -inf gives rcp(inf) = 0, p -> +inf gives rcp(1) = 1
+__device__ __forceinline__ float sigmoid(float p) { return rcp_approx(1.0f + ex2_approx(p * -1.4426950408889634f)); }
+
 // canonical K-major offset (in floats) of element (row, k) in a tile with `kgroups` 16-byte groups along K
 __device__ __forceinline__ int canon_off(int row, int k, int kgroups) {
   return (row >> 3) * (kgroups * 32) + (k >> 2) * 32 + (row & 7) * 4 + (k & 3);

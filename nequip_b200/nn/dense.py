@@ -4,7 +4,8 @@ channel-contiguous ``ir_mul`` node layout).
 Each block is ONE launch of the grouped 3xTF32 GEMM (``nequip_b200/csrc/nqb_gemm.cu``) per
 direction; the weights are prepared (scaled, split hi/lo, tiled) once.  Reference ops:
 
-* ``RadialMLPGemm``      ScalarMLPFunction, depth 1            nequip/nn/mlp.py:80-195, 262-268
+* ``RadialMLPGemm``      ScalarMLPFunction, depth >= 1 (one launch per layer, SiLU in the GEMM epilogue)
+                         nequip/nn/mlp.py:80-195, 262-268
 * ``IrrepsLinearGemm``   e3nn o3.Linear (linear_1, linear_2)   nequip/nn/interaction_block.py:82-87,129-138
 * ``SelfConnectionGemm`` e3nn FullyConnectedTensorProduct(x, node_attrs) with node_attrs =
                          type_embed[atom_types]                nequip/nn/interaction_block.py:140-146,175
@@ -146,59 +147,129 @@ class SelfConnectionGemm:
 # ---------------------------------------------------------------------------------------
 class _RadialMLPGemmFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, emb, mlp: "RadialMLPGemm"):
+    def forward(ctx, emb, mlp: "RadialMLPGemm", need_bwd: bool):
         E = emb.shape[0]
         out = torch.empty((E, mlp.W), dtype=emb.dtype, device=emb.device)
-        mlp.fwd.run(mlp.hidden(emb), out, E)
+        pre = [] if need_bwd else None
+        mlp.fwd.run(mlp.hidden(emb, pre), out, E)
         ctx.mlp = mlp
-        ctx.save_for_backward(emb)  # the pre-activation is recomputed in the backward (8 FMAs per value)
+        if need_bwd:
+            ctx.save_for_backward(emb, *pre)
         return out
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, gw):
-        (emb,) = ctx.saved_tensors
-        return ctx.mlp.grad_emb(emb, gw), None
+        emb, *pre = ctx.saved_tensors
+        return ctx.mlp.grad_emb(emb, gw, pre), None, None
 
 
 class RadialMLPGemm:
-    def __init__(self, lin1, lin2, device):
-        self.w1s = (lin1.weight.detach() * lin1.alpha).contiguous()
-        hid, W = lin2.weight.shape
-        self.W = W
-        a2 = float(lin2.alpha)
-        self.fwd = ops.GroupedGemm([ops.GemmProblem(0, hid, 0, W, lin2.weight.detach(), scale=a2)], device)
-        self.bwd = ops.GroupedGemm([ops.GemmProblem(0, W, 0, hid, lin2.weight.detach(), scale=a2, transposed=True)], device)
-        # the CUDA-core hidden-layer kernels are built for [E, 8] x [8, 128] only; other widths run through torch
-        self._hidden_kernel = tuple(self.w1s.shape) == (8, 128)
+    """ScalarMLPFunction of any depth >= 1 (no bias, SiLU between layers) on the project's kernels.
+
+    ``first`` [num_bessels, H], ``middle`` [H, H] each, ``last`` [H, W] (``ScalarLinearLayer`` modules).
+    Forward: the first layer runs on ``k_hidden_fwd`` when it is [8, 128], otherwise as a ``k_gemm3x`` problem with
+    the SiLU epilogue (K = num_bessels); every middle layer is one such problem; the last layer is a plain problem.
+    With a backward pass ahead, each hidden layer on ``k_gemm3x`` also stores its pre-activation ([E, H] float32).
+    Backward: the transposed GEMM of each layer multiplies by silu' of the saved pre-activation of the layer below;
+    into an [8, 128] first layer it gives grad_h for ``k_hidden_bwd`` (pre-activation recomputed), and a generic
+    first layer ends with a plain transposed GEMM into grad_emb [E, num_bessels]."""
+
+    def __init__(self, first, last, device, middle=()):
+        self.w1s = (first.weight.detach() * first.alpha).contiguous()
+        self.W = last.weight.shape[1]
+        plan = self.plan(first, last, middle)
+        self._hidden_kernel = plan["hidden_kernel"]
+
+        def gemm(p):
+            return ops.GroupedGemm([p], device)
+
+        self.fwd = gemm(plan["fwd"])
+        # the last layer's plain transposed GEMM, grad_h = gw @ (W_last a)^T
+        self.bwd = gemm(plan["bwd"])
+        self._hidden = [(gemm(save), gemm(plain), save.B.shape[1]) for save, plain in plan["hidden"]]
+        self._chain = [(self.bwd if p is plan["bwd"] else gemm(p), width, pre) for p, width, pre in plan["chain"]]
 
     @staticmethod
-    def supported(lin1, lin2, dtype) -> bool:
-        return dtype == torch.float32 and lin2.weight.shape[0] % 4 == 0 and lin2.weight.shape[1] % 4 == 0
+    def uses_hidden_kernel(first) -> bool:
+        """The CUDA-core hidden-layer kernels are built for [E, 8] x [8, 128] only."""
+        return tuple(first.weight.shape) == (8, 128)
 
-    def hidden(self, emb):
-        """``h = silu(emb @ w1s)``."""
-        if self._hidden_kernel:
-            h = torch.empty((emb.shape[0], self.w1s.shape[1]), dtype=emb.dtype, device=emb.device)
-            ops.mlp_hidden_fwd(emb, self.w1s, h)
-            return h
-        return torch.nn.functional.silu(torch.mm(emb, self.w1s))
+    @classmethod
+    def plan(cls, first, last, middle=()):
+        """The grouped-GEMM problems of the forward and backward pass (needs no device):
 
-    def grad_emb(self, emb, gw):
-        """Gradient of ``emb`` from the gradient ``gw`` of the edge weights: the transposed second-layer GEMM gives
-        ``grad_h``, then the hidden layer's backward (pre-activation recomputed)."""
+        * ``hidden``: per hidden layer on ``k_gemm3x``, in order, its ("silu_save", "silu") problems;
+        * ``fwd`` / ``bwd``: the last layer's problem and its plain transposed problem;
+        * ``chain``: the backward launches in order, (problem, output width, index into the saved pre-activations
+          of the ``hidden`` layers or None);
+        * ``hidden_kernel``: the first layer runs on ``k_hidden_fwd`` / ``k_hidden_bwd``."""
+
+        def prob(lin, act="none", transposed=False):
+            k, n = lin.weight.shape
+            lda, ldc = (n, k) if transposed else (k, n)
+            return ops.GemmProblem(0, lda, 0, ldc, lin.weight.detach(), scale=float(lin.alpha), transposed=transposed,
+                                   act=act)
+
+        layers = [first, *middle, last]
+        kernel = cls.uses_hidden_kernel(first)
+        skip = 1 if kernel else 0  # hidden layers before the first one on k_gemm3x
+        bwd = prob(last, transposed=True)
+        chain = []
+        for i in range(len(layers) - 1, 0, -1):  # layer i's transposed GEMM, then silu' of hidden layer i - 1
+            pre = i - 1 - skip
+            if pre >= 0:
+                p = prob(layers[i], "silu_grad", True)
+            else:  # into k_hidden_bwd: plain grad_h
+                p = bwd if i == len(layers) - 1 else prob(layers[i], transposed=True)
+            chain.append((p, layers[i].weight.shape[0], pre if pre >= 0 else None))
+        if not kernel:
+            chain.append((prob(first, transposed=True), first.weight.shape[0], None))
+        return dict(hidden_kernel=kernel, hidden=[(prob(l, "silu_save"), prob(l, "silu")) for l in layers[skip:-1]],
+                    fwd=prob(last), bwd=bwd, chain=chain)
+
+    @staticmethod
+    def supported(first, last, dtype, middle=()) -> bool:
+        """float32, and num_bessels and every width a multiple of 4 (the grouped GEMM's K, N and strides)."""
+        dims = [first.weight.shape[0]] + [l.weight.shape[1] for l in (first, *middle, last)]
+        return dtype == torch.float32 and all(d % 4 == 0 for d in dims)
+
+    def hidden(self, emb, pre: Optional[list] = None):
+        """The last hidden activation ``silu(... silu(emb @ w1s) ...)``.  ``pre``: a list that receives the
+        pre-activation of every hidden layer on ``k_gemm3x`` (what ``grad_emb`` needs); None keeps none."""
         E = emb.shape[0]
-        gh = torch.empty((E, self.w1s.shape[1]), dtype=emb.dtype, device=emb.device)
-        self.bwd.run(gw.contiguous(), gh, E)
+        x = emb
+        if self._hidden_kernel:
+            x = torch.empty((E, self.w1s.shape[1]), dtype=emb.dtype, device=emb.device)
+            ops.mlp_hidden_fwd(emb, self.w1s, x)
+        for save, plain, width in self._hidden:
+            h = torch.empty((E, width), dtype=emb.dtype, device=emb.device)
+            if pre is None:
+                plain.run(x, h, E)
+            else:
+                p = torch.empty((E, width), dtype=emb.dtype, device=emb.device)
+                save.run(x, h, E, aux=p)
+                pre.append(p)
+            x = h
+        return x
+
+    def grad_emb(self, emb, gw, pre=()):
+        """Gradient of ``emb`` from the gradient ``gw`` of the edge weights, with ``pre`` the pre-activations that
+        ``hidden`` saved."""
+        E = emb.shape[0]
+        g = gw.contiguous()
+        for gemm, width, k in self._chain:
+            out = torch.empty((E, width), dtype=g.dtype, device=g.device)
+            gemm.run(g, out, E, aux=None if k is None else pre[k])
+            g = out
         if self._hidden_kernel:
             gemb = torch.empty_like(emb)
-            ops.mlp_hidden_bwd(emb, self.w1s, gh, gemb)
+            ops.mlp_hidden_bwd(emb, self.w1s, g, gemb)
             return gemb
-        pre = torch.mm(emb, self.w1s)
-        return torch.mm(torch.ops.aten.silu_backward(gh, pre), self.w1s.t())
+        return g
 
     def __call__(self, emb):
-        return _RadialMLPGemmFn.apply(emb.contiguous(), self)
+        return _RadialMLPGemmFn.apply(emb.contiguous(), self, torch.is_grad_enabled() and emb.requires_grad)
 
 
 # ---------------------------------------------------------------------------------------
@@ -208,28 +279,30 @@ class _FusedRadialTPFn(torch.autograd.Function):
     they are written once on the side only when a backward pass will need them)."""
 
     @staticmethod
-    def forward(ctx, emb, x, y, edge_src, mod: "FusedRadialTP", csr):
-        h = mod.mlp.hidden(emb)
+    def forward(ctx, emb, x, y, edge_src, mod: "FusedRadialTP", csr, need_emb_grad: bool):
+        pre = [] if need_emb_grad else None
+        h = mod.mlp.hidden(emb, pre)
         need_bwd = any(ctx.needs_input_grad[:3])
         out, w = ops.tp_fused_fwd(mod.fw, x, y, h, edge_src, csr, want_w=need_bwd)
         ctx.mod, ctx.csr = mod, csr
         if need_bwd:
-            ctx.save_for_backward(emb, x, y, w, edge_src)
+            ctx.save_for_backward(emb, x, y, w, edge_src, *(pre or ()))
         return out
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, gout):
-        emb, x, y, w, edge_src = ctx.saved_tensors
+        emb, x, y, w, edge_src, *pre = ctx.saved_tensors
         mod = ctx.mod
         gx, gy, gw = ops.tp_scatter_bwd_raw(mod.plan, x, y, w, edge_src, ctx.csr, gout, need_x=ctx.needs_input_grad[1])
-        gemb = mod.mlp.grad_emb(emb, gw) if ctx.needs_input_grad[0] else None
-        return gemb, gx, (gy if ctx.needs_input_grad[2] else None), None, None, None
+        gemb = mod.mlp.grad_emb(emb, gw, pre) if ctx.needs_input_grad[0] else None
+        return gemb, gx, (gy if ctx.needs_input_grad[2] else None), None, None, None, None
 
 
 class FusedRadialTP:
-    """Radial MLP (one hidden layer) + TensorProductScatter of one interaction layer as a single forward kernel
-    (``nqb_tp_fused_fwd``); backward = ``nqb_tp_scatter_bwd`` + the layer's ``RadialMLPGemm.grad_emb``."""
+    """Radial MLP (any depth; the last layer fused) + TensorProductScatter of one interaction layer as a single
+    forward kernel (``nqb_tp_fused_fwd``) after the hidden layers; backward = ``nqb_tp_scatter_bwd`` + the layer's
+    ``RadialMLPGemm.grad_emb``."""
 
     def __init__(self, mlp: RadialMLPGemm, lin2, plan: ops.TPPlan, device):
         """``mlp``: the layer's unfused radial MLP (built from the same weights), whose hidden layer and backward GEMM
@@ -249,4 +322,5 @@ class FusedRadialTP:
         csr = ops.csr_cache.get(edge_dst.long().contiguous() if edge_dst.dtype != torch.int64 else edge_dst, x.shape[0])
         if csr.perm is not None:
             return None  # unsorted neighbour list: the caller uses the unfused kernels (which take the permutation)
-        return _FusedRadialTPFn.apply(emb.contiguous(), x.contiguous(), y.contiguous(), edge_src.long().contiguous(), self, csr)
+        return _FusedRadialTPFn.apply(emb.contiguous(), x.contiguous(), y.contiguous(), edge_src.long().contiguous(), self, csr,
+                                      torch.is_grad_enabled() and emb.requires_grad)

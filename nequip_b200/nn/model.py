@@ -427,8 +427,8 @@ class InteractionBlock(torch.nn.Module):
             if tc["mlp"] is not None:
                 w = tc["mlp"](edge_embedding)
             else:
-                self._note_fallback("radial MLP shape not supported by the grouped GEMM (needs one hidden layer, "
-                                    "widths multiples of 4)")
+                self._note_fallback("radial MLP shape not supported by the grouped GEMM (needs at least one hidden "
+                                    "layer, num_bessels and widths multiples of 4)")
                 w = self._edge_weights(edge_embedding)
             x = self.tp_scatter(x=x, edge_attr=edge_attrs, edge_weight=w, edge_dst=edge_index[0], edge_src=edge_index[1])
             if n_own is not None:
@@ -483,11 +483,11 @@ class InteractionBlock(torch.nn.Module):
         dev = x.device
         lins = [m for m in self.edge_mlp.mlp if isinstance(m, ScalarLinearLayer)]
         mlp = fused = None
-        if len(lins) == 2 and dense.RadialMLPGemm.supported(lins[0], lins[1], x.dtype):
-            mlp = dense.RadialMLPGemm(lins[0], lins[1], dev)
-            # FusedRadialTP.supported implies RadialMLPGemm.supported: the fused block shares the layer's mlp
-            if dense.FusedRadialTP.supported(lins[0], lins[1], self.tp_scatter._plan, x.dtype):
-                fused = dense.FusedRadialTP(mlp, lins[1], self.tp_scatter._plan, dev)
+        if len(lins) >= 2 and dense.RadialMLPGemm.supported(lins[0], lins[-1], x.dtype, middle=lins[1:-1]):
+            mlp = dense.RadialMLPGemm(lins[0], lins[-1], dev, middle=lins[1:-1])
+            # the fused block shares the layer's mlp (its hidden layers and backward GEMMs)
+            if dense.FusedRadialTP.supported(lins[0], lins[-1], self.tp_scatter._plan, x.dtype):
+                fused = dense.FusedRadialTP(mlp, lins[-1], self.tp_scatter._plan, dev)
         blocks = dict(
             fused=fused,
             lin1=(dense.IrrepsLinearGemm(self.linear_1, dev, extra_scale=float(self.norm_const.view(-1)[0]))

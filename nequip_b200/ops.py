@@ -584,6 +584,15 @@ class GemmProblem:
     rs_off: int = -1  # row of the [R, M] row-scale matrix, -1 = none
     skip_zero_rows: bool = False  # rows with row scale 0 are left untouched (disjoint row-masked writers)
     atomic: bool = False  # C += ... with red.global.add (several problems of one launch add into the same C)
+    # activation epilogue (nqb_gemm_grouped_act), v = the product above:
+    #   "silu"       C = silu(v)
+    #   "silu_save"  C = silu(v) and aux = v (the pre-activation, addressed like C)
+    #   "silu_grad"  C = v * silu'(aux)  (aux = the pre-activation saved by "silu_save")
+    act: str = "none"
+
+
+# descriptor flag bits of each GemmProblem.act (nqb.h)
+GEMM_ACT_FLAGS = {"none": 0, "silu": 8, "silu_save": 8 | 16, "silu_grad": 32}
 
 
 class GroupedGemm:
@@ -592,31 +601,47 @@ class GroupedGemm:
     def __init__(self, problems, device):
         L = _capi.lib()
         self.problems = list(problems)
-        if not self.problems:
+        rows = self.descriptor_rows(self.problems)
+        blobs = []
+        for p, row in zip(self.problems, rows):
+            K, N = row[6], row[7]
+            Bc = p.B.detach().to(device).contiguous()
+            prep = torch.empty(int(L.nqb_gemm_prepared_floats(K, N)), dtype=torch.float32, device=device)
+            _capi.check(L.nqb_gemm_prepare(_ptr(Bc), Bc.shape[1], K, N, int(p.transposed), float(p.scale), _ptr(prep),
+                                           _stream()), "nqb_gemm_prepare")
+            blobs.append(prep)
+        self.act = any(p.act != "none" for p in self.problems)
+        self.needs_aux = any(p.act in ("silu_save", "silu_grad") for p in self.problems)
+        self.ntiles_total = rows[-1][10] + rows[-1][9]
+        self.tile_ctas, self.sched_ctas = self._weighted_split(rows, device)
+        self.prepared = torch.cat(blobs)
+        self.descs = torch.tensor(rows, dtype=torch.int64, device=device)
+        self.ndesc = len(rows)
+
+    @staticmethod
+    def descriptor_rows(problems) -> List[List[int]]:
+        """The checked 12-int64 descriptor of each problem (nqb.h), with the weights laid out one after another."""
+        if not problems:
             raise ValueError("GroupedGemm: empty problem list")
-        rows, blobs, b_off, tile0 = [], [], 0, 0
-        for p in self.problems:
+        L = _capi.lib()
+        rows, b_off, tile0 = [], 0, 0
+        for p in problems:
             K, N = (p.B.shape[1], p.B.shape[0]) if p.transposed else (p.B.shape[0], p.B.shape[1])
             if any(v % 4 for v in (K, N, p.lda, p.ldc, p.a_off, p.c_off)):
                 raise ValueError("GroupedGemm: K, N, lda, ldc and offsets must be multiples of 4")
             if p.B.dtype != torch.float32:
                 raise TypeError("GroupedGemm: float32 only")
-            Bc = p.B.detach().to(device).contiguous()
-            nfl = int(L.nqb_gemm_prepared_floats(K, N))
-            prep = torch.empty(nfl, dtype=torch.float32, device=device)
-            _capi.check(L.nqb_gemm_prepare(_ptr(Bc), Bc.shape[1], K, N, int(p.transposed), float(p.scale), _ptr(prep),
-                                           _stream()), "nqb_gemm_prepare")
+            if p.act not in GEMM_ACT_FLAGS:
+                raise ValueError(f"GroupedGemm: unknown act {p.act!r} (one of {', '.join(GEMM_ACT_FLAGS)})")
+            if p.act != "none" and (p.accumulate or p.atomic):
+                raise ValueError("GroupedGemm: an activation cannot be combined with accumulate or atomic")
             kchunks, ntiles = (K + 31) // 32, (N + 127) // 128
             rows.append([p.a_off, p.c_off, b_off, p.rs_off, p.lda, p.ldc, K, N, kchunks, ntiles, tile0,
-                         (1 if p.accumulate else 0) | (2 if p.skip_zero_rows else 0) | (4 if p.atomic else 0)])
-            blobs.append(prep)
-            b_off += nfl
+                         (1 if p.accumulate else 0) | (2 if p.skip_zero_rows else 0) | (4 if p.atomic else 0)
+                         | GEMM_ACT_FLAGS[p.act]])
+            b_off += int(L.nqb_gemm_prepared_floats(K, N))
             tile0 += ntiles
-        self.ntiles_total = tile0
-        self.tile_ctas, self.sched_ctas = self._weighted_split(rows, device)
-        self.prepared = torch.cat(blobs)
-        self.descs = torch.tensor(rows, dtype=torch.int64, device=device)
-        self.ndesc = len(rows)
+        return rows
 
     @staticmethod
     def _weighted_split(rows, device):
@@ -645,15 +670,35 @@ class GroupedGemm:
             c0 += n[j]
         return torch.tensor(tab, dtype=torch.int32, device=device), c0
 
-    def run(self, a: torch.Tensor, c: torch.Tensor, M: int, rowscale: Optional[torch.Tensor] = None):
+    def run(self, a: torch.Tensor, c: torch.Tensor, M: int, rowscale: Optional[torch.Tensor] = None,
+            aux: Optional[torch.Tensor] = None):
+        """``aux``: the pre-activation matrix of "silu_save" (written) / "silu_grad" (read) problems."""
         _require_cuda(a, c)
         if a.dtype != torch.float32 or c.dtype != torch.float32:
             raise TypeError("GroupedGemm.run: float32 only")
+        rs_ld = int(rowscale.shape[-1]) if rowscale is not None else 0
+        if not self.act:
+            if aux is not None:
+                raise ValueError("GroupedGemm.run: aux given, but no problem sets an activation")
+            _capi.check(
+                _capi.lib().nqb_gemm_grouped(_ptr(self.descs), self.ndesc, self.ntiles_total, _ptr(self.tile_ctas),
+                                             int(self.sched_ctas), _ptr(a), _ptr(self.prepared), _ptr(c),
+                                             _ptr(rowscale), rs_ld, int(M), _stream()),
+                "nqb_gemm_grouped",
+            )
+            return c
+        if self.needs_aux and aux is None:
+            raise ValueError("GroupedGemm.run: silu_save / silu_grad problems need aux")
+        if aux is not None:
+            _require_cuda(aux)
+            if aux.dtype != torch.float32:
+                raise TypeError("GroupedGemm.run: float32 only")
+        # "silu"-only launches never touch aux; the entry point still takes a valid base
         _capi.check(
-            _capi.lib().nqb_gemm_grouped(_ptr(self.descs), self.ndesc, self.ntiles_total, _ptr(self.tile_ctas),
-                                         int(self.sched_ctas), _ptr(a), _ptr(self.prepared), _ptr(c), _ptr(rowscale),
-                                         (int(rowscale.shape[-1]) if rowscale is not None else 0), int(M), _stream()),
-            "nqb_gemm_grouped",
+            _capi.lib().nqb_gemm_grouped_act(_ptr(self.descs), self.ndesc, self.ntiles_total, _ptr(self.tile_ctas),
+                                             int(self.sched_ctas), _ptr(a), _ptr(self.prepared), _ptr(c),
+                                             _ptr(rowscale), rs_ld, int(M), _ptr(c if aux is None else aux), _stream()),
+            "nqb_gemm_grouped_act",
         )
         return c
 
