@@ -9,6 +9,7 @@ import math
 import pytest
 import torch
 
+from cell_frames import cell_frame
 from nequip_b200 import data as D
 from nequip_b200 import ops
 from oracle import model as omodel
@@ -57,6 +58,22 @@ def test_edge_embed(dtype, periodic):
     if not periodic:
         keep = (sysd["edge_cell_shift"].abs().sum(1) == 0)
         ei = ei[:, keep]
+    _check_edge_embed(pos, ei, cell, shift, dtype)
+
+
+@pytest.mark.parametrize("dtype", [torch.float32, torch.float64], ids=["f32", "f64"])
+@pytest.mark.parametrize("name", ["tilted", "left"])
+def test_edge_embed_triclinic(dtype, name):
+    """A triclinic (and a left-handed) cell with atoms several cells away: every edge has a non-zero shift, so the
+    edge vector depends on all nine cell entries (a transposed cell gives other vectors)."""
+    f = cell_frame("li3po4", 5, name, seed=3, outside=True)
+    cell, shift = f["cell"], f["edge_cell_shift"]
+    assert float((cell - cell.t()).abs().max()) > 1.0
+    assert float(shift.abs().max()) >= 3 and int((shift != 0).any(1).sum()) > 0.9 * shift.shape[0]
+    _check_edge_embed(f["pos"], f["edge_index"], cell, shift, dtype)
+
+
+def _check_edge_embed(pos, ei, cell, shift, dtype):
     lmax, nb, r_max, p = 2, 8, 5.0, 6.0
     E = ei.shape[1]
     g = torch.Generator().manual_seed(5)

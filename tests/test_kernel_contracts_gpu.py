@@ -654,15 +654,21 @@ def test_sh_and_edge_embed_write_contracts(E, dtype):
     ggv.check_guards("sh grad_vec")
     assert_elementwise(gys.view, y_o.detach(), t * (1 + y_o.detach().abs()), "sh y")
     assert_elementwise(ggv.view, gv_o, 10 * t * (1 + gv_o.abs()), "sh grad_vec")
-    # nqb_edge_embed_fwd / bwd
+    # nqb_edge_embed_fwd / bwd; E = 257 with a triclinic cell and integer shifts in -1..1 (the kernel's cell branch)
+    cell = shift = None
+    if E == 257:
+        cell = torch.tensor([[3.1, 0.0, 0.0], [0.9, 2.8, 0.0], [-0.6, 0.7, 3.3]], dtype=F64)
+        shift = torch.randint(-1, 2, (E, 3), generator=g).to(F64)
     pf = 2 * math.pi / r_max ** 2
     po = pos.clone().requires_grad_(True)
-    vec_o, ye_o, emb_o = omodel.edge_embed(po, ei, None, None, lmax, nb, r_max, p, dtype)
+    vec_o, ye_o, emb_o = omodel.edge_embed(po, ei, cell, shift, lmax, nb, r_max, p, dtype)
     (gp_o,) = torch.autograd.grad([ye_o, emb_o], [po], [gy.to(dtype), gemb.to(dtype)])
     gpos, gei, ggy, gge = _data(pos), _data(ei), _data(gy, dtype), _data(gemb, dtype)
+    gsh, gcell = (None, None) if cell is None else (_data(shift), _data(cell))
     gv, gye, gem = Guarded(E, 3, F64), Guarded(E, S, dtype), Guarded(E, nb, dtype)
-    _capi.check(L.nqb_edge_embed_fwd(lmax, nb, r_max, p, pf, P(gpos.view), P(gei.view), 0, 0, N, E, dt, P(gv.view),
-                                     P(gye.view), P(gem.view), st))
+    _capi.check(L.nqb_edge_embed_fwd(lmax, nb, r_max, p, pf, P(gpos.view), P(gei.view),
+                                     0 if gsh is None else P(gsh.view), 0 if gcell is None else P(gcell.view), N, E,
+                                     dt, P(gv.view), P(gye.view), P(gem.view), st))
     gp = Guarded(N, 3, F64, body="random", generator=g)
     gvo = Guarded(E, 3, F64)
     _capi.check(L.nqb_edge_embed_bwd(lmax, nb, r_max, p, pf, P(gv.view), P(gei.view), N, E, dt, P(ggy.view),
@@ -670,6 +676,11 @@ def test_sh_and_edge_embed_write_contracts(E, dtype):
     torch.cuda.synchronize()
     for nm, b in (("vec", gv), ("y", gye), ("emb", gem), ("grad_pos", gp), ("grad_vec", gvo), ("pos", gpos)):
         b.check_guards(f"edge_embed {nm}")
+    if cell is not None:
+        gsh.check_guards("edge_embed shift")
+        gcell.check_guards("edge_embed cell")
+        r = vec_o.detach().norm(dim=1)
+        assert int((shift != 0).any(1).sum()) > E // 2 and int((r < r_max).sum()) > E // 4
     assert_elementwise(gv.view, vec_o.detach(), 1e-13 * (1 + vec_o.detach().abs()), "edge vec")
     assert_elementwise(gye.view, ye_o.detach().double(), t * (1 + ye_o.detach().double().abs()), "edge y")
     assert_elementwise(gem.view, emb_o.detach().double(), t * (1 + emb_o.detach().double().abs()), "edge emb")

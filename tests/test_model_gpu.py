@@ -5,6 +5,7 @@ model_tests_basic.py:631-672, permutation equivariance :450-461, smooth cutoff :
 import pytest
 import torch
 
+from cell_frames import cell_frame
 from nequip_b200 import data as D
 from nequip_b200.nn.model import NequIPEnergyModel
 from oracle import model as omodel
@@ -24,8 +25,11 @@ CONFIGS = {
 KIND = {"tutorial_l1": "water", "water_l2_f32": "water", "li3po4_l2_f64feat": "li3po4", "asi_l3": "asi"}
 
 
-def _build(name, dtype, n_side=6, seed=0):
-    sysd = D.make_system(KIND[name], n_side, r_max=5.0, seed=seed)
+def _build(name, dtype, n_side=6, seed=0, cell="cubic"):
+    if cell == "cubic":
+        sysd = D.make_system(KIND[name], n_side, r_max=5.0, seed=seed)
+    else:  # a named cell of tests/cell_frames.py, atoms spread over several cells
+        sysd = cell_frame(KIND[name], n_side, cell, seed=seed, outside=True)
     meta = sysd.pop("_meta")
     model = NequIPEnergyModel(r_max=5.0, type_names=meta["type_names"], parity=True,
                               avg_num_neighbors=meta["avg_num_neighbors"], model_dtype=dtype, **CONFIGS[name]).cuda()
@@ -143,16 +147,20 @@ def test_fused_gate_matches_torch_gate(layout, dtype, tol):
 
 
 @pytest.mark.parametrize("dtype,tol", [(torch.float64, 1e-9), (torch.float32, 1e-5)])
-def test_stress_and_virial_match_oracle(dtype, tol):
-    """ForceStressOutput (grad_output.py:162-268): stress/virial from the per-edge gradients == the oracle's
-    displacement-trick autograd; plus a finite-difference check of dE/d(strain) in float64."""
-    model, sysd = _build("water_l2_f32", dtype, n_side=5, seed=5)
+@pytest.mark.parametrize("cell", ["cubic", "tilted", "left", "small"])
+def test_stress_and_virial_match_oracle(cell, dtype, tol):
+    """ForceStressOutput (grad_output.py:162-268): energy, forces, stress and virial from the per-edge gradients ==
+    the oracle's displacement-trick autograd, in a cubic, a triclinic, a left-handed (det < 0) and a smaller-than-
+    r_max triclinic cell; plus a finite-difference check of dE/d(strain) in float64, off-diagonal strains included."""
+    model, sysd = _build("water_l2_f32", dtype, n_side=2 if cell == "small" else 5, seed=5, cell=cell)
     for p in model.parameters():
         p.requires_grad_(False)
     dev = D.to_device(sysd, "cuda")
     out = model(dev, compute_stress=True)
     e_ref, f_ref, s_ref, v_ref = omodel.energy_forces_stress(model.state_dict(), model.config, sysd, dtype)
     assert out["stress"].shape == (1, 3, 3) and out["virial"].shape == (1, 3, 3)
+    escale = float(out["atomic_energy"].abs().sum())
+    assert abs(float(out["total_energy"]) - float(e_ref)) <= tol * escale, (float(out["total_energy"]), float(e_ref))
     sscale = float(s_ref.abs().max())
     assert float((out["stress"].cpu() - s_ref).abs().max()) <= tol * sscale, float((out["stress"].cpu() - s_ref).abs().max()) / sscale
     assert float((out["virial"].cpu() - v_ref).abs().max()) <= tol * float(v_ref.abs().max())
@@ -160,7 +168,7 @@ def test_stress_and_virial_match_oracle(dtype, tol):
     if dtype == torch.float64:
         eps = 1e-5
         vol = float(torch.linalg.det(sysd["cell"]).abs())
-        for (a, b) in [(0, 0), (0, 1), (2, 1)]:
+        for (a, b) in [(0, 0), (0, 1), (2, 1)] if cell == "cubic" else [(0, 0), (0, 1), (1, 2), (2, 0)]:
             es = []
             for sgn in (+1, -1):
                 strain = torch.zeros(3, 3, dtype=torch.float64)

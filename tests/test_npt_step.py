@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+from cell_frames import brute_list
 from nequip_b200 import _capi
 from nequip_b200 import data as D
 from nequip_b200 import ops
@@ -97,23 +98,6 @@ def test_pack_rejects_open_directions_and_bad_grids():
 # ------------------------------------------------------------------------------------------------------------------
 # null edges with the per-cell shift on the float64 oracle, stress and virial included
 # ------------------------------------------------------------------------------------------------------------------
-def _brute_list(pos, cell):
-    """Full list within R_MAX for any cell (all images that can reach the cutoff), sorted by (i, j, shift)."""
-    perp = 1.0 / np.linalg.norm(np.linalg.inv(cell), axis=0)
-    k = [int(np.ceil(R_MAX / p)) + 1 for p in perp]
-    imgs = np.array([(a, b, c) for a in range(-k[0], k[0] + 1) for b in range(-k[1], k[1] + 1)
-                     for c in range(-k[2], k[2] + 1)], dtype=np.float64)
-    n = pos.shape[0]
-    vec = pos[None, :, None, :] - pos[:, None, None, :] + (imgs @ cell)[None, None]  # [i, j, img, 3]
-    d2 = (vec * vec).sum(-1)
-    home = np.all(imgs == 0, axis=1)
-    self_home = np.eye(n, dtype=bool)[:, :, None] & home[None, None, :]
-    i, j, m = np.nonzero((d2 < R_MAX * R_MAX) & ~self_home)
-    sh = imgs[m]
-    order = np.lexsort((sh[:, 2], sh[:, 1], sh[:, 0], j, i))
-    return np.stack([i[order], j[order]]).astype(np.int64), sh[order]
-
-
 def _pad_rows(ei, sh, n_atoms, pad_shift, seed):
     rng = np.random.default_rng(seed)
     extra = rng.integers(0, 4, n_atoms)
@@ -145,7 +129,7 @@ def test_null_edges_change_nothing_on_the_oracle_with_stress():
     for pos, cell, types in frames:
         assert np.count_nonzero(cell - np.diag(np.diagonal(cell))) > 0, "the frames are triclinic"
         N = pos.shape[0]
-        ei, sh = _brute_list(pos, cell)
+        ei, sh = brute_list(pos, cell, True, R_MAX)
         type_names = meta["type_names"] if int(types.max()) >= 2 else ["H", "O"]
         model = NequIPEnergyModel(r_max=R_MAX, type_names=type_names, parity=True, l_max=2, num_layers=3,
                                   num_features=16, radial_mlp_depth=1, radial_mlp_width=16,
