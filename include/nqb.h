@@ -157,6 +157,27 @@ int nqb_edge_embed_bwd(int lmax, int num_bessel, double r_max, double poly_p, do
                        int out_dtype, const void* grad_y, const void* grad_emb, double* grad_pos,
                        double* grad_vec, nqb_stream_t st);
 
+/* ZBL pair energy (nequip/nn/pair_potential.py:230-386), everything in fp64.  Per edge e = (i -> j), i =
+ * edge_index[0][e]:  eps_e = A[ti,tj] / r * psi((S[ti,tj] * r) / a0) * f_c(r / r_max),  psi = the four-exponential
+ * LAMMPS screening function, f_c = PolynomialCutoff(poly_p) (rounded to float32 when cutoff_f32 != 0).
+ *   Geometry: either pos [N,3] with optional shift [E,3] + cell [3,3] (r = pos[j] - pos[i] + shift @ cell, the
+ *   arithmetic of nqb_edge_embed_fwd), or given edge vectors vec [E,3] (pos, shift, cell NULL).
+ *   types [N] i64 in [0, T); table [T,T,2] f64: {A = 0.5 * qqr2e * Z_i Z_j, S = Z_i^0.23 + Z_j^0.23} per ordered pair.
+ * nqb_zbl_fwd: row_ptr [N+1] / perm [E] or NULL: the destination CSR of edge_index[0] (nqb_csr_from_sorted).
+ *   e_atom [N] is fully written, each element once, no atomics: e_atom[i] = sum of the row's eps_e in CSR order
+ *   (bitwise repeatable; a row without edges gives 0; an edge with r >= r_max adds exactly +0).
+ * nqb_zbl_bwd: g_e = grad_e_atom[i] * d eps_e / dr * r / |r|.  grad_pos [N,3] (positions only) is ACCUMULATED INTO:
+ *   grad_pos[j] += g_e, grad_pos[i] -= g_e (fp64 atomics); grad_vec [E,3] is fully written with g_e.  At least one
+ *   of the two must be given; E = 0 writes nothing. */
+int nqb_zbl_fwd(const double* pos, const int64_t* edge_index, const double* shift, const double* cell,
+                const double* vec, const int64_t* types, const double* table, int T, const int64_t* row_ptr,
+                const int64_t* perm, int64_t N, int64_t E, double r_max, double poly_p, int cutoff_f32,
+                double* e_atom, nqb_stream_t st);
+int nqb_zbl_bwd(const double* pos, const int64_t* edge_index, const double* shift, const double* cell,
+                const double* vec, const int64_t* types, const double* table, int T, int64_t N, int64_t E,
+                double r_max, double poly_p, int cutoff_f32, const double* grad_e_atom, double* grad_pos,
+                double* grad_vec, nqb_stream_t st);
+
 /* Neighbour list on the device (cell list; full list, both directions, periodic images, no self edge in the home
  * image) -- replaces the host construction of nequip/data/_nl.py:60-152,292-361 and emits what
  * SortedNeighborListTransform (nequip/data/transforms/neighborlist.py:120-157) produces: edges sorted by

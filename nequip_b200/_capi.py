@@ -64,6 +64,10 @@ SIGNATURES = {
         _i32, [_i32, _i32, _dbl, _dbl, _dbl, _vp, _vp, _vp, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp]),
     "nqb_edge_embed_bwd": (
         _i32, [_i32, _i32, _dbl, _dbl, _dbl, _vp, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_zbl_fwd": (
+        _i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _i64, _dbl, _dbl, _i32, _vp, _vp]),
+    "nqb_zbl_bwd": (
+        _i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _dbl, _dbl, _i32, _vp, _vp, _vp, _vp]),
     "nqb_mlp_hidden_fwd": (_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_gemm_prepared_floats": (_i64, [_i32, _i32]),

@@ -4,9 +4,11 @@ The reference assembles a ``SequentialGraphNetwork`` with the module names of
 nequip/model/nequip_models.py:288-399 -- ``type_embed`` (``NodeTypeEmbed.embed_module``, nn/embedding/node.py:75),
 ``layer{i}_convnet.conv.{linear_1, linear_2, sc, edge_mlp.mlp.{2k}}`` (nn/convnetlayer.py:142,
 nn/interaction_block.py:82-146, nn/mlp.py:134-192), ``per_atom_energy_readout.mlp_module`` (nn/mlp.py:62),
-``per_type_energy_scale_shift.{scales, shifts}`` (nn/atomwise.py:206-233) -- wrapped in ``ForceStressOutput.func``
-and possibly ``GraphModel.model``.  Parameters are matched by SUFFIX, so any wrapper prefix is accepted; e3nn's
-persistent buffers (``tp_scatter.tp.*``, ``*.output_mask``, ...) carry no learnable state and are ignored.
+``per_type_energy_scale_shift.{scales, shifts}`` (nn/atomwise.py:206-233) and, in a model with a pair potential,
+``pair_potential.{atomic_numbers, _qqr2exesquare}`` (model/energy_modules.py:20-27, nn/pair_potential.py:336-358) --
+wrapped in ``ForceStressOutput.func`` and possibly ``GraphModel.model``.  Parameters are matched by SUFFIX, so any
+wrapper prefix is accepted; e3nn's persistent buffers (``tp_scatter.tp.*``, ``*.output_mask``, ...) carry no
+learnable state and are ignored.
 
 Flattening conventions assumed for the e3nn weights (SURVEY.md Appendix A.4; e3nn itself is not installed here, so
 this is stated, not verified): ``o3.Linear.weight`` = concatenation over instructions (i_in-major over equal irreps)
@@ -23,8 +25,8 @@ import torch
 _IGNORED = re.compile(r"(tp_scatter\.tp\.|\.output_mask$|_w3j|\.tp\._|norm_const$|\.alpha$|bessel_weights$|_empty$)")
 
 
-def reference_key_map(num_layers: int, radial_mlp_depth: int = 1) -> Dict[str, str]:
-    """reference key suffix -> ``NequIPEnergyModel.state_dict()`` key."""
+def reference_key_map(num_layers: int, radial_mlp_depth: int = 1, pair_potential: bool = False) -> Dict[str, str]:
+    """reference key suffix -> ``NequIPEnergyModel.state_dict()`` key (``pair_potential``: the model has ZBL)."""
     m = {
         "type_embed.embed_module.weight": "type_embed.weight",
         "per_atom_energy_readout.mlp_module.mlp.0.weight": "readout.mlp.0.weight",
@@ -39,13 +41,20 @@ def reference_key_map(num_layers: int, radial_mlp_depth: int = 1) -> Dict[str, s
             m[ref + "sc.weight"] = ours + "sc.weight"
         for q in range(radial_mlp_depth + 1):
             m[ref + f"edge_mlp.mlp.{2 * q}.weight"] = ours + f"edge_mlp.mlp.{2 * q}.weight"
+    if pair_potential:
+        for k in ("pair_potential.atomic_numbers", "pair_potential._qqr2exesquare"):
+            m[k] = k
     return m
+
+
+def _key_map(model) -> Dict[str, str]:
+    cfg = model.config
+    return reference_key_map(cfg["num_layers"], cfg["radial_mlp_depth"], cfg.get("pair_potential") is not None)
 
 
 def to_reference_state_dict(model, prefix: str = "model.func.") -> Dict[str, torch.Tensor]:
     """This model's parameters under the reference's names (e3nn buffers are not produced)."""
-    cfg = model.config
-    inv = {v: k for k, v in reference_key_map(cfg["num_layers"], cfg["radial_mlp_depth"]).items()}
+    inv = {v: k for k, v in _key_map(model).items()}
     out = {}
     for k, v in model.state_dict().items():
         if k in inv:
@@ -58,8 +67,7 @@ def to_reference_state_dict(model, prefix: str = "model.func.") -> Dict[str, tor
 def load_reference_state_dict(model, ref_sd: Dict[str, torch.Tensor], strict: bool = True) -> Tuple[list, list]:
     """Load a reference (nequip) state dict into ``model``.  Returns (missing, unexpected) like
     ``torch.nn.Module.load_state_dict``; with ``strict`` both must be empty (ignored e3nn buffers aside)."""
-    cfg = model.config
-    kmap = reference_key_map(cfg["num_layers"], cfg["radial_mlp_depth"])
+    kmap = _key_map(model)
     own = model.state_dict()
     new, unexpected, used = {}, [], set()
     for rk, v in ref_sd.items():

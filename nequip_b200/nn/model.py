@@ -27,6 +27,7 @@ import torch
 
 from .. import ops
 from ..irreps import Irrep, Irreps, build_tp_instructions, tp_path_exists
+from .pair import ZBL, ZBL_TARGET, parse_pair_potential
 from .tp_scatter import B200TensorProductScatter
 
 # e3nn.math.normalize2mom constants: (E_{z~N(0,1)} act(z)^2)^(-1/2) estimated from
@@ -547,12 +548,19 @@ class NequIPEnergyModel(torch.nn.Module):
                  radial_mlp_width: int = 128, num_bessels: int = 8, polynomial_cutoff_p: float = 6.0,
                  avg_num_neighbors: float = 1.0, per_type_energy_scales: Optional[Sequence[float]] = None,
                  per_type_energy_shifts: Optional[Sequence[float]] = None, model_dtype=torch.float32,
-                 seed: int = 123, node_layout: str = "ir_mul", strict_fast_path: bool = False):
+                 seed: int = 123, node_layout: str = "ir_mul", strict_fast_path: bool = False,
+                 pair_potential: Optional[dict] = None):
         """``num_features``: one width for every degree, or a list of l_max + 1 widths (one per degree, e.g.
         ``[128, 64, 32]`` = 128x0e + 64x1o + 32x2e for l_max = 2 without parity), as in nequip_models.py:164-190.
         ``type_embed_num_features``: width of the type embedding, which is also the first layer's input and the
-        self-connection's attribute width (nequip_models.py:171-174, 294); defaults to ``num_features[0]``."""
+        self-connection's attribute width (nequip_models.py:171-174, 294); defaults to ``num_features[0]``.
+        ``pair_potential``: the reference's config block of a pair potential (energy_modules.py:10-35), e.g.
+        ``{"_target_": "nequip.nn.pair_potential.ZBL", "units": "metal", "chemical_species": ["C", "H", "O", "Cu"]}``
+        (``_target_`` may be left out; optional ``polynomial_cutoff_p``, default 6, independent of the model's).  Its
+        per-atom energies are added after the per-type scale and shift, before the sum (submodule ``pair_potential``).
+        """
         super().__init__()
+        pair_spec = parse_pair_potential(pair_potential, len(type_names))
         widths = feature_widths(l_max, num_features)
         f_embed = int(type_embed_num_features) if type_embed_num_features is not None else widths[0]
         self.r_max, self.l_max, self.num_bessels, self.poly_p = float(r_max), l_max, num_bessels, float(polynomial_cutoff_p)
@@ -608,6 +616,10 @@ class NequIPEnergyModel(torch.nn.Module):
 
         self.register_buffer("scales", table(per_type_energy_scales, "per_type_energy_scales"))
         self.register_buffer("shifts", table(per_type_energy_shifts, "per_type_energy_shifts"))
+        self.pair_potential = None
+        if pair_spec is not None:
+            self.pair_potential = ZBL(type_names, model_dtype=model_dtype, **pair_spec)
+            self.config["pair_potential"] = dict(_target_=ZBL_TARGET, **pair_spec)
         self.set_strict_fast_path(strict_fast_path)
 
     @classmethod
@@ -648,6 +660,7 @@ class NequIPEnergyModel(torch.nn.Module):
         if cell is None:
             shift = None
         pre = (2 * math.pi) / (self.r_max * self.r_max)
+        sink = data.get("_edge_grad_sink")
         if EDGE_VECTORS_KEY in data:
             # the caller (LAMMPS ML-IAP) supplies the edge vectors: with_edge_vectors_ keeps them (nn/utils.py:68-118)
             edge_attrs, edge_embedding = ops.edge_embed_from_vectors(
@@ -656,7 +669,7 @@ class NequIPEnergyModel(torch.nn.Module):
         else:
             _vec, edge_attrs, edge_embedding = ops.edge_embed(
                 pos, edge_index, shift, cell, lmax=self.l_max, num_bessel=self.num_bessels, r_max=self.r_max,
-                poly_p=self.poly_p, prefactor=pre, out_dtype=self.model_dtype, edge_grad_sink=data.get("_edge_grad_sink"))
+                poly_p=self.poly_p, prefactor=pre, out_dtype=self.model_dtype, edge_grad_sink=sink)
         for layer in self.layers:
             x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight)
         e_atom = self.readout(x).to(torch.float64)
@@ -664,6 +677,13 @@ class NequIPEnergyModel(torch.nn.Module):
             e_atom = e_atom * self.scales[types]
         if self.shifts.numel():
             e_atom = e_atom + self.shifts[types]
+        if self.pair_potential is not None:
+            if EDGE_VECTORS_KEY in data:
+                e_pair = self.pair_potential(types, edge_index, self.r_max, edge_vectors=data[EDGE_VECTORS_KEY])
+            else:
+                e_pair = self.pair_potential(types, edge_index, self.r_max, pos=pos, shift=shift, cell=cell,
+                                             edge_grad_sink=sink)
+            e_atom = e_atom + e_pair
         data[PER_ATOM_ENERGY_KEY] = e_atom
         data[TOTAL_ENERGY_KEY] = self._reduce_energy(e_atom, data)
         return data
@@ -689,6 +709,9 @@ class NequIPEnergyModel(torch.nn.Module):
             e_atom = e_atom * self.scales[t_own]
         if self.shifts.numel():
             e_atom = e_atom + self.shifts[t_own]
+        if self.pair_potential is not None:
+            # every edge's centre is owned: the owned rows are complete, the ghost rows (no edges) are 0
+            e_atom = e_atom + self.pair_potential(types, edge_index, self.r_max, pos=pos, shift=shift, cell=cell)[:n_own]
         return e_atom
 
     def forward(self, data: Dict[str, torch.Tensor], compute_forces: bool = True,
@@ -731,7 +754,10 @@ class NequIPEnergyModel(torch.nn.Module):
         data.pop("_edge_grad_sink", None)
         data[FORCE_KEY] = torch.neg(g)
         if sink is not None:
-            v = torch.einsum("ea,eb->ab", sink["edge_vectors"], sink["edge_vector_grad"])
+            g_edge = sink["edge_vector_grad"]
+            if "pair_edge_vector_grad" in sink:  # the pair potential's share of dE/d(edge vector)
+                g_edge = g_edge + sink["pair_edge_vector_grad"]
+            v = torch.einsum("ea,eb->ab", sink["edge_vectors"], g_edge)
             v = 0.5 * (v + v.t())
             vol = torch.linalg.det(data[CELL_KEY].double().view(3, 3)).abs()
             data[STRESS_KEY] = (v / vol).view(1, 3, 3)

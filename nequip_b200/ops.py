@@ -567,6 +567,88 @@ def edge_embed(pos, edge_index, shift=None, cell=None, *, lmax: int, num_bessel:
 
 
 # ---------------------------------------------------------------------------------------
+# ZBL pair energy -- nqb_zbl_fwd / nqb_zbl_bwd
+# ---------------------------------------------------------------------------------------
+class _ZBLFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, geom, edge_index, shift, cell, types, table, r_max, poly_p, cutoff_f32, from_vectors, sink):
+        N, E, T = types.numel(), edge_index.shape[1], table.shape[0]
+        csr = csr_cache.get(edge_index[0], N)  # the CSR the first interaction layer already built
+        pos, vec = (None, geom) if from_vectors else (geom, None)
+        e_atom = torch.empty((N, 1), dtype=torch.float64, device=types.device)
+        _capi.check(
+            _capi.lib().nqb_zbl_fwd(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(vec), _ptr(types),
+                                    _ptr(table), T, _ptr(csr.row_ptr), _ptr(csr.perm), N, E, r_max, poly_p,
+                                    int(cutoff_f32), _ptr(e_atom), _stream()),
+            "nqb_zbl_fwd",
+        )
+        ctx.args = (r_max, poly_p, cutoff_f32, from_vectors)
+        ctx.sink = sink
+        ctx.save_for_backward(geom, edge_index, shift, cell, types, table)
+        return e_atom
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, ge):
+        geom, edge_index, shift, cell, types, table = ctx.saved_tensors
+        r_max, poly_p, cutoff_f32, from_vectors = ctx.args
+        N, E = types.numel(), edge_index.shape[1]
+        pos, vec = (None, geom) if from_vectors else (geom, None)
+        gpos = None if from_vectors else torch.zeros_like(geom)
+        gvec = torch.empty((E, 3), dtype=torch.float64, device=geom.device) \
+            if from_vectors or ctx.sink is not None else None
+        ge = ge.to(torch.float64).contiguous()
+        _capi.check(
+            _capi.lib().nqb_zbl_bwd(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(vec), _ptr(types),
+                                    _ptr(table), table.shape[0], N, E, r_max, poly_p, int(cutoff_f32), _ptr(ge),
+                                    _ptr(gpos), _ptr(gvec), _stream()),
+            "nqb_zbl_bwd",
+        )
+        if ctx.sink is not None:
+            # kept apart from the edge embedding's gradient: the stress assembly adds the two once both backwards ran
+            ctx.sink["pair_edge_vector_grad"] = gvec
+        return (gvec if from_vectors else gpos), None, None, None, None, None, None, None, None, None, None
+
+
+def zbl_energy(pos, edge_index, types, table, *, shift=None, cell=None, edge_vectors=None, r_max: float,
+               poly_p: float = 6.0, cutoff_dtype=torch.float64, edge_grad_sink=None):
+    """ZBL per-atom energies ``[N, 1]`` f64 (``N = types.numel()``), summed onto the centre ``edge_index[0]``.
+
+    ``table`` [T, T, 2] f64 holds ``0.5 * qqr2e * Z_i Z_j`` and ``Z_i^0.23 + Z_j^0.23`` per ordered type pair
+    (``nn.pair.ZBL.table``).  The geometry comes from ``pos`` (+ ``shift``/``cell``) or, with ``pos=None``, from the
+    given ``edge_vectors`` [E, 3] (the ML-IAP branch); the result is differentiable w.r.t. whichever was given.
+    ``cutoff_dtype=torch.float32`` rounds the cutoff as a float32 model does.  ``edge_grad_sink`` (a dict): the backward
+    pass also stores dE/d(edge vector) in it under ``pair_edge_vector_grad``."""
+    _require_cuda(edge_index, types, table)
+    edge_index = edge_index.long().contiguous()
+    types = types.view(-1).long().contiguous()
+    table = table.to(torch.float64).contiguous()
+    if table.dim() != 3 or table.shape[0] != table.shape[1] or table.shape[2] != 2:
+        raise ValueError(f"zbl_energy: table must be [T, T, 2], got {tuple(table.shape)}")
+    if cutoff_dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"zbl_energy: cutoff_dtype must be float32 or float64, got {cutoff_dtype}")
+    if (pos is None) == (edge_vectors is None):
+        raise ValueError("zbl_energy: give exactly one of pos and edge_vectors")
+    if (shift is None) != (cell is None):
+        raise ValueError("shift and cell must be given together")
+    if edge_vectors is not None:
+        _require_cuda(edge_vectors)
+        if shift is not None:
+            raise ValueError("zbl_energy: edge_vectors already include the cell shifts")
+        geom, from_vectors = edge_vectors.double().contiguous(), True
+    else:
+        _require_cuda(pos)
+        geom, from_vectors = pos.double().contiguous(), False
+        if geom.shape != (types.numel(), 3):
+            raise ValueError(f"zbl_energy: pos must be [{types.numel()}, 3], got {tuple(geom.shape)}")
+        if shift is not None:
+            shift = shift.double().contiguous()
+            cell = cell.double().reshape(3, 3).contiguous()
+    return _ZBLFn.apply(geom, edge_index, shift, cell, types, table, float(r_max), float(poly_p),
+                        cutoff_dtype == torch.float32, from_vectors, edge_grad_sink)
+
+
+# ---------------------------------------------------------------------------------------
 # grouped fp32-accurate GEMM on the tensor cores (wgmma 3xTF32) -- nqb_gemm_grouped
 # ---------------------------------------------------------------------------------------
 @dataclass
