@@ -20,7 +20,8 @@
 //   * it stages its own A rows, one 32-wide K chunk at a time, with 16-byte cp.async (DEPTH chunks ahead across
 //     work-item boundaries) into the canonical K-major core-matrix layout, and writes their tf32 low parts;
 //   * it issues wgmma m64n128k8 from shared memory (4 k-steps x 3 terms per chunk) into two register
-//     accumulators (hi*hi and cross terms) and stores C straight from them.
+//     accumulators (hi*hi and cross terms), keeps one chunk's MMAs in flight while it stages the next chunk of
+//     the same accumulation segment, and stores C straight from the accumulators.
 // Thread 0 streams the pre-split weight chunks [hi | lo] x [128 x 32] with cp.async.bulk into a ring of BSLOTS
 // slots (mbarrier complete_tx); a problem with K <= 128 keeps its chunks resident for all of the CTA's M-tiles.
 #include <cuda_runtime.h>
@@ -215,7 +216,13 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
     const float* B = b_base + d->b_off + (int64_t)w.nt * w.kchunks * BLOCK_FLOATS;
     if (tid == 0)
       for (int64_t c = 0; c < min((int64_t)BSLOTS, nload); ++c) load_slot((int)c, B + (c % w.kchunks) * BLOCK_FLOATS, bytes);
-    int64_t x = 0;  // chunk loads of this N-tile consumed (streaming mode)
+    int64_t x = 0, xr = 0;  // streaming mode: chunk loads of this N-tile consumed / given back to the loader
+    // chunk y's MMAs have retired: its slot is free for chunk y + BSLOTS
+    auto release = [&](int64_t y) {
+      const int slot = (int)(y % BSLOTS);
+      if (lane == 0) mbar_arrive(&S.b_empty[slot]);
+      if (tid == 0 && y + BSLOTS < nload) load_slot(slot, B + ((y + BSLOTS) % w.kchunks) * BLOCK_FLOATS, bytes);
+    };
     // flags: bit0 read-modify-write accumulate (single writer per element within the launch),
     //        bit1 rows whose row scale is zero are not touched (disjoint row-masked writers),
     //        bit2 accumulate with red.global.add (several problems of this launch add into the same C)
@@ -231,6 +238,8 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
       for (int seg = 0; seg < nseg; ++seg) {
         const int h1 = min(w.kchunks, (seg + 1) * SEG);
         for (int h = seg * SEG; h < h1; ++h, ++i) {
+          // chunk i - 1's MMAs (if any) run during everything up to this chunk's first wgmma; chunk i - 2, the
+          // last reader of low-part slot i % NLO, has retired
           cp_async_wait<DEPTH - 1>();  // my parts of chunk i have landed
           const float* raw = S.araw[wg][i % RAW] + my_off;
           float* lo = S.alo[wg][i % NLO] + my_off;
@@ -249,7 +258,7 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
             slot = h;
             if (first_mt) { mbar_wait(&S.b_full[slot], (bpar >> slot) & 1); bpar ^= 1u << slot; }
           } else {
-            slot = (uint32_t)(x % BSLOTS);
+            slot = (uint32_t)(x++ % BSLOTS);
             mbar_wait(&S.b_full[slot], (bpar >> slot) & 1);
             bpar ^= 1u << slot;
           }
@@ -265,14 +274,12 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
 #pragma unroll
           for (int ks = 0; ks < KC / 8; ++ks) wgmma_tf32_m64n128(xx, a_hi + ks * 16, b_lo + ks * 16, 1u);
           wgmma_commit();
-          wgmma_wait<0>();
-          if (!w.resident) {
-            if (lane == 0) mbar_arrive(&S.b_empty[slot]);
-            if (tid == 0 && x + BSLOTS < nload) load_slot(slot, B + ((x + BSLOTS) % w.kchunks) * BLOCK_FLOATS, bytes);
-            ++x;
-          }
-          issue();  // chunk i + DEPTH into the stage of chunk i - 1 (read by the MMAs waited for above)
+          wgmma_wait<1>();  // chunk i - 1 has retired, chunk i stays in flight
+          if (xr + 1 < x) release(xr++);
+          issue();  // chunk i + DEPTH into the stage of chunk i - 1
         }
+        wgmma_wait<0>();  // the sums below and the epilogue read the accumulators
+        if (xr < x) release(xr++);
         // segment sums in registers; the last segment leaves the result in hh
         if (seg + 1 < nseg) {
 #pragma unroll
