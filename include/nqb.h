@@ -246,6 +246,28 @@ int nqb_mlp_hidden_fwd(const float* emb, const float* W1s, int64_t E, int num_be
 int nqb_mlp_hidden_bwd(const float* emb, const float* W1s, const float* grad_h, int64_t E, int num_bessel,
                        int hidden, float* grad_emb, nqb_stream_t st);
 
+/* Reverse-edge pair map of the radial MLP: the MLP's input is the edge embedding alone, so two edges whose embedding
+ * rows are bitwise equal get bitwise-equal MLP outputs, and the rows can be computed once.
+ *   edge_index [2,E] i64 (i = edge_index[0][e], j = edge_index[1][e]); shift [E,3] f64 or NULL (all zero);
+ *   emb [E,num_bessel] f32; row_ptr [N+1] / perm [E] or NULL: the destination CSR of edge_index[0]
+ *   (nqb_csr_from_sorted).
+ *   The candidate of e = (i -> j) is the first edge f != e in CSR order of row j with edge_index[1][f] = i,
+ *   shift[f] = -shift[e] (compared as values: -0 equals 0) and emb[f] bitwise equal to emb[e].  e and f are
+ *   partners when each is the other's candidate; an edge without a partner has a slot of its own.
+ *   pair_rows [E,2] i64 (16-byte aligned): slot u < U holds {representative edge, partner or -1}, the representative
+ *   being the smaller edge id of a pair, slots ordered by representative.  count [1] i64 = U (left on the device).
+ *   Writes pair_rows rows < U and count, nothing else (E = 0: count = 0 only).  No host synchronisation: the launches
+ *   depend on E only, so they can be captured in a CUDA graph.
+ *   work: nqb_edge_pairs_work_size(E) i64 of scratch. */
+int64_t nqb_edge_pairs_work_size(int64_t E);
+int nqb_edge_pairs(const int64_t* edge_index, int64_t E, int64_t N, const double* shift, const float* emb,
+                   int num_bessel, const int64_t* row_ptr, const int64_t* perm, int64_t* work, int64_t* pair_rows,
+                   int64_t* count, nqb_stream_t st);
+/* The first radial layer on the slots of nqb_edge_pairs:  h[u] = silu(emb[pair_rows[u][0]] @ W1s)  for
+ * u < min(*count, capacity).  Writes rows < U of h [capacity, hidden] only; the grid depends on capacity alone. */
+int nqb_mlp_hidden_fwd_rows(const float* emb, const float* W1s, const int64_t* pair_rows, const int64_t* count,
+                            int64_t capacity, int num_bessel, int hidden, float* h, nqb_stream_t st);
+
 /* Grouped fp32-accurate GEMM on the tensor cores (wgmma tf32, 3xTF32, segmented fp32
  * accumulation):  C_p[M, N_p] (+)= rowscale_p[m] * A_p[M, K_p] @ B_p[K_p, N_p]  for a list of problems
  * sharing M.  Replaces the dense algebra around the convolution: ScalarMLPFunction's torch.mm
@@ -287,6 +309,14 @@ int nqb_gemm_grouped(const void* descs_dev, int ndesc, int ntiles_total, const i
 int nqb_gemm_grouped_act(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
                          int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
                          const float* rowscale_base, int64_t rs_ld, int64_t M, float* aux_base, nqb_stream_t st);
+/* The same GEMM on the slots of nqb_edge_pairs (plain problems only: no row scale, no flag bits; the host rejects
+ * others).  M = min(*count_dev, capacity) is read on the device, A holds one row per slot (the compact h), and result
+ * row m is stored to C rows pair_rows[m][0] and, when it is >= 0, pair_rows[m][1].  Write contract: every C row listed
+ * in pair_rows[0 .. M) is written once in columns < N_p, nothing else of C is written; A is read in rows < M only.
+ * pair_rows must be 16-byte aligned; the grid depends on capacity alone (capturable). */
+int nqb_gemm_grouped_pairs(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
+                           int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
+                           const int64_t* pair_rows, const int64_t* count_dev, int64_t capacity, nqb_stream_t st);
 
 /* Gate nonlinearity (e3nn nn.Gate with normalize2mom'd SiLU for even / tanh for odd scalars and gates,
  * nequip/nn/convnetlayer.py:42-56,104-112), one kernel per direction.  Column tables (device, int32) are

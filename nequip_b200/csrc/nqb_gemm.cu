@@ -115,14 +115,18 @@ __device__ __forceinline__ void bar_wg(int wg) { asm volatile("bar.sync %0, 128;
 
 // ACT = false: the plain GEMM.  ACT = true also honours the activation bits 3-5 of a problem's flags in the
 // epilogue, with the auxiliary matrix at aux_base (addressed with C's c_off and ldc); see nqb.h.
-template <bool ACT>
+// PAIRS = true (plain problems only): M = min(M, *m_dev) is read on the device, and result row m is stored to the C
+// rows pair_rows[m][0] and, when it is >= 0, pair_rows[m][1] (nqb_gemm_grouped_pairs).
+template <bool ACT, bool PAIRS = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const int32_t* __restrict__ tile_ctas,
          int sched_ctas, const float* __restrict__ a_base, const float* __restrict__ b_base, float* __restrict__ c_base,
-         const float* __restrict__ rs_base, int64_t rs_ld, int64_t M, float* __restrict__ aux_base) {
+         const float* __restrict__ rs_base, int64_t rs_ld, int64_t M, float* __restrict__ aux_base,
+         const int64_t* __restrict__ m_dev, const int64_t* __restrict__ pair_rows) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& S = *reinterpret_cast<Smem*>(smem_raw);
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+  if constexpr (PAIRS) M = min(M, *m_dev);  // the schedule does not depend on M, only the M-tiles and row guards
   const int64_t mtiles = (M + TM - 1) / TM;
 
   if (tid == 0) {
@@ -291,6 +295,24 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
       }
       // ---- epilogue: C rows r0 and r0 + 8 of this warpgroup, two adjacent columns per store --------------------
       const int64_t m0 = mt * TM + wg * MW + r0;
+      if constexpr (PAIRS) {
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const int64_t m = m0 + half * 8;
+          if (m >= M) continue;
+          const longlong2 pr = __ldg(reinterpret_cast<const longlong2*>(pair_rows) + m);
+          float* crow0 = C + pr.x * ldc + c0;
+          float* crow1 = C + pr.y * ldc + c0;  // stored to only when pr.y >= 0
+#pragma unroll
+          for (int j = 0; j < TN / 8; ++j) {
+            if (j * 8 + c0 < w.ncols) {
+              const float2 v = make_float2(hh[4 * j + 2 * half], hh[4 * j + 2 * half + 1]);
+              *reinterpret_cast<float2*>(crow0 + j * 8) = v;
+              if (pr.y >= 0) *reinterpret_cast<float2*>(crow1 + j * 8) = v;
+            }
+          }
+        }
+      } else
 #pragma unroll
       for (int half = 0; half < 2; ++half) {
         const int64_t m = m0 + half * 8;
@@ -397,12 +419,13 @@ extern "C" int nqb_gemm_prepare(const float* B, int64_t ldb, int K, int N, int t
   return 0;
 }
 
-// the launcher of both entry points; errors are reported under the entry point's name
-template <bool ACT>
+// the launcher of the entry points; errors are reported under the entry point's name
+template <bool ACT, bool PAIRS = false>
 static int gemm_grouped_launch(const char* who, const void* descs_dev, int ndesc, int ntiles_total,
                                const int32_t* tile_ctas_dev, int sched_ctas, const float* a_base,
                                const float* prepared_base, float* c_base, float* aux_base, const float* rowscale_base,
-                               int64_t rs_ld, int64_t M, nqb_stream_t st) {
+                               int64_t rs_ld, int64_t M, nqb_stream_t st, const int64_t* m_dev = nullptr,
+                               const int64_t* pair_rows = nullptr) {
   auto fail = [&](const char* what) {
     char msg[160];  // nqb_set_error copies it
     snprintf(msg, sizeof(msg), "%s: %s", who, what);
@@ -414,6 +437,8 @@ static int gemm_grouped_launch(const char* who, const void* descs_dev, int ndesc
   if (!descs_dev || !a_base || !prepared_base || !c_base) return fail("null pointer");
   // the device descriptors cannot be read here: an activation launch always takes an aux matrix
   if (ACT && !aux_base) return fail("aux_base is null (bit4 / bit5 problems store to or read from it)");
+  if (PAIRS && (!m_dev || !pair_rows)) return fail("pair_rows or count is null");
+  if (PAIRS && ((uintptr_t)pair_rows & 15)) return fail("pair_rows must be 16-byte aligned");
   // A is staged with 16-byte cp.async, the weights with bulk copies, C and aux are stored in float2 pairs
   if (((uintptr_t)a_base | (uintptr_t)prepared_base | (uintptr_t)c_base | (uintptr_t)aux_base) & 15)
     return fail(ACT ? "a_base, prepared_base, c_base and aux_base must be 16-byte aligned"
@@ -421,7 +446,8 @@ static int gemm_grouped_launch(const char* who, const void* descs_dev, int ndesc
   static bool attr_set[64] = {false};
   const int dev = gemm_device();
   if (!attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(k_gemm3x<ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem) + 1024);
+    cudaError_t e = cudaFuncSetAttribute(k_gemm3x<ACT, PAIRS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)sizeof(Smem) + 1024);
     if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
     attr_set[dev] = true;
   }
@@ -429,9 +455,9 @@ static int gemm_grouped_launch(const char* who, const void* descs_dev, int ndesc
   int grid = (int)(nwork < gemm_sm_count() ? nwork : gemm_sm_count());
   if (tile_ctas_dev != nullptr && sched_ctas > 0 && sched_ctas <= gemm_sm_count()) grid = sched_ctas;
   else tile_ctas_dev = nullptr;
-  k_gemm3x<ACT><<<grid, NTHREADS, sizeof(Smem) + 1024, (cudaStream_t)st>>>(
+  k_gemm3x<ACT, PAIRS><<<grid, NTHREADS, sizeof(Smem) + 1024, (cudaStream_t)st>>>(
       (const GemmDesc*)descs_dev, ndesc, ntiles_total, tile_ctas_dev, sched_ctas, a_base, prepared_base, c_base,
-      rowscale_base, rs_ld, M, aux_base);
+      rowscale_base, rs_ld, M, aux_base, m_dev, pair_rows);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -451,4 +477,13 @@ extern "C" int nqb_gemm_grouped_act(const void* descs_dev, int ndesc, int ntiles
                                     nqb_stream_t st) {
   return gemm_grouped_launch<true>("nqb_gemm_grouped_act", descs_dev, ndesc, ntiles_total, tile_ctas_dev, sched_ctas,
                                    a_base, prepared_base, c_base, aux_base, rowscale_base, rs_ld, M, st);
+}
+
+extern "C" int nqb_gemm_grouped_pairs(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
+                                      int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
+                                      const int64_t* pair_rows, const int64_t* count_dev, int64_t capacity,
+                                      nqb_stream_t st) {
+  return gemm_grouped_launch<false, true>("nqb_gemm_grouped_pairs", descs_dev, ndesc, ntiles_total, tile_ctas_dev,
+                                          sched_ctas, a_base, prepared_base, c_base, nullptr, nullptr, 0, capacity,
+                                          st, count_dev, pair_rows);
 }

@@ -42,6 +42,17 @@ __device__ __forceinline__ Basis8 load_basis(const float* __restrict__ emb, int6
   }
   return r;
 }
+// the basis values of slot u < n: edge u itself, or with ROWS the edge rows[2 u]
+template <bool ROWS>
+__device__ __forceinline__ Basis8 load_slot(const float* __restrict__ emb, const int64_t* __restrict__ rows, int64_t u,
+                                            int64_t n) {
+  if constexpr (ROWS) {
+    const int64_t e = u < n ? __ldg(rows + 2 * u) : 0;
+    return load_basis(emb, e, u < n ? e + 1 : 0);
+  } else {
+    return load_basis(emb, u, n);
+  }
+}
 // the 8 basis values of the batch's edge j (held by lane j), broadcast to every lane
 __device__ __forceinline__ void bcast_basis(const Basis8& mine, int j, float (&x)[NB]) {
   x[0] = __shfl_sync(0xffffffffu, mine.a.x, j); x[1] = __shfl_sync(0xffffffffu, mine.a.y, j);
@@ -62,9 +73,15 @@ __device__ __forceinline__ void preact4(const float (&x)[NB], const float2 (&w01
   }
 }
 
+// ROWS = true: h[u] = silu(emb[rows[2 u]] @ W1s) for u < min(E, *count) (the representative edges of the slots of
+// nqb_edge_pairs); the grid is sized for E
+template <bool ROWS = false>
 __global__ void __launch_bounds__(256) k_hidden_fwd(const float* __restrict__ emb, const float* __restrict__ W1s,
-                                                    int64_t E, float* __restrict__ h) {
+                                                    int64_t E, float* __restrict__ h,
+                                                    const int64_t* __restrict__ rows = nullptr,
+                                                    const int64_t* __restrict__ count = nullptr) {
   const int lane = threadIdx.x & 31, m0 = lane * 4;
+  if constexpr (ROWS) E = min(E, *count);
   float2 w01[NB], w23[NB];
 #pragma unroll
   for (int k = 0; k < NB; ++k) {
@@ -75,10 +92,10 @@ __global__ void __launch_bounds__(256) k_hidden_fwd(const float* __restrict__ em
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const int64_t nbatch = (E + 31) >> 5;
   int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  Basis8 cur = load_basis(emb, b * 32 + lane, b < nbatch ? E : 0);
+  Basis8 cur = load_slot<ROWS>(emb, rows, b * 32 + lane, b < nbatch ? E : 0);
   for (; b < nbatch; b += nwarps) {
     const int64_t bn = b + nwarps;
-    const Basis8 nxt = load_basis(emb, bn * 32 + lane, bn < nbatch ? E : 0);  // in flight during this batch
+    const Basis8 nxt = load_slot<ROWS>(emb, rows, bn * 32 + lane, bn < nbatch ? E : 0);  // in flight during this batch
     const int64_t e0 = b * 32;
     const int cnt = (int)((E - e0) < 32 ? (E - e0) : 32);  // warp-uniform
     float* hrow = h + e0 * H + m0;
@@ -167,6 +184,142 @@ __global__ void __launch_bounds__(256) k_hidden_bwd(const float* __restrict__ em
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// reverse-edge pair map (nqb_edge_pairs): the radial MLP's input is the edge embedding alone, so an edge and its
+// reverse edge with a bitwise-equal embedding row get bitwise-equal MLP outputs and share one row of work.
+//   k_pair_candidates: cand[e] = the first edge f != e, in CSR order of the row idx1[e], with idx1[f] = idx0[e],
+//     shift[f] = -shift[e] (as values) and emb[f] bitwise emb[e]; -1 if none.  Eight lanes scan one row, eight
+//     slots per step (coalesced loads), and stop at the first step with a hit;
+//   an edge's partner is cand[e] when the relation is mutual (cand[cand[e]] = e); it represents a slot when it has
+//     no partner or is the smaller of the two.  Slots are numbered by an exclusive scan over the edge ids:
+//   k_pair_block_counts: representatives per tile of PT edges;
+//   k_pair_write: each tile adds the counts of the tiles before it, scans its own edges and writes its slots; the
+//     last tile writes the total.
+// ---------------------------------------------------------------------------------------------
+constexpr int PT = 1024;  // edges per tile of the slot scan (256 threads x 4)
+
+__global__ void __launch_bounds__(256) k_pair_candidates(const int64_t* __restrict__ ei, int64_t E, int64_t N,
+                                                         const double* __restrict__ shift,
+                                                         const uint32_t* __restrict__ emb, int words,
+                                                         const int64_t* __restrict__ row_ptr,
+                                                         const int64_t* __restrict__ perm, int64_t* __restrict__ cand) {
+  const int lane = threadIdx.x & 31, g = lane >> 3, r = lane & 7;
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t wv = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); wv * 4 < E; wv += nwarps) {
+    const int64_t e = wv * 4 + g;  // four edges per warp, one per group of eight lanes
+    int64_t a = -1, s = 0, s1 = 0;
+    if (e < E) {
+      a = ei[e];
+      const int64_t b = ei[E + e];
+      if (b >= 0 && b < N) {
+        s = row_ptr[b];
+        s1 = row_ptr[b + 1];
+      }
+    }
+    int64_t found = -1;
+    bool done = s >= s1;
+    while (__any_sync(0xffffffffu, !done)) {
+      int64_t f = -1;
+      bool hit = false;
+      if (!done && s + r < s1) {
+        f = perm ? perm[s + r] : s + r;
+        hit = f != e && ei[E + f] == a;
+        if (hit && shift)
+          hit = shift[3 * f] == -shift[3 * e] && shift[3 * f + 1] == -shift[3 * e + 1] &&
+                shift[3 * f + 2] == -shift[3 * e + 2];
+        for (int k = 0; hit && k < words; ++k) hit = emb[f * words + k] == emb[e * words + k];
+      }
+      const uint32_t grp = (__ballot_sync(0xffffffffu, hit) >> (8 * g)) & 0xffu;
+      const int64_t first = __shfl_sync(0xffffffffu, f, 8 * g + (grp ? __ffs(grp) - 1 : 0));
+      if (!done && grp) {
+        found = first;
+        done = true;
+      }
+      s += 8;
+      if (s >= s1) done = true;
+    }
+    if (r == 0 && e < E) cand[e] = found;
+  }
+}
+
+// 1 when edge e represents a slot; its partner (or -1) in *partner
+__device__ __forceinline__ int pair_rep(const int64_t* __restrict__ cand, int64_t e, int64_t* partner) {
+  const int64_t c = cand[e];
+  const int64_t p = (c >= 0 && cand[c] == e) ? c : -1;
+  *partner = p;
+  return (p < 0 || e < p) ? 1 : 0;
+}
+
+// inclusive sum over the 256 threads of the block (scratch: 8 ints), returned to every thread together with the total
+__device__ __forceinline__ int block_scan256(int v, int* scratch, int* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += t;
+  }
+  if (lane == 31) scratch[warp] = v;
+  __syncthreads();
+  int before = 0, all = 0;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) {
+    const int x = scratch[w];
+    before += (w < warp) ? x : 0;
+    all += x;
+  }
+  __syncthreads();
+  *total = all;
+  return v + before;
+}
+
+__global__ void __launch_bounds__(256) k_pair_block_counts(const int64_t* __restrict__ cand, int64_t E,
+                                                           int64_t* __restrict__ counts) {
+  __shared__ int scratch[8];
+  const int64_t e0 = (int64_t)blockIdx.x * PT + threadIdx.x * 4;
+  int n = 0;
+  int64_t p;
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (e0 + k < E) n += pair_rep(cand, e0 + k, &p);
+  int total;
+  block_scan256(n, scratch, &total);
+  if (threadIdx.x == 0) counts[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(256) k_pair_write(const int64_t* __restrict__ cand, int64_t E,
+                                                    const int64_t* __restrict__ counts, int64_t* __restrict__ pair_rows,
+                                                    int64_t* __restrict__ count) {
+  __shared__ int scratch[8];
+  __shared__ int64_t base_part[8];
+  // slots of the tiles before this one
+  int64_t before = 0;
+  for (int64_t t = threadIdx.x; t < blockIdx.x; t += blockDim.x) before += counts[t];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) before += __shfl_xor_sync(0xffffffffu, before, o);
+  if ((threadIdx.x & 31) == 0) base_part[threadIdx.x >> 5] = before;
+  __syncthreads();
+  int64_t base = 0;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) base += base_part[w];
+  const int64_t e0 = (int64_t)blockIdx.x * PT + threadIdx.x * 4;
+  int rep[4], n = 0;
+  int64_t partner[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    rep[k] = (e0 + k < E) ? pair_rep(cand, e0 + k, &partner[k]) : 0;
+    n += rep[k];
+  }
+  int total;
+  int64_t u = base + block_scan256(n, scratch, &total) - n;
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (rep[k]) {
+      reinterpret_cast<longlong2*>(pair_rows)[u] = make_longlong2(e0 + k, partner[k]);
+      ++u;
+    }
+  if (threadIdx.x == 0 && blockIdx.x == gridDim.x - 1) *count = base + total;
+}
+
 }  // namespace
 
 extern "C" int nqb_set_error(const char* msg);  // defined in nqb_runtime.cu
@@ -176,7 +329,7 @@ extern "C" void nqb_count_launch(void);
 // its next batch is always prefetched; fewer CTAs when there are fewer batches than warps
 template <typename K>
 static unsigned hidden_grid(K kernel, int which, int64_t E) {
-  static int ctas_dev[2][64] = {{0}, {0}};
+  static int ctas_dev[3][64] = {{0}, {0}, {0}};
   int dev = 0;
   cudaGetDevice(&dev);
   dev &= 63;
@@ -196,7 +349,23 @@ extern "C" int nqb_mlp_hidden_fwd(const float* emb, const float* W1s, int64_t E,
   if (E < 0) return nqb_set_error("nqb_mlp_hidden_fwd: negative size");
   if (E == 0) return 0;
   if (!emb || !W1s || !h) return nqb_set_error("nqb_mlp_hidden_fwd: null pointer");
-  k_hidden_fwd<<<hidden_grid(k_hidden_fwd, 0, E), 256, 0, (cudaStream_t)st>>>(emb, W1s, E, h);
+  k_hidden_fwd<<<hidden_grid(k_hidden_fwd<false>, 0, E), 256, 0, (cudaStream_t)st>>>(emb, W1s, E, h);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int nqb_mlp_hidden_fwd_rows(const float* emb, const float* W1s, const int64_t* pair_rows,
+                                       const int64_t* count, int64_t capacity, int num_bessel, int hidden, float* h,
+                                       nqb_stream_t st) {
+  if (num_bessel != NB || hidden != H)
+    return nqb_set_error("nqb_mlp_hidden_fwd_rows: only num_bessel=8, hidden=128 is built");
+  if (capacity < 0) return nqb_set_error("nqb_mlp_hidden_fwd_rows: negative size");
+  if (capacity == 0) return 0;
+  if (!emb || !W1s || !pair_rows || !count || !h) return nqb_set_error("nqb_mlp_hidden_fwd_rows: null pointer");
+  k_hidden_fwd<true><<<hidden_grid(k_hidden_fwd<true>, 2, capacity), 256, 0, (cudaStream_t)st>>>(emb, W1s, capacity, h,
+                                                                                                 pair_rows, count);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -210,6 +379,38 @@ extern "C" int nqb_mlp_hidden_bwd(const float* emb, const float* W1s, const floa
   if (E == 0) return 0;
   if (!emb || !W1s || !grad_h || !grad_emb) return nqb_set_error("nqb_mlp_hidden_bwd: null pointer");
   k_hidden_bwd<<<hidden_grid(k_hidden_bwd, 1, E), 256, 0, (cudaStream_t)st>>>(emb, W1s, grad_h, E, grad_emb);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int64_t nqb_edge_pairs_work_size(int64_t E) { return E > 0 ? E + (E + PT - 1) / PT : 0; }
+
+extern "C" int nqb_edge_pairs(const int64_t* edge_index, int64_t E, int64_t N, const double* shift, const float* emb,
+                              int num_bessel, const int64_t* row_ptr, const int64_t* perm, int64_t* work,
+                              int64_t* pair_rows, int64_t* count, nqb_stream_t st) {
+  if (E < 0 || N < 0 || num_bessel <= 0) return nqb_set_error("nqb_edge_pairs: bad size");
+  if (!count) return nqb_set_error("nqb_edge_pairs: null pointer");
+  if (E == 0) {
+    cudaError_t e = cudaMemsetAsync(count, 0, sizeof(int64_t), (cudaStream_t)st);
+    return e == cudaSuccess ? 0 : nqb_set_error(cudaGetErrorString(e));
+  }
+  if (!edge_index || !emb || !row_ptr || !work || !pair_rows) return nqb_set_error("nqb_edge_pairs: null pointer");
+  if ((uintptr_t)pair_rows & 15) return nqb_set_error("nqb_edge_pairs: pair_rows must be 16-byte aligned");
+  const int64_t tiles = (E + PT - 1) / PT;
+  int sms = 0, dev = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int64_t warps = (E + 3) / 4, cap = (int64_t)(sms > 0 ? sms : 132) * 8;  // 8 CTAs of 8 warps per SM
+  const unsigned cblocks = (unsigned)((warps + 7) / 8 < cap ? (warps + 7) / 8 : cap);
+  k_pair_candidates<<<cblocks, 256, 0, (cudaStream_t)st>>>(edge_index, E, N, shift,
+                                                            reinterpret_cast<const uint32_t*>(emb), num_bessel, row_ptr,
+                                                            perm, work);
+  nqb_count_launch();
+  k_pair_block_counts<<<(unsigned)tiles, 256, 0, (cudaStream_t)st>>>(work, E, work + E);
+  nqb_count_launch();
+  k_pair_write<<<(unsigned)tiles, 256, 0, (cudaStream_t)st>>>(work, E, work + E, pair_rows, count);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));

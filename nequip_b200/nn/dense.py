@@ -147,11 +147,17 @@ class SelfConnectionGemm:
 # ---------------------------------------------------------------------------------------
 class _RadialMLPGemmFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, emb, mlp: "RadialMLPGemm", need_bwd: bool):
+    def forward(ctx, emb, mlp: "RadialMLPGemm", need_bwd: bool, pairs):
         E = emb.shape[0]
         out = torch.empty((E, mlp.W), dtype=emb.dtype, device=emb.device)
         pre = [] if need_bwd else None
-        mlp.fwd.run(mlp.hidden(emb, pre), out, E)
+        if pairs is not None and mlp.shares_pairs:
+            # one row of h and of the GEMM per slot of the pair map, stored to both edges of the slot
+            h = torch.empty((E, mlp.w1s.shape[1]), dtype=emb.dtype, device=emb.device)  # rows < count are used
+            ops.mlp_hidden_fwd_rows(emb, mlp.w1s, pairs, h)
+            mlp.fwd.run_pairs(h, out, pairs)
+        else:
+            mlp.fwd.run(mlp.hidden(emb, pre), out, E)
         ctx.mlp = mlp
         if need_bwd:
             ctx.save_for_backward(emb, *pre)
@@ -161,7 +167,7 @@ class _RadialMLPGemmFn(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, gw):
         emb, *pre = ctx.saved_tensors
-        return ctx.mlp.grad_emb(emb, gw, pre), None, None
+        return ctx.mlp.grad_emb(emb, gw, pre), None, None, None
 
 
 class RadialMLPGemm:
@@ -171,6 +177,9 @@ class RadialMLPGemm:
     Forward: the first layer runs on ``k_hidden_fwd`` when it is [8, 128], otherwise as a ``k_gemm3x`` problem with
     the SiLU epilogue (K = num_bessels); every middle layer is one such problem; the last layer is a plain problem.
     With a backward pass ahead, each hidden layer on ``k_gemm3x`` also stores its pre-activation ([E, H] float32).
+    Given the reverse-edge pair map (``ops.edge_pairs``), an [8, 128] -> [128, W] MLP computes one row per slot
+    (``k_hidden_fwd`` on the slots' representative edges, then the paired ``k_gemm3x`` that stores each result row to
+    both edges of its slot); deeper MLPs keep the per-edge forward.
     Backward: the transposed GEMM of each layer multiplies by silu' of the saved pre-activation of the layer below;
     into an [8, 128] first layer it gives grad_h for ``k_hidden_bwd`` (pre-activation recomputed), and a generic
     first layer ends with a plain transposed GEMM into grad_emb [E, num_bessels]."""
@@ -189,6 +198,8 @@ class RadialMLPGemm:
         self.bwd = gemm(plan["bwd"])
         self._hidden = [(gemm(save), gemm(plain), save.B.shape[1]) for save, plain in plan["hidden"]]
         self._chain = [(self.bwd if p is plan["bwd"] else gemm(p), width, pre) for p, width, pre in plan["chain"]]
+        # the forward can share rows between the two edges of a pair slot (no per-edge pre-activation is kept)
+        self.shares_pairs = self._hidden_kernel and not self._hidden
 
     @staticmethod
     def uses_hidden_kernel(first) -> bool:
@@ -268,8 +279,9 @@ class RadialMLPGemm:
             return gemb
         return g
 
-    def __call__(self, emb):
-        return _RadialMLPGemmFn.apply(emb.contiguous(), self, torch.is_grad_enabled() and emb.requires_grad)
+    def __call__(self, emb, pairs: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
+        """``pairs``: ``ops.edge_pairs`` of the edge list whose embedding ``emb`` is (the per-edge forward without)."""
+        return _RadialMLPGemmFn.apply(emb.contiguous(), self, torch.is_grad_enabled() and emb.requires_grad, pairs)
 
 
 # ---------------------------------------------------------------------------------------

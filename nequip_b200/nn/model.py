@@ -349,7 +349,7 @@ class InteractionBlock(torch.nn.Module):
         weights, float64 and unusual shapes; frozen float32 ir_mul models use ``_tensor_core_blocks``."""
         return self.edge_mlp(edge_embedding)
 
-    def _use_fused(self, tc, edge_embedding, x, edge_attrs, edge_index) -> bool:
+    def _use_fused(self, tc, edge_embedding, x, edge_attrs, edge_index, pairs=None) -> bool:
         """``use_fused_radial_tp``: True / False, or "auto" (default) = time the fused kernel against the unfused pair
         (grouped GEMM + TP kernel) ONCE per layer on the first real call and keep the faster one.  The fused kernel
         never materialises the [E, W] weights in the forward pass, but its path-parallel decomposition gives up the
@@ -375,7 +375,7 @@ class InteractionBlock(torch.nn.Module):
 
                 xd, yd, ed = x.detach(), edge_attrs.detach(), edge_embedding.detach()
                 tf = t(lambda: tc["fused"](ed, xd, yd, edge_index[0], edge_index[1]))
-                tu = t(lambda: self.tp_scatter(x=xd, edge_attr=yd, edge_weight=tc["mlp"](ed), edge_dst=edge_index[0],
+                tu = t(lambda: self.tp_scatter(x=xd, edge_attr=yd, edge_weight=tc["mlp"](ed, pairs), edge_dst=edge_index[0],
                                                edge_src=edge_index[1]))
             self._fused_choice = bool(tf < tu)
             self.fused_timing_ms = {"fused": tf, "unfused": tu}
@@ -397,11 +397,12 @@ class InteractionBlock(torch.nn.Module):
                           f"wgmma kernels: {reason}", RuntimeWarning, stacklevel=3)
 
     def forward(self, x, node_attrs, edge_attrs, edge_embedding, edge_index, types=None, type_table=None,
-                n_own: Optional[int] = None, halo=None):
+                n_own: Optional[int] = None, halo=None, pairs=None):
         """``n_own``/``halo``: sharded frames (owned atoms first, then ghosts).  As in the reference
         (interaction_block.py:159-199) the first layer sees the type embedding of owned + ghost atoms;
         later layers work on owned rows, refresh the ghosts through ``halo`` right before the
-        TP+scatter and truncate to the owned rows right after it."""
+        TP+scatter and truncate to the owned rows right after it.  ``pairs``: the reverse-edge pair map of the
+        edge list (``ops.edge_pairs``), with which the radial MLP computes one row per pair."""
         if n_own is not None and not self.is_first_layer:
             x = x[:n_own]
             node_attrs = node_attrs[:n_own]
@@ -414,7 +415,7 @@ class InteractionBlock(torch.nn.Module):
             x = tc["lin1"](x) if self.norm_shortcut else tc["lin1"](x, self.norm_const.view(-1)[types].view(1, -1).contiguous())
             if halo is not None and not self.is_first_layer:
                 x = halo(x)
-            if tc["fused"] is not None and self._use_fused(tc, edge_embedding, x, edge_attrs, edge_index):
+            if tc["fused"] is not None and self._use_fused(tc, edge_embedding, x, edge_attrs, edge_index, pairs):
                 # one kernel: last radial layer (wgmma, weights resident in shared memory) -> TP -> scatter
                 y = tc["fused"](edge_embedding, x, edge_attrs, edge_index[0], edge_index[1])
                 if y is not None:
@@ -426,7 +427,7 @@ class InteractionBlock(torch.nn.Module):
                         x = tc["sc"](x_in, types, x)
                     return x
             if tc["mlp"] is not None:
-                w = tc["mlp"](edge_embedding)
+                w = tc["mlp"](edge_embedding, pairs)
             else:
                 self._note_fallback("radial MLP shape not supported by the grouped GEMM (needs at least one hidden "
                                     "layer, num_bessels and widths multiples of 4)")
@@ -512,8 +513,8 @@ class ConvNetLayer(torch.nn.Module):
         self.irreps_out = layer_out
 
     def forward(self, x, node_attrs, edge_attrs, edge_embedding, edge_index, types=None, type_table=None,
-                n_own=None, halo=None):
-        x = self.conv(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, type_table, n_own, halo)
+                n_own=None, halo=None, pairs=None):
+        x = self.conv(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, type_table, n_own, halo, pairs)
         return self.equivariant_nonlin(x)
 
 
@@ -634,6 +635,17 @@ class NequIPEnergyModel(torch.nn.Module):
             layer.conv.strict_fast_path = bool(on)
         return self
 
+    def _edge_pairs(self, edge_index, shift, edge_embedding, num_nodes):
+        """The reverse-edge pair map (``ops.edge_pairs``) that every layer's radial MLP shares, built on every call
+        (the edge list changes between MD steps); None when the radial MLP cannot use it (it needs the [8, 128] ->
+        [128, W] tensor-core MLP on float32)."""
+        if not (self.num_bessels == 8 and self.config["radial_mlp_depth"] == 1 and self.config["radial_mlp_width"] == 128
+                and edge_embedding.dtype == torch.float32 and self.node_layout == "ir_mul"):
+            return None
+        dst = edge_index[0]
+        csr = ops.csr_cache.get(dst if dst.dtype == torch.int64 else dst.long().contiguous(), num_nodes)
+        return ops.edge_pairs(edge_index, shift, edge_embedding, csr)
+
     @staticmethod
     def _reduce_energy(e_atom: torch.Tensor, data: Dict[str, torch.Tensor]) -> torch.Tensor:
         """AtomwiseReduce (atomwise.py:92-113): per-graph sum -> [num_graphs, 1]; one frame without ``batch``."""
@@ -670,8 +682,9 @@ class NequIPEnergyModel(torch.nn.Module):
             _vec, edge_attrs, edge_embedding = ops.edge_embed(
                 pos, edge_index, shift, cell, lmax=self.l_max, num_bessel=self.num_bessels, r_max=self.r_max,
                 poly_p=self.poly_p, prefactor=pre, out_dtype=self.model_dtype, edge_grad_sink=sink)
+        pairs = self._edge_pairs(edge_index, None if EDGE_VECTORS_KEY in data else shift, edge_embedding, types.numel())
         for layer in self.layers:
-            x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight)
+            x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight, pairs=pairs)
         e_atom = self.readout(x).to(torch.float64)
         if self.scales.numel():
             e_atom = e_atom * self.scales[types]
@@ -701,8 +714,10 @@ class NequIPEnergyModel(torch.nn.Module):
         _vec, edge_attrs, edge_embedding = ops.edge_embed(
             pos, edge_index, shift, cell, lmax=self.l_max, num_bessel=self.num_bessels, r_max=self.r_max,
             poly_p=self.poly_p, prefactor=(2 * math.pi) / (self.r_max * self.r_max), out_dtype=self.model_dtype)
+        pairs = self._edge_pairs(edge_index, shift, edge_embedding, types.numel())
         for layer in self.layers:
-            x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight, n_own, halo)
+            x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight, n_own, halo,
+                      pairs)
         e_atom = self.readout(x).to(torch.float64)
         t_own = types[:n_own]
         if self.scales.numel():

@@ -784,6 +784,62 @@ class GroupedGemm:
         )
         return c
 
+    def run_pairs(self, a: torch.Tensor, c: torch.Tensor, pairs: Tuple[torch.Tensor, torch.Tensor]):
+        """C on the slots of ``edge_pairs``: ``a`` holds one row per slot (rows < U are read) and result row u is
+        stored to the C rows ``pair_rows[u]`` (the second when >= 0).  Plain problems only."""
+        pair_rows, count = pairs
+        _require_cuda(a, c, pair_rows, count)
+        if a.dtype != torch.float32 or c.dtype != torch.float32:
+            raise TypeError("GroupedGemm.run_pairs: float32 only")
+        if any(p.act != "none" or p.accumulate or p.atomic or p.skip_zero_rows or p.rs_off >= 0 for p in self.problems):
+            raise ValueError("GroupedGemm.run_pairs: plain problems only (no row scale, accumulate, atomic or activation)")
+        if pair_rows.dtype != torch.int64 or count.dtype != torch.int64 or pair_rows.dim() != 2 or pair_rows.shape[1] != 2:
+            raise ValueError("GroupedGemm.run_pairs: pair_rows must be [E, 2] and count [1], int64")
+        _capi.check(
+            _capi.lib().nqb_gemm_grouped_pairs(_ptr(self.descs), self.ndesc, self.ntiles_total, _ptr(self.tile_ctas),
+                                               int(self.sched_ctas), _ptr(a), _ptr(self.prepared), _ptr(c),
+                                               _ptr(pair_rows), _ptr(count), int(pair_rows.shape[0]), _stream()),
+            "nqb_gemm_grouped_pairs",
+        )
+        return c
+
+
+def edge_pairs(edge_index: torch.Tensor, shift: Optional[torch.Tensor], emb: torch.Tensor,
+               csr: EdgeCSR) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Reverse-edge pair map of the radial MLP (``nqb_edge_pairs``): ``(pair_rows [E, 2], count [1])``, int64 on the
+    device.  Slot u < count holds (representative edge, its reverse edge or -1); the two edges of a slot have bitwise
+    equal ``emb`` rows, so the radial MLP computes the slot's row once.  ``shift`` [E, 3] or None; ``csr``: the
+    destination CSR of ``edge_index[0]`` (``csr_cache``).  No host synchronisation (capturable)."""
+    _require_cuda(edge_index, emb)
+    if emb.dtype != torch.float32 or emb.dim() != 2:
+        raise TypeError("edge_pairs: emb must be [E, num_bessel] float32")
+    edge_index = edge_index.long().contiguous()
+    E = edge_index.shape[1]
+    if emb.shape[0] != E or csr.num_edges != E:
+        raise ValueError("edge_pairs: emb / csr do not match edge_index")
+    emb = emb.contiguous()
+    if shift is not None:
+        shift = shift.double().contiguous()
+    L = _capi.lib()
+    dev = edge_index.device
+    pair_rows = torch.empty((E, 2), dtype=torch.int64, device=dev)
+    count = torch.empty(1, dtype=torch.int64, device=dev)
+    work = torch.empty(int(L.nqb_edge_pairs_work_size(E)), dtype=torch.int64, device=dev)
+    _capi.check(L.nqb_edge_pairs(_ptr(edge_index), E, csr.num_nodes, _ptr(shift), _ptr(emb), emb.shape[1],
+                                 _ptr(csr.row_ptr), _ptr(csr.perm), _ptr(work), _ptr(pair_rows), _ptr(count), _stream()),
+                "nqb_edge_pairs")
+    return pair_rows, count
+
+
+def mlp_hidden_fwd_rows(emb: torch.Tensor, w1s: torch.Tensor, pairs: Tuple[torch.Tensor, torch.Tensor],
+                        h: torch.Tensor) -> None:
+    """``h[u] = silu(emb[pair_rows[u, 0]] @ w1s)`` for the slots u < count of ``edge_pairs``."""
+    pair_rows, count = pairs
+    _require_cuda(emb, w1s, pair_rows, count, h)
+    _capi.check(_capi.lib().nqb_mlp_hidden_fwd_rows(_ptr(emb), _ptr(w1s), _ptr(pair_rows), _ptr(count),
+                                                    pair_rows.shape[0], emb.shape[1], w1s.shape[1], _ptr(h), _stream()),
+                "nqb_mlp_hidden_fwd_rows")
+
 
 def mlp_hidden_fwd(emb: torch.Tensor, w1s: torch.Tensor, h: torch.Tensor, h_lo=None) -> None:
     """``h = silu(emb @ w1s)`` ([E,8] x [8,128]).  ``h_lo`` exists only so that ``bench.py``'s four-argument call
