@@ -156,6 +156,22 @@ int nqb_edge_embed_bwd(int lmax, int num_bessel, double r_max, double poly_p, do
                        const double* vec, const int64_t* edge_index, int64_t N, int64_t E,
                        int out_dtype, const void* grad_y, const void* grad_emb, double* grad_pos,
                        double* grad_vec, nqb_stream_t st);
+/* Per-edge-type cutoffs (nequip/nn/embedding/_edge.py:65-80 with per_edge_type_cutoff): as nqb_edge_embed_fwd/bwd,
+ * with the normalised length x = |r| * recip[T * types[type_index[0][e]] + types[type_index[1][e]]] (and dx/d|r| =
+ * that recip) in place of |r| / r_max; prefactor stays the caller's (2 pi / r_max^2 of the global r_max).
+ * types [N'] i64 in [0, T), type_index [2,E] i64, recip [T*T] f64 (1 / rc[source, target]): device arrays.
+ * type_index is edge_index for positions; given edge vectors come with made-up positions, and type_index is then the
+ * real list.  Same write contracts. */
+int nqb_edge_embed_fwd_typed(int lmax, int num_bessel, double r_max, double poly_p, double prefactor,
+                             const double* pos, const int64_t* edge_index, const double* shift,
+                             const double* cell, int64_t N, int64_t E, const int64_t* types,
+                             const int64_t* type_index, const double* recip, int T, int out_dtype, double* vec,
+                             void* y, void* emb, nqb_stream_t st);
+int nqb_edge_embed_bwd_typed(int lmax, int num_bessel, double r_max, double poly_p, double prefactor,
+                             const double* vec, const int64_t* edge_index, int64_t N, int64_t E,
+                             const int64_t* types, const int64_t* type_index, const double* recip, int T,
+                             int out_dtype, const void* grad_y, const void* grad_emb, double* grad_pos,
+                             double* grad_vec, nqb_stream_t st);
 
 /* ZBL pair energy (nequip/nn/pair_potential.py:230-386), everything in fp64.  Per edge e = (i -> j), i =
  * edge_index[0][e]:  eps_e = A[ti,tj] / r * psi((S[ti,tj] * r) / a0) * f_c(r / r_max),  psi = the four-exponential
@@ -177,6 +193,16 @@ int nqb_zbl_bwd(const double* pos, const int64_t* edge_index, const double* shif
                 const double* vec, const int64_t* types, const double* table, int T, int64_t N, int64_t E,
                 double r_max, double poly_p, int cutoff_f32, const double* grad_e_atom, double* grad_pos,
                 double* grad_vec, nqb_stream_t st);
+/* Per-edge-type cutoffs: the envelope takes x = r * recip[T * t_i + t_j] (recip [T*T] f64, device) instead of
+ * r * (1 / r_max); the ZBL term itself keeps r.  An edge with x >= 1 adds exactly +0.  Same write contracts. */
+int nqb_zbl_fwd_typed(const double* pos, const int64_t* edge_index, const double* shift, const double* cell,
+                      const double* vec, const int64_t* types, const double* table, int T, const int64_t* row_ptr,
+                      const int64_t* perm, int64_t N, int64_t E, double r_max, double poly_p, int cutoff_f32,
+                      const double* recip, double* e_atom, nqb_stream_t st);
+int nqb_zbl_bwd_typed(const double* pos, const int64_t* edge_index, const double* shift, const double* cell,
+                      const double* vec, const int64_t* types, const double* table, int T, int64_t N, int64_t E,
+                      double r_max, double poly_p, int cutoff_f32, const double* recip, const double* grad_e_atom,
+                      double* grad_pos, double* grad_vec, nqb_stream_t st);
 
 /* Neighbour list on the device (cell list; full list, both directions, periodic images, no self edge in the home
  * image) -- replaces the host construction of nequip/data/_nl.py:60-152,292-361 and emits what
@@ -236,6 +262,35 @@ int nqb_nl_fill_capacity_dp(int64_t N, int64_t capacity, const void* params_dev,
                             const int64_t* row_ptr_pad /* [N+1] */, const int32_t* overflow /* [1] */,
                             int64_t* edge_index /* [2,capacity] */, double* shifts /* [capacity,3] */,
                             nqb_stream_t st);
+/* Per-edge-type cutoffs: count, fill and fill with capacity (by value and _dp) with the membership test
+ * d2 < rc2[T * types[i] + types[j]] in place of d2 < r_max^2.  types [N] i64 in [0, T) and rc2 [T*T] f64 (rc * rc in
+ * float64, every rc <= r_max) are device arrays; bins, search ranges and parameter blocks stay those of r_max, so
+ * nqb_nl_bin, nqb_nl_pad and nqb_nl_params_pack are shared.  Same write contracts as the untyped calls. */
+int nqb_nl_count_typed(int64_t N, const double* cell_host, const double* inv_host, const int* pbc, const int* nbins,
+                       const int* search, double r_max, const double* wpos, const int32_t* cidx, const int64_t* order,
+                       const int64_t* bin_start, const int64_t* types, const double* rc2, int T,
+                       int64_t* counts /* [N] */, nqb_stream_t st);
+int nqb_nl_fill_typed(int64_t N, int64_t E, const double* cell_host, const double* inv_host, const int* pbc,
+                      const int* nbins, const int* search, double r_max, const double* wpos, const int32_t* cidx,
+                      const int32_t* base, const int64_t* order, const int64_t* bin_start,
+                      const int64_t* row_ptr /* [N+1] */, const int64_t* types, const double* rc2, int T,
+                      int64_t* edge_index /* [2,E] */, double* shifts /* [E,3] */, nqb_stream_t st);
+int nqb_nl_fill_capacity_typed(int64_t N, int64_t capacity, const double* cell_host, const double* inv_host,
+                               const int* pbc, const int* nbins, const int* search, double r_max, const double* wpos,
+                               const int32_t* cidx, const int32_t* base, const int64_t* order,
+                               const int64_t* bin_start, const int64_t* row_ptr_pad /* [N+1] */,
+                               const int32_t* overflow /* [1] */, const double* pad_shift_host, const int64_t* types,
+                               const double* rc2, int T, int64_t* edge_index /* [2,capacity] */,
+                               double* shifts /* [capacity,3] */, nqb_stream_t st);
+int nqb_nl_count_dp_typed(int64_t N, const void* params_dev, const double* wpos, const int32_t* cidx,
+                          const int64_t* order, const int64_t* bin_start, const int64_t* types, const double* rc2,
+                          int T, int64_t* counts /* [N] */, nqb_stream_t st);
+int nqb_nl_fill_capacity_dp_typed(int64_t N, int64_t capacity, const void* params_dev, const double* wpos,
+                                  const int32_t* cidx, const int32_t* base, const int64_t* order,
+                                  const int64_t* bin_start, const int64_t* row_ptr_pad /* [N+1] */,
+                                  const int32_t* overflow /* [1] */, const int64_t* types, const double* rc2, int T,
+                                  int64_t* edge_index /* [2,capacity] */, double* shifts /* [capacity,3] */,
+                                  nqb_stream_t st);
 
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).

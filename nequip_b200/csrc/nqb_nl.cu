@@ -15,6 +15,7 @@
 // explicitly rounded operations (no FMA contraction), so the edge set is bit-identical.
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdio.h>
 #include <string.h>
 
 #include "../../include/nqb.h"
@@ -52,6 +53,15 @@ __device__ __forceinline__ double3 nl_pad_shift(const NlParams&, double3 pad_shi
 __device__ __forceinline__ double3 nl_pad_shift(NlBlockPtr b, double3) {
   return make_double3(b->pad_shift[0], b->pad_shift[1], b->pad_shift[2]);
 }
+
+// Per-edge-type cutoffs (kTyped): the pair (i, j) is a neighbour when d2 < rc2[T * types[i] + types[j]] instead of
+// d2 < r2.  rc2 = rc * rc is computed on the host in float64; the bins stay sized by the global r_max >= every rc.
+// The untyped kernels take this parameter last and never read it, so their code is unchanged.
+struct NlTypes {
+  const int64_t* types;  // [N]
+  const double* rc2;     // [T * T]
+  int T;
+};
 
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
@@ -97,11 +107,12 @@ __global__ void k_nl_bin(PS ps, const double* __restrict__ pos, int64_t N, doubl
 }
 
 // visit every (neighbour atom j, image) candidate of atom i; F(j, img[3], within cutoff)
-template <class F>
-__device__ __forceinline__ void nl_visit(const NlParams& p, int64_t i, const double* __restrict__ wpos,
+template <bool kTyped, class F>
+__device__ __forceinline__ void nl_visit(const NlParams& p, const NlTypes& ty, int64_t i, const double* __restrict__ wpos,
                                          const int32_t* __restrict__ cidx, const int64_t* __restrict__ order,
                                          const int64_t* __restrict__ bin_start, F&& f) {
   const double xi = wpos[3 * i], yi = wpos[3 * i + 1], zi = wpos[3 * i + 2];
+  const double* rc2_i = kTyped ? ty.rc2 + (int64_t)ty.T * ty.types[i] : nullptr;
   const int c0 = cidx[3 * i], c1 = cidx[3 * i + 1], c2 = cidx[3 * i + 2];
   for (int oz = -p.sr[2]; oz <= p.sr[2]; ++oz) {
     int bz = c2 + oz, iz = 0;
@@ -132,21 +143,21 @@ __device__ __forceinline__ void nl_visit(const NlParams& p, int64_t i, const dou
           const double dx = dadd(dadd(wpos[3 * j], sx), -xi), dy = dadd(dadd(wpos[3 * j + 1], sy), -yi),
                        dz = dadd(dadd(wpos[3 * j + 2], sz), -zi);
           const double d2 = dadd(dadd(dmul(dx, dx), dmul(dy, dy)), dmul(dz, dz));
-          if (d2 < p.r2) f(j, ix, iy, iz);
+          if (kTyped ? d2 < rc2_i[ty.types[j]] : d2 < p.r2) f(j, ix, iy, iz);
         }
       }
     }
   }
 }
 
-template <class PS>
+template <class PS, bool kTyped = false>
 __global__ void k_nl_count(PS ps, int64_t N, const double* __restrict__ wpos, const int32_t* __restrict__ cidx,
                            const int64_t* __restrict__ order, const int64_t* __restrict__ bin_start,
-                           int64_t* __restrict__ counts) {
+                           int64_t* __restrict__ counts, NlTypes ty) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   int64_t n = 0;
-  nl_visit(nl_p(ps), i, wpos, cidx, order, bin_start, [&](int64_t, int, int, int) { ++n; });
+  nl_visit<kTyped>(nl_p(ps), ty, i, wpos, cidx, order, bin_start, [&](int64_t, int, int, int) { ++n; });
   counts[i] = n;
 }
 
@@ -163,19 +174,19 @@ __device__ __forceinline__ bool nl_less(int64_t ja, const double* sa, int64_t jb
 // hold null edges (i, i, pad_shift).  The trailing parameters are appended so the unpadded variant's code is unchanged.
 // With PS = NlBlockPtr (only with kCapacity) the null-edge shift comes from the block and the pad_shift argument is
 // not read.
-template <bool kCapacity, class PS>
+template <bool kCapacity, class PS, bool kTyped = false>
 __global__ void k_nl_fill(PS ps, int64_t N, const double* __restrict__ wpos, const int32_t* __restrict__ cidx,
                           const int32_t* __restrict__ base, const int64_t* __restrict__ order,
                           const int64_t* __restrict__ bin_start, const int64_t* __restrict__ row_ptr, int64_t E,
                           int64_t* __restrict__ edge_index, double* __restrict__ shifts,
-                          const int32_t* __restrict__ overflow, double3 pad_shift) {
+                          const int32_t* __restrict__ overflow, double3 pad_shift, NlTypes ty) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   const int64_t beg = row_ptr[i];
   int64_t n = 0;
   int64_t* ej = edge_index + E;  // neighbours (row 1)
   if (!kCapacity || *overflow == 0) {
-    nl_visit(nl_p(ps), i, wpos, cidx, order, bin_start, [&](int64_t j, int ix, int iy, int iz) {
+    nl_visit<kTyped>(nl_p(ps), ty, i, wpos, cidx, order, bin_start, [&](int64_t j, int ix, int iy, int iz) {
       // insertion into the sorted prefix of the row (rows hold a few dozen neighbours)
       double s[3] = {(double)(ix + base[3 * j] - base[3 * i]), (double)(iy + base[3 * j + 1] - base[3 * i + 1]),
                      (double)(iz + base[3 * j + 2] - base[3 * i + 2])};
@@ -266,7 +277,8 @@ extern "C" int nqb_nl_count(int64_t N, const double* cell_host, const double* in
   if (!wpos || !cidx || !order || !bin_start || !counts) return nqb_set_error("nqb_nl_count: null pointer");
   NlParams p;
   nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
-  k_nl_count<NlParams><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(p, N, wpos, cidx, order, bin_start, counts);
+  k_nl_count<NlParams><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(p, N, wpos, cidx, order, bin_start, counts,
+                                                                                NlTypes{});
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -285,7 +297,8 @@ extern "C" int nqb_nl_fill(int64_t N, int64_t E, const double* cell_host, const 
   NlParams p;
   nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
   k_nl_fill<false, NlParams><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
-      p, N, wpos, cidx, base, order, bin_start, row_ptr, E, edge_index, shifts, nullptr, make_double3(0.0, 0.0, 0.0));
+      p, N, wpos, cidx, base, order, bin_start, row_ptr, E, edge_index, shifts, nullptr, make_double3(0.0, 0.0, 0.0),
+      NlTypes{});
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -320,7 +333,7 @@ extern "C" int nqb_nl_fill_capacity(int64_t N, int64_t capacity, const double* c
   nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
   const double3 ps = make_double3(pad_shift_host[0], pad_shift_host[1], pad_shift_host[2]);
   k_nl_fill<true, NlParams><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
-      p, N, wpos, cidx, base, order, bin_start, row_ptr_pad, capacity, edge_index, shifts, overflow, ps);
+      p, N, wpos, cidx, base, order, bin_start, row_ptr_pad, capacity, edge_index, shifts, overflow, ps, NlTypes{});
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -367,7 +380,7 @@ extern "C" int nqb_nl_count_dp(int64_t N, const void* params_dev, const double* 
   if (!params_dev || !wpos || !cidx || !order || !bin_start || !counts)
     return nqb_set_error("nqb_nl_count_dp: null pointer");
   k_nl_count<NlBlockPtr><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
-      (const NlBlock*)params_dev, N, wpos, cidx, order, bin_start, counts);
+      (const NlBlock*)params_dev, N, wpos, cidx, order, bin_start, counts, NlTypes{});
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -385,9 +398,114 @@ extern "C" int nqb_nl_fill_capacity_dp(int64_t N, int64_t capacity, const void* 
     return nqb_set_error("nqb_nl_fill_capacity_dp: null pointer");
   k_nl_fill<true, NlBlockPtr><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
       (const NlBlock*)params_dev, N, wpos, cidx, base, order, bin_start, row_ptr_pad, capacity, edge_index, shifts,
-      overflow, make_double3(0.0, 0.0, 0.0));
+      overflow, make_double3(0.0, 0.0, 0.0), NlTypes{});
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
   return 0;
+}
+
+// Per-edge-type cutoffs: nqb_nl_count, nqb_nl_fill, nqb_nl_fill_capacity and their _dp forms with the membership test
+// d2 < rc2[T * types[i] + types[j]].  types [N] i64 in [0, T) and rc2 [T * T] f64 (rc * rc, every rc <= r_max) are
+// device arrays; the bins, search ranges and parameter blocks are those of r_max.
+static int nl_types(const char* what, const int64_t* types, const double* rc2, int T, NlTypes& ty) {
+  if (T < 1 || !types || !rc2) {
+    static thread_local char msg[160];
+    snprintf(msg, sizeof(msg), "%s: needs types, rc2 and T >= 1", what);
+    return nqb_set_error(msg);
+  }
+  ty = NlTypes{types, rc2, T};
+  return 0;
+}
+
+static int nl_launch_done() {
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int nqb_nl_count_typed(int64_t N, const double* cell_host, const double* inv_host, const int* pbc,
+                                  const int* nbins, const int* search, double r_max, const double* wpos,
+                                  const int32_t* cidx, const int64_t* order, const int64_t* bin_start,
+                                  const int64_t* types, const double* rc2, int T, int64_t* counts, nqb_stream_t st) {
+  if (N <= 0) return 0;
+  if (!wpos || !cidx || !order || !bin_start || !counts) return nqb_set_error("nqb_nl_count_typed: null pointer");
+  NlTypes ty;
+  if (int rc = nl_types("nqb_nl_count_typed", types, rc2, T, ty)) return rc;
+  NlParams p;
+  nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
+  k_nl_count<NlParams, true><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(p, N, wpos, cidx, order, bin_start,
+                                                                                      counts, ty);
+  return nl_launch_done();
+}
+
+extern "C" int nqb_nl_fill_typed(int64_t N, int64_t E, const double* cell_host, const double* inv_host, const int* pbc,
+                                 const int* nbins, const int* search, double r_max, const double* wpos,
+                                 const int32_t* cidx, const int32_t* base, const int64_t* order,
+                                 const int64_t* bin_start, const int64_t* row_ptr, const int64_t* types,
+                                 const double* rc2, int T, int64_t* edge_index, double* shifts, nqb_stream_t st) {
+  if (N <= 0 || E <= 0) return 0;
+  if (!wpos || !cidx || !base || !order || !bin_start || !row_ptr || !edge_index || !shifts)
+    return nqb_set_error("nqb_nl_fill_typed: null pointer");
+  NlTypes ty;
+  if (int rc = nl_types("nqb_nl_fill_typed", types, rc2, T, ty)) return rc;
+  NlParams p;
+  nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
+  k_nl_fill<false, NlParams, true><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
+      p, N, wpos, cidx, base, order, bin_start, row_ptr, E, edge_index, shifts, nullptr, make_double3(0.0, 0.0, 0.0), ty);
+  return nl_launch_done();
+}
+
+extern "C" int nqb_nl_fill_capacity_typed(int64_t N, int64_t capacity, const double* cell_host, const double* inv_host,
+                                          const int* pbc, const int* nbins, const int* search, double r_max,
+                                          const double* wpos, const int32_t* cidx, const int32_t* base,
+                                          const int64_t* order, const int64_t* bin_start, const int64_t* row_ptr_pad,
+                                          const int32_t* overflow, const double* pad_shift_host, const int64_t* types,
+                                          const double* rc2, int T, int64_t* edge_index, double* shifts,
+                                          nqb_stream_t st) {
+  if (N <= 0 || capacity < 0) return nqb_set_error("nqb_nl_fill_capacity_typed: needs N > 0 and capacity >= 0");
+  if (capacity == 0) return 0;
+  if (!wpos || !cidx || !base || !order || !bin_start || !row_ptr_pad || !overflow || !pad_shift_host || !edge_index ||
+      !shifts)
+    return nqb_set_error("nqb_nl_fill_capacity_typed: null pointer");
+  NlTypes ty;
+  if (int rc = nl_types("nqb_nl_fill_capacity_typed", types, rc2, T, ty)) return rc;
+  NlParams p;
+  nl_params(cell_host, inv_host, pbc, nbins, search, r_max, p);
+  const double3 ps = make_double3(pad_shift_host[0], pad_shift_host[1], pad_shift_host[2]);
+  k_nl_fill<true, NlParams, true><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
+      p, N, wpos, cidx, base, order, bin_start, row_ptr_pad, capacity, edge_index, shifts, overflow, ps, ty);
+  return nl_launch_done();
+}
+
+extern "C" int nqb_nl_count_dp_typed(int64_t N, const void* params_dev, const double* wpos, const int32_t* cidx,
+                                     const int64_t* order, const int64_t* bin_start, const int64_t* types,
+                                     const double* rc2, int T, int64_t* counts, nqb_stream_t st) {
+  if (N <= 0) return 0;
+  if (!params_dev || !wpos || !cidx || !order || !bin_start || !counts)
+    return nqb_set_error("nqb_nl_count_dp_typed: null pointer");
+  NlTypes ty;
+  if (int rc = nl_types("nqb_nl_count_dp_typed", types, rc2, T, ty)) return rc;
+  k_nl_count<NlBlockPtr, true><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
+      (const NlBlock*)params_dev, N, wpos, cidx, order, bin_start, counts, ty);
+  return nl_launch_done();
+}
+
+extern "C" int nqb_nl_fill_capacity_dp_typed(int64_t N, int64_t capacity, const void* params_dev, const double* wpos,
+                                             const int32_t* cidx, const int32_t* base, const int64_t* order,
+                                             const int64_t* bin_start, const int64_t* row_ptr_pad,
+                                             const int32_t* overflow, const int64_t* types, const double* rc2, int T,
+                                             int64_t* edge_index, double* shifts, nqb_stream_t st) {
+  if (N <= 0 || capacity < 0) return nqb_set_error("nqb_nl_fill_capacity_dp_typed: needs N > 0 and capacity >= 0");
+  if (capacity == 0) return 0;
+  if (!params_dev || !wpos || !cidx || !base || !order || !bin_start || !row_ptr_pad || !overflow || !edge_index ||
+      !shifts)
+    return nqb_set_error("nqb_nl_fill_capacity_dp_typed: null pointer");
+  NlTypes ty;
+  if (int rc = nl_types("nqb_nl_fill_capacity_dp_typed", types, rc2, T, ty)) return rc;
+  k_nl_fill<true, NlBlockPtr, true><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
+      (const NlBlock*)params_dev, N, wpos, cidx, base, order, bin_start, row_ptr_pad, capacity, edge_index, shifts,
+      overflow, make_double3(0.0, 0.0, 0.0), ty);
+  return nl_launch_done();
 }

@@ -18,6 +18,8 @@
 //              grad_vec[e].
 // Edges with x = r / r_max >= 1 (null edges of a padded list among them) return eps = 0 and d eps / dr = 0 before any
 // exponential is evaluated, so they add exactly +0 to their row and nothing to the gradients.
+// Per-edge-type cutoffs (kTyped, nqb_zbl_*_typed): the envelope takes x = r * recip[T * t_i + t_j]
+// (pair_potential.py:374 reads the normalised length of EdgeLengthNormalizer); the ZBL physics keeps r.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -69,9 +71,11 @@ __device__ __forceinline__ void edge_vector(const ZblGeom& g, int64_t e, int64_t
   }
 }
 
-// eps and (when dedr != NULL) d eps / dr of one edge of length r; A, S from the type-pair table
-__device__ __forceinline__ double zbl_edge(double r, double A, double S, const ZblParams& q, double* dedr) {
-  const double xc = r * (1.0 / q.r_max);  // EdgeLengthNormalizer: r * (1 / r_max)
+// eps and (when dedr != NULL) d eps / dr of one edge of length r; A, S from the type-pair table; recip = 1 / rc of the
+// edge's type pair (read only when kTyped)
+template <bool kTyped>
+__device__ __forceinline__ double zbl_edge(double r, double A, double S, const ZblParams& q, double recip, double* dedr) {
+  const double xc = kTyped ? r * recip : r * (1.0 / q.r_max);  // EdgeLengthNormalizer: r * (1 / r_max)
   if (!(xc < 1.0)) {
     if (dedr) *dedr = 0.0;
     return 0.0;
@@ -90,15 +94,17 @@ __device__ __forceinline__ double zbl_edge(double r, double A, double S, const Z
   if (dedr) {
     const double dpsi = (kC1 * kD1 * e1 + kC2 * kD2 * e2 + kC3 * kD3 * e3 + kC4 * kD4 * e4) * (S / kA0);
     const double xpm1 = pow(xc, p - 1.0);
-    const double dfc = 0.5 * p * (p + 1.0) * (p + 2.0) * (-xpm1 + 2.0 * xpm1 * xc - xpm1 * xc * xc) / q.r_max;
+    const double dpoly = 0.5 * p * (p + 1.0) * (p + 2.0) * (-xpm1 + 2.0 * xpm1 * xc - xpm1 * xc * xc);
+    const double dfc = kTyped ? dpoly * recip : dpoly / q.r_max;
     *dedr = A * inv_r * ((dpsi - psi * inv_r) * fc + psi * dfc);
   }
   return A * inv_r * psi * fc;
 }
 
+template <bool kTyped = false>
 __global__ void k_zbl_fwd(ZblGeom g, ZblParams q, const int64_t* __restrict__ types, const double* __restrict__ table,
                           const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ perm, int64_t N,
-                          double* __restrict__ e_atom) {
+                          double* __restrict__ e_atom, const double* __restrict__ recip) {
   const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= N) return;  // uniform over the warp
@@ -114,8 +120,9 @@ __global__ void k_zbl_fwd(ZblGeom g, ZblParams q, const int64_t* __restrict__ ty
       double vx, vy, vz;
       edge_vector(g, e, i0, i1, vx, vy, vz);
       const double r = sqrt(vx * vx + vy * vy + vz * vz);
-      const double* t = table + 2 * (ti * q.T + types[i1]);
-      eps = zbl_edge(r, t[0], t[1], q, nullptr);
+      const int64_t tt = ti * q.T + types[i1];
+      const double* t = table + 2 * tt;
+      eps = zbl_edge<kTyped>(r, t[0], t[1], q, kTyped ? recip[tt] : 0.0, nullptr);
     }
     const int cnt = (int)min((int64_t)32, end - base);
     for (int k = 0; k < cnt; ++k) s += __shfl_sync(0xffffffffu, eps, k);  // CSR order
@@ -123,17 +130,20 @@ __global__ void k_zbl_fwd(ZblGeom g, ZblParams q, const int64_t* __restrict__ ty
   if (lane == 0) e_atom[row] = s;
 }
 
+template <bool kTyped = false>
 __global__ void k_zbl_bwd(ZblGeom g, ZblParams q, const int64_t* __restrict__ types, const double* __restrict__ table,
-                          const double* __restrict__ grad_e, double* __restrict__ gpos, double* __restrict__ gvec) {
+                          const double* __restrict__ grad_e, double* __restrict__ gpos, double* __restrict__ gvec,
+                          const double* __restrict__ recip) {
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= g.E) return;
   const int64_t i0 = g.eidx[e], i1 = g.eidx[g.E + e];
   double vx, vy, vz;
   edge_vector(g, e, i0, i1, vx, vy, vz);
   const double r = sqrt(vx * vx + vy * vy + vz * vz);
-  const double* t = table + 2 * (types[i0] * q.T + types[i1]);
+  const int64_t tt = types[i0] * q.T + types[i1];
+  const double* t = table + 2 * tt;
   double dedr;
-  zbl_edge(r, t[0], t[1], q, &dedr);
+  zbl_edge<kTyped>(r, t[0], t[1], q, kTyped ? recip[tt] : 0.0, &dedr);
   const double c = dedr == 0.0 ? 0.0 : grad_e[i0] * dedr / r;
   const double gx = c * vx, gy = c * vy, gz = c * vz;
   if (gvec != nullptr) { gvec[3 * e] = gx; gvec[3 * e + 1] = gy; gvec[3 * e + 2] = gz; }
@@ -175,7 +185,7 @@ extern "C" int nqb_zbl_fwd(const double* pos, const int64_t* edge_index, const d
   ZblGeom g{pos, edge_index, shift, cell, vec, E};
   ZblParams q{r_max, poly_p, cutoff_f32 ? 1 : 0, T};
   const unsigned blocks = (unsigned)((N + 3) / 4);  // 4 rows (warps) per 128-thread block
-  k_zbl_fwd<<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, row_ptr, perm, N, e_atom);
+  k_zbl_fwd<<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, row_ptr, perm, N, e_atom, nullptr);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -194,7 +204,49 @@ extern "C" int nqb_zbl_bwd(const double* pos, const int64_t* edge_index, const d
   ZblGeom g{pos, edge_index, shift, cell, vec, E};
   ZblParams q{r_max, poly_p, cutoff_f32 ? 1 : 0, T};
   const unsigned blocks = (unsigned)((E + 127) / 128);
-  k_zbl_bwd<<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, grad_e_atom, grad_pos, grad_vec);
+  k_zbl_bwd<<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, grad_e_atom, grad_pos, grad_vec, nullptr);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+// Per-edge-type cutoffs: as above, with the envelope at x = r * recip[T * t_i + t_j] (recip [T * T] f64, device).
+extern "C" int nqb_zbl_fwd_typed(const double* pos, const int64_t* edge_index, const double* shift, const double* cell,
+                                 const double* vec, const int64_t* types, const double* table, int T,
+                                 const int64_t* row_ptr, const int64_t* perm, int64_t N, int64_t E, double r_max,
+                                 double poly_p, int cutoff_f32, const double* recip, double* e_atom, nqb_stream_t st) {
+  if (int rc = check_common("nqb_zbl_fwd_typed", pos, edge_index, shift, cell, vec, types, table, T, N, E, r_max,
+                            poly_p))
+    return rc;
+  if (N == 0) return 0;
+  if (!row_ptr || !e_atom) return nqb_set_error("nqb_zbl_fwd_typed: null row_ptr / e_atom");
+  if (!recip) return nqb_set_error("nqb_zbl_fwd_typed: null recip");
+  ZblGeom g{pos, edge_index, shift, cell, vec, E};
+  ZblParams q{r_max, poly_p, cutoff_f32 ? 1 : 0, T};
+  const unsigned blocks = (unsigned)((N + 3) / 4);
+  k_zbl_fwd<true><<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, row_ptr, perm, N, e_atom, recip);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int nqb_zbl_bwd_typed(const double* pos, const int64_t* edge_index, const double* shift, const double* cell,
+                                 const double* vec, const int64_t* types, const double* table, int T, int64_t N,
+                                 int64_t E, double r_max, double poly_p, int cutoff_f32, const double* recip,
+                                 const double* grad_e_atom, double* grad_pos, double* grad_vec, nqb_stream_t st) {
+  if (int rc = check_common("nqb_zbl_bwd_typed", pos, edge_index, shift, cell, vec, types, table, T, N, E, r_max,
+                            poly_p))
+    return rc;
+  if (grad_pos != nullptr && vec != nullptr) return nqb_set_error("nqb_zbl_bwd_typed: grad_pos needs positions, not vec");
+  if (E == 0) return 0;
+  if (!grad_e_atom || (!grad_pos && !grad_vec)) return nqb_set_error("nqb_zbl_bwd_typed: null grad_e_atom / outputs");
+  if (!recip) return nqb_set_error("nqb_zbl_bwd_typed: null recip");
+  ZblGeom g{pos, edge_index, shift, cell, vec, E};
+  ZblParams q{r_max, poly_p, cutoff_f32 ? 1 : 0, T};
+  const unsigned blocks = (unsigned)((E + 127) / 128);
+  k_zbl_bwd<true><<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, grad_e_atom, grad_pos, grad_vec, recip);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));

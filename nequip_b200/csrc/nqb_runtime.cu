@@ -565,10 +565,26 @@ __device__ __forceinline__ double poly_cutoff_deriv(double x, double p) {
   return 0.5 * p * (p + 1.0) * (p + 2.0) * (-xpm1 + 2.0 * xpm1 * x - xpm1 * x * x);
 }
 
-template <int LMAX, typename TO>
+// Per-edge-type cutoffs (nequip/nn/embedding/_edge.py:65-80 with per_edge_type_cutoff): the normalised length is
+// x = r * recip[T * type(tidx[0][e]) + type(tidx[1][e])] instead of r / r_max.  tidx names the edge's atoms for the
+// type lookup; it is the geometry's eidx except in the edge-vector branch, whose eidx indexes made-up positions.
+struct EdgeTypes {
+  const int64_t* types;  // [N'] atom types of the atoms tidx names
+  const int64_t* tidx;   // [2, E]
+  const double* recip;   // [T * T] 1 / rc[source, target]
+  int T;
+};
+
+// kTyped = false: x = r / r_max, and the trailing EdgeTypes parameter is not read (appended, so the code of the
+// untyped variants is unchanged)
+__device__ __forceinline__ double edge_recip(const EdgeTypes& et, int64_t E, int64_t e) {
+  return et.recip[et.T * et.types[et.tidx[e]] + et.types[et.tidx[E + e]]];
+}
+
+template <int LMAX, typename TO, bool kTyped = false>
 __global__ void k_edge_embed_fwd(EmbedParams prm, const double* __restrict__ pos, const int64_t* __restrict__ eidx,
                                  const double* __restrict__ shift, const double* __restrict__ cell, int64_t E,
-                                 double* __restrict__ vec, TO* __restrict__ yout, TO* __restrict__ emb) {
+                                 double* __restrict__ vec, TO* __restrict__ yout, TO* __restrict__ emb, EdgeTypes et) {
   constexpr int S = (LMAX + 1) * (LMAX + 1);
   int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
@@ -590,7 +606,7 @@ __global__ void k_edge_embed_fwd(EmbedParams prm, const double* __restrict__ pos
 #pragma unroll
   for (int q = 0; q < S; ++q) yout[e * S + q] = (TO)Y[q];
   // radial embedding: (TO)bessel * (TO)cutoff * (TO)prefactor, as the reference rounds it
-  const double x = r / prm.r_max;
+  const double x = kTyped ? r * edge_recip(et, E, e) : r / prm.r_max;
   const TO fc = (TO)poly_cutoff(x, prm.poly_p);
   const TO pre = (TO)prm.prefactor;
   for (int n = 1; n <= prm.num_bessel; ++n) {
@@ -601,10 +617,10 @@ __global__ void k_edge_embed_fwd(EmbedParams prm, const double* __restrict__ pos
   }
 }
 
-template <int LMAX, typename TO>
+template <int LMAX, typename TO, bool kTyped = false>
 __global__ void k_edge_embed_bwd(EmbedParams prm, const double* __restrict__ vec, const int64_t* __restrict__ eidx,
                                  int64_t E, const TO* __restrict__ gy, const TO* __restrict__ gemb,
-                                 double* __restrict__ gpos, double* __restrict__ gvec) {
+                                 double* __restrict__ gpos, double* __restrict__ gvec, EdgeTypes et) {
   constexpr int S = (LMAX + 1) * (LMAX + 1);
   int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
@@ -622,7 +638,8 @@ __global__ void k_edge_embed_bwd(EmbedParams prm, const double* __restrict__ vec
     gxv = (Gx - D * ux) * inv; gyv = (Gy - D * uy) * inv; gzv = (Gz - D * uz) * inv;
   }
   if (gemb != nullptr) {
-    const double x = r / prm.r_max;
+    const double recip = kTyped ? edge_recip(et, E, e) : 0.0;
+    const double x = kTyped ? r * recip : r / prm.r_max;
     const double fc = poly_cutoff(x, prm.poly_p), dfc = poly_cutoff_deriv(x, prm.poly_p);
     double dr = 0.0;
     for (int n = 1; n <= prm.num_bessel; ++n) {
@@ -636,7 +653,7 @@ __global__ void k_edge_embed_bwd(EmbedParams prm, const double* __restrict__ vec
       }
       dr += (double)gemb[e * prm.num_bessel + (n - 1)] * (db * fc + b * dfc);
     }
-    dr *= prm.prefactor / prm.r_max;
+    dr *= kTyped ? prm.prefactor * recip : prm.prefactor / prm.r_max;  // dx/dr = recip (typed) or 1 / r_max
     gxv += dr * ux; gyv += dr * uy; gzv += dr * uz;
   }
   if (gvec != nullptr) { gvec[3 * e] = gxv; gvec[3 * e + 1] = gyv; gvec[3 * e + 2] = gzv; }
@@ -663,7 +680,7 @@ extern "C" int nqb_edge_embed_fwd(int lmax, int num_bessel, double r_max, double
   EmbedParams prm{num_bessel, r_max, poly_p, prefactor};
   unsigned blocks = (unsigned)((E + 127) / 128);
   cudaStream_t s = (cudaStream_t)st;
-#define EE_FWD(L, TT) k_edge_embed_fwd<L, TT><<<blocks, 128, 0, s>>>(prm, pos, edge_index, shift, cell, E, vec, (TT*)y, (TT*)emb)
+#define EE_FWD(L, TT) k_edge_embed_fwd<L, TT><<<blocks, 128, 0, s>>>(prm, pos, edge_index, shift, cell, E, vec, (TT*)y, (TT*)emb, EdgeTypes{})
   if (out_dtype == NQB_F32) {
     switch (lmax) { case 0: EE_FWD(0, float); break; case 1: EE_FWD(1, float); break; case 2: EE_FWD(2, float); break; case 3: EE_FWD(3, float); break; default: EE_FWD(4, float); break; }
   } else {
@@ -689,7 +706,7 @@ extern "C" int nqb_edge_embed_bwd(int lmax, int num_bessel, double r_max, double
   EmbedParams prm{num_bessel, r_max, poly_p, prefactor};
   unsigned blocks = (unsigned)((E + 127) / 128);
   cudaStream_t s = (cudaStream_t)st;
-#define EE_BWD(L, TT) k_edge_embed_bwd<L, TT><<<blocks, 128, 0, s>>>(prm, vec, edge_index, E, (const TT*)grad_y, (const TT*)grad_emb, grad_pos, grad_vec)
+#define EE_BWD(L, TT) k_edge_embed_bwd<L, TT><<<blocks, 128, 0, s>>>(prm, vec, edge_index, E, (const TT*)grad_y, (const TT*)grad_emb, grad_pos, grad_vec, EdgeTypes{})
   if (out_dtype == NQB_F32) {
     switch (lmax) { case 0: EE_BWD(0, float); break; case 1: EE_BWD(1, float); break; case 2: EE_BWD(2, float); break; case 3: EE_BWD(3, float); break; default: EE_BWD(4, float); break; }
   } else {
@@ -697,6 +714,72 @@ extern "C" int nqb_edge_embed_bwd(int lmax, int num_bessel, double r_max, double
   }
 #undef EE_BWD
   NQB_LAUNCH_CHECK("nqb_edge_embed_bwd");
+  return 0;
+}
+
+static int check_edge_types(const char* what, const int64_t* types, const int64_t* type_index, const double* recip,
+                            int T) {
+  if (T < 1) return fail("%s: need at least one type", what);
+  if (!types || !type_index || !recip) return fail("%s: null types / type_index / recip", what);
+  return 0;
+}
+
+extern "C" int nqb_edge_embed_fwd_typed(int lmax, int num_bessel, double r_max, double poly_p, double prefactor,
+                                        const double* pos, const int64_t* edge_index, const double* shift,
+                                        const double* cell, int64_t N, int64_t E, const int64_t* types,
+                                        const int64_t* type_index, const double* recip, int T, int out_dtype,
+                                        double* vec, void* y, void* emb, nqb_stream_t st) {
+  (void)N;
+  if (lmax < 0 || lmax > 4) return fail("nqb_edge_embed_fwd_typed: lmax=%d unsupported (0..4)", lmax);
+  if (num_bessel < 1 || num_bessel > NQB_MAX_BESSEL) return fail("nqb_edge_embed_fwd_typed: bad num_bessel %d", num_bessel);
+  if (out_dtype != NQB_F32 && out_dtype != NQB_F64) return fail("nqb_edge_embed_fwd_typed: bad dtype");
+  if (!(r_max > 0.0) || !(poly_p >= 2.0)) return fail("nqb_edge_embed_fwd_typed: need r_max > 0 and p >= 2");
+  if (E < 0) return fail("nqb_edge_embed_fwd_typed: negative size");
+  if (E == 0) return 0;
+  if (!pos || !edge_index || !vec || !y || !emb) return fail("nqb_edge_embed_fwd_typed: null pointer");
+  if ((shift == nullptr) != (cell == nullptr)) return fail("nqb_edge_embed_fwd_typed: shift and cell must come together");
+  if (int rc = check_edge_types("nqb_edge_embed_fwd_typed", types, type_index, recip, T)) return rc;
+  EmbedParams prm{num_bessel, r_max, poly_p, prefactor};
+  const EdgeTypes et{types, type_index, recip, T};
+  unsigned blocks = (unsigned)((E + 127) / 128);
+  cudaStream_t s = (cudaStream_t)st;
+#define EE_FWD(L, TT) k_edge_embed_fwd<L, TT, true><<<blocks, 128, 0, s>>>(prm, pos, edge_index, shift, cell, E, vec, (TT*)y, (TT*)emb, et)
+  if (out_dtype == NQB_F32) {
+    switch (lmax) { case 0: EE_FWD(0, float); break; case 1: EE_FWD(1, float); break; case 2: EE_FWD(2, float); break; case 3: EE_FWD(3, float); break; default: EE_FWD(4, float); break; }
+  } else {
+    switch (lmax) { case 0: EE_FWD(0, double); break; case 1: EE_FWD(1, double); break; case 2: EE_FWD(2, double); break; case 3: EE_FWD(3, double); break; default: EE_FWD(4, double); break; }
+  }
+#undef EE_FWD
+  NQB_LAUNCH_CHECK("nqb_edge_embed_fwd_typed");
+  return 0;
+}
+
+extern "C" int nqb_edge_embed_bwd_typed(int lmax, int num_bessel, double r_max, double poly_p, double prefactor,
+                                        const double* vec, const int64_t* edge_index, int64_t N, int64_t E,
+                                        const int64_t* types, const int64_t* type_index, const double* recip, int T,
+                                        int out_dtype, const void* grad_y, const void* grad_emb, double* grad_pos,
+                                        double* grad_vec, nqb_stream_t st) {
+  (void)N;
+  if (lmax < 0 || lmax > 4) return fail("nqb_edge_embed_bwd_typed: lmax=%d unsupported (0..4)", lmax);
+  if (num_bessel < 1 || num_bessel > NQB_MAX_BESSEL) return fail("nqb_edge_embed_bwd_typed: bad num_bessel %d", num_bessel);
+  if (out_dtype != NQB_F32 && out_dtype != NQB_F64) return fail("nqb_edge_embed_bwd_typed: bad dtype");
+  if (E < 0) return fail("nqb_edge_embed_bwd_typed: negative size");
+  if (E == 0) return 0;
+  if (!vec) return fail("nqb_edge_embed_bwd_typed: null vec");
+  if (grad_pos && !edge_index) return fail("nqb_edge_embed_bwd_typed: grad_pos needs edge_index");
+  if (int rc = check_edge_types("nqb_edge_embed_bwd_typed", types, type_index, recip, T)) return rc;
+  EmbedParams prm{num_bessel, r_max, poly_p, prefactor};
+  const EdgeTypes et{types, type_index, recip, T};
+  unsigned blocks = (unsigned)((E + 127) / 128);
+  cudaStream_t s = (cudaStream_t)st;
+#define EE_BWD(L, TT) k_edge_embed_bwd<L, TT, true><<<blocks, 128, 0, s>>>(prm, vec, edge_index, E, (const TT*)grad_y, (const TT*)grad_emb, grad_pos, grad_vec, et)
+  if (out_dtype == NQB_F32) {
+    switch (lmax) { case 0: EE_BWD(0, float); break; case 1: EE_BWD(1, float); break; case 2: EE_BWD(2, float); break; case 3: EE_BWD(3, float); break; default: EE_BWD(4, float); break; }
+  } else {
+    switch (lmax) { case 0: EE_BWD(0, double); break; case 1: EE_BWD(1, double); break; case 2: EE_BWD(2, double); break; case 3: EE_BWD(3, double); break; default: EE_BWD(4, double); break; }
+  }
+#undef EE_BWD
+  NQB_LAUNCH_CHECK("nqb_edge_embed_bwd_typed");
   return 0;
 }
 

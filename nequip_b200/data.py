@@ -38,15 +38,42 @@ def jittered_lattice(n_side: int, density: float, jitter: float = 0.22, seed: in
     return pos, cell
 
 
-def neighbor_list(pos: np.ndarray, cell: Optional[np.ndarray], r_max: float, pbc: bool = True):
+def edge_type_rc2(atom_types, cutoffs, r_max: float) -> np.ndarray:
+    """[T, T] float64 ``rc * rc`` of a per-edge-type cutoff table ``cutoffs[source, target]`` (0 < rc <= r_max), after
+    checking the table and the types."""
+    rc = np.asarray(cutoffs.detach().cpu() if torch.is_tensor(cutoffs) else cutoffs, dtype=np.float64)
+    if rc.ndim != 2 or rc.shape[0] != rc.shape[1]:
+        raise ValueError(f"cutoffs must be a [T, T] table, got shape {rc.shape}")
+    if not (np.all(rc > 0) and np.all(rc <= r_max)):
+        raise ValueError(f"cutoffs: every entry must satisfy 0 < rc <= r_max = {r_max}")
+    t = np.asarray(atom_types).reshape(-1)
+    if t.size and (t.min() < 0 or t.max() >= rc.shape[0]):
+        raise ValueError(f"atom_types must lie in [0, {rc.shape[0]})")
+    return rc * rc
+
+
+def neighbor_list(pos: np.ndarray, cell: Optional[np.ndarray], r_max: float, pbc: bool = True, atom_types=None,
+                  cutoffs=None):
     """Full neighbour list within r_max.  Orthorhombic cells only.  Returns
-    (edge_index [2,E] int64, shifts [E,3] float64) sorted by (centre, neighbour)."""
+    (edge_index [2,E] int64, shifts [E,3] float64) sorted by (centre, neighbour).
+
+    Per-edge-type cutoffs (nequip/data/transforms/neighborlist.py:9-117): ``cutoffs`` [T, T] (``rc[source, target]``)
+    with ``atom_types`` [N] keeps the pair (i, j) when ``dist2 < rc[t_i, t_j]^2`` (``rc * rc`` in float64) instead of
+    ``dist2 < r_max^2``, in both paths below.  A table of r_max everywhere gives the list without it."""
     N = pos.shape[0]
+    thr = None  # [N, N] squared cutoff of each (centre, neighbour) pair, or None for r_max
+    if cutoffs is not None:
+        if atom_types is None:
+            raise ValueError("cutoffs need atom_types")
+        t = np.asarray(atom_types).reshape(-1).astype(np.int64)
+        if t.size != N:
+            raise ValueError(f"atom_types must hold {N} types")
+        thr = edge_type_rc2(t, cutoffs, r_max)[t[:, None], t[None, :]]
     if not isinstance(pbc, (bool, np.bool_)):  # per-direction flags (mixed boundary conditions, e.g. a slab)
         flags = [bool(b) for b in pbc]
         if cell is not None and any(flags) and not all(flags):
             assert np.allclose(cell, np.diag(np.diag(cell))), "orthorhombic cells only"
-            return _nl_bruteforce(pos, np.diag(cell).copy(), r_max, periodic=np.array(flags))
+            return _nl_bruteforce(pos, np.diag(cell).copy(), r_max, periodic=np.array(flags), thr=thr)
         pbc = all(flags)
     if cell is None or not pbc:
         L = None
@@ -54,7 +81,7 @@ def neighbor_list(pos: np.ndarray, cell: Optional[np.ndarray], r_max: float, pbc
         assert np.allclose(cell, np.diag(np.diag(cell))), "orthorhombic cells only"
         L = np.diag(cell).copy()
     if L is None or np.any(np.floor(L / r_max) < 3) or N < 64:
-        return _nl_bruteforce(pos, L, r_max)
+        return _nl_bruteforce(pos, L, r_max, thr=thr)
     nc = np.floor(L / r_max).astype(np.int64)
     frac = pos / L
     wrapped = frac - np.floor(frac)
@@ -85,8 +112,8 @@ def neighbor_list(pos: np.ndarray, cell: Optional[np.ndarray], r_max: float, pbc
         cj = np.where(valid, cand, 0)
         d = wpos[cj] + (img[:, :, None, :] * L) - wpos[sl][:, None, None, :]
         dist2 = (d * d).sum(-1)
-        ok = valid & (dist2 < r_max * r_max)
         ai = np.broadcast_to(np.arange(sl.start, sl.stop)[:, None, None], cand.shape)
+        ok = valid & (dist2 < (r_max * r_max if thr is None else thr[ai, cj]))
         ok &= ~((cj == ai) & (img == 0).all(-1)[:, :, None])
         i_sel = ai[ok]
         j_sel = cj[ok]
@@ -103,8 +130,10 @@ def neighbor_list(pos: np.ndarray, cell: Optional[np.ndarray], r_max: float, pbc
     return np.stack([ii[o], jj[o]]).astype(np.int64), sh[o]
 
 
-def _nl_bruteforce(pos, L, r_max, periodic=None):
-    """``periodic`` (optional bool[3]): directions without periodic images (their cell length is ignored)."""
+def _nl_bruteforce(pos, L, r_max, periodic=None, thr=None):
+    """``periodic`` (optional bool[3]): directions without periodic images (their cell length is ignored).
+    ``thr`` (optional [N, N]): squared cutoff of each (centre, neighbour) pair in place of r_max^2."""
+    r2 = r_max * r_max if thr is None else thr
     if L is not None and periodic is not None:
         per = np.asarray(periodic, dtype=bool)
         Lp = np.where(per, L, 1.0)
@@ -116,7 +145,7 @@ def _nl_bruteforce(pos, L, r_max, periodic=None):
         ii, jj, ss = [], [], []
         for s in shifts:
             d = w[None, :, :] + s * Lp - w[:, None, :]
-            ok = (d * d).sum(-1) < r_max * r_max
+            ok = (d * d).sum(-1) < r2
             if not np.any(s):
                 ok &= ~np.eye(pos.shape[0], dtype=bool)
             i, j = np.nonzero(ok)
@@ -133,7 +162,7 @@ def _nl_bruteforce(pos, L, r_max, periodic=None):
             # atoms outside the home cell (unwrapped trajectories, nequip/utils/unittests/model_tests_basic.py:326-383):
             # search among the wrapped images, then express the shifts for the positions as given --
             # pos[j] - pos[i] + shift * L is the same vector as for the wrapped atoms
-            ei, sh = _nl_bruteforce(pos - cells * L, L, r_max)
+            ei, sh = _nl_bruteforce(pos - cells * L, L, r_max, thr=thr)
             return ei, sh + cells[ei[0]] - cells[ei[1]]
     N = pos.shape[0]
     if L is None:
@@ -147,7 +176,7 @@ def _nl_bruteforce(pos, L, r_max, periodic=None):
         off = (s * L) if L is not None else 0.0
         d = pos[None, :, :] + off - pos[:, None, :]
         dist2 = (d * d).sum(-1)
-        ok = dist2 < r_max * r_max
+        ok = dist2 < r2
         if not np.any(s):
             ok &= ~np.eye(N, dtype=bool)
         i, j = np.nonzero(ok)

@@ -161,6 +161,9 @@ class GraphedMDStep(GraphedEnergyForces):
     ``capacity = ceil(1.02 * needed)`` and the same positions are computed again, so a returned result never comes
     from a truncated list; ``capacity`` only grows and ``recaptures`` counts the re-captures.
 
+    A model with per-edge-type cutoffs (``per_edge_type_cutoff``) gets a neighbour list pruned by its table: the
+    default capacity is sized from the pruned count, and the atom types of ``example`` are fixed for the graph.
+
     ``variable_cell=True`` (NPT): ``g(pos, cell)`` also takes the step's cell ([3,3], host or device; a device cell
     costs one device-to-host read).  It is copied into the static ``cell`` input the model reads and handed to the
     neighbour list (``ops.NeighborListPlan.set_cell``) before the replay.  The captured call is
@@ -174,7 +177,8 @@ class GraphedMDStep(GraphedEnergyForces):
         if example.get("cell") is None:
             raise ValueError("GraphedMDStep needs a periodic cell")
         if capacity is None:
-            e0 = int(ops.neighbor_list(example["pos"], example["cell"], True, model.r_max)["edge_index"].shape[1])
+            e0 = int(ops.neighbor_list(example["pos"], example["cell"], True, model.r_max,
+                                       **self._edge_type_args(model, example))["edge_index"].shape[1])
             capacity = e0 + math.ceil(CAPACITY_SLACK * e0)
         self.variable_cell = bool(variable_cell)
         self.recaptures = 0
@@ -183,10 +187,17 @@ class GraphedMDStep(GraphedEnergyForces):
         self._overflow_host = torch.zeros(1, dtype=torch.int32).pin_memory()
         self._capture(model, {k: example[k] for k in ("pos", "atom_types", "cell")}, int(capacity))
 
+    @staticmethod
+    def _edge_type_args(model, example: Dict[str, torch.Tensor]) -> dict:
+        """The neighbour list's per-edge-type cutoffs: the model's table and the frame's (static) atom types."""
+        table = getattr(model, "per_edge_type_cutoff", None)
+        return {} if table is None else dict(atom_types=example["atom_types"], edge_type_cutoff=table)
+
     def _capture(self, model, example: Dict[str, torch.Tensor], capacity: int) -> None:
         self.capacity = capacity
         self.plan = ops.NeighborListPlan(example["pos"].shape[0], example["cell"], True, model.r_max, capacity,
-                                         device=example["pos"].device, variable_cell=self.variable_cell)
+                                         device=example["pos"].device, variable_cell=self.variable_cell,
+                                         **self._edge_type_args(model, example))
         super().__init__(model, example, warmup=self._warmup)
         ops.src_csr_cache.clear()  # like csr_cache: an entry made during the capture lives in the graph's pool
         out, self._out = self._out, None

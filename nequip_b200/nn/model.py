@@ -529,6 +529,38 @@ NEQUIP_PRESETS: Dict[str, dict] = {
 NEQUIP_STANDARD_PRESET = dict(parity=False, type_embed_num_features=32, radial_mlp_depth=1, radial_mlp_width=128)
 
 
+def parse_per_edge_type_cutoff(spec: dict, type_names: Sequence[str], r_max: float) -> torch.Tensor:
+    """The reference's ``per_edge_type_cutoff`` (nn/embedding/utils.py:15-83) as a [T, T] float64 table
+    ``rc[source, target]``: ``spec`` maps a source type name to one cutoff (every target) or to a dict {target type
+    name: cutoff}; missing sources and targets get ``r_max``.  The table may be asymmetric.  Raises ``ValueError`` for
+    unknown type names, cutoffs outside 0 < rc <= r_max and any other nesting."""
+    names = list(type_names)
+    if not isinstance(spec, dict):
+        raise ValueError(f"per_edge_type_cutoff: expected a dict, got {type(spec).__name__}")
+
+    def value(v, where):
+        if isinstance(v, bool) or not isinstance(v, (int, float)):
+            raise ValueError(f"per_edge_type_cutoff[{where}]: expected a number, got {v!r}")
+        v = float(v)
+        if not 0.0 < v <= r_max:
+            raise ValueError(f"per_edge_type_cutoff[{where}] = {v}: must satisfy 0 < rc <= r_max = {r_max}")
+        return v
+
+    table = torch.full((len(names), len(names)), float(r_max), dtype=torch.float64)
+    for src, entry in spec.items():
+        if src not in names:
+            raise ValueError(f"per_edge_type_cutoff: unknown source type {src!r} (types: {names})")
+        a = names.index(src)
+        if isinstance(entry, dict):
+            for tgt, v in entry.items():
+                if tgt not in names:
+                    raise ValueError(f"per_edge_type_cutoff[{src!r}]: unknown target type {tgt!r} (types: {names})")
+                table[a, names.index(tgt)] = value(v, f"{src!r}][{tgt!r}")
+        else:
+            table[a, :] = value(entry, repr(src))
+    return table
+
+
 def preset_kwargs(name: str, **overrides) -> dict:
     """Constructor arguments of preset ``name`` (case-insensitive): standard preset < named preset < ``overrides``."""
     key = name.upper()
@@ -550,7 +582,7 @@ class NequIPEnergyModel(torch.nn.Module):
                  avg_num_neighbors: float = 1.0, per_type_energy_scales: Optional[Sequence[float]] = None,
                  per_type_energy_shifts: Optional[Sequence[float]] = None, model_dtype=torch.float32,
                  seed: int = 123, node_layout: str = "ir_mul", strict_fast_path: bool = False,
-                 pair_potential: Optional[dict] = None):
+                 pair_potential: Optional[dict] = None, per_edge_type_cutoff: Optional[dict] = None):
         """``num_features``: one width for every degree, or a list of l_max + 1 widths (one per degree, e.g.
         ``[128, 64, 32]`` = 128x0e + 64x1o + 32x2e for l_max = 2 without parity), as in nequip_models.py:164-190.
         ``type_embed_num_features``: width of the type embedding, which is also the first layer's input and the
@@ -559,9 +591,19 @@ class NequIPEnergyModel(torch.nn.Module):
         ``{"_target_": "nequip.nn.pair_potential.ZBL", "units": "metal", "chemical_species": ["C", "H", "O", "Cu"]}``
         (``_target_`` may be left out; optional ``polynomial_cutoff_p``, default 6, independent of the model's).  Its
         per-atom energies are added after the per-type scale and shift, before the sum (submodule ``pair_potential``).
+        ``per_edge_type_cutoff``: the reference's partial table of cutoffs per ordered type pair (source = centre
+        ``edge_index[0]``, target = neighbour), e.g. ``{"H": 2.0, "C": {"H": 4.0, "C": 3.5}}``; missing entries are
+        ``r_max``, every entry satisfies 0 < rc <= r_max (``parse_per_edge_type_cutoff``).  The edge embedding and the
+        ZBL envelope then take the normalised length ``r / rc[t_i, t_j]`` (the Bessel prefactor keeps ``r_max``), so an
+        edge at or beyond its pair's cutoff contributes exactly zero; the full table is ``self.per_edge_type_cutoff``
+        [T, T] f64, its reciprocal the buffer ``rmax_recip`` [T * T] f64 (the reference's ``edge_norm._rmax_recip``).
+        Neighbour lists built with the table (``ops.neighbor_list(..., atom_types=, edge_type_cutoff=)``) drop those
+        edges, and every per-edge cost shrinks with them.
         """
         super().__init__()
         pair_spec = parse_pair_potential(pair_potential, len(type_names))
+        cutoff_table = (None if per_edge_type_cutoff is None
+                        else parse_per_edge_type_cutoff(per_edge_type_cutoff, type_names, float(r_max)))
         widths = feature_widths(l_max, num_features)
         f_embed = int(type_embed_num_features) if type_embed_num_features is not None else widths[0]
         self.r_max, self.l_max, self.num_bessels, self.poly_p = float(r_max), l_max, num_bessels, float(polynomial_cutoff_p)
@@ -621,6 +663,11 @@ class NequIPEnergyModel(torch.nn.Module):
         if pair_spec is not None:
             self.pair_potential = ZBL(type_names, model_dtype=model_dtype, **pair_spec)
             self.config["pair_potential"] = dict(_target_=ZBL_TARGET, **pair_spec)
+        self.per_edge_type_cutoff: Optional[torch.Tensor] = cutoff_table
+        if cutoff_table is not None:
+            self.register_buffer("rmax_recip", cutoff_table.reciprocal().reshape(-1))
+            self.config["per_edge_type_cutoff"] = {k: (dict(v) if isinstance(v, dict) else v)
+                                                   for k, v in per_edge_type_cutoff.items()}
         self.set_strict_fast_path(strict_fast_path)
 
     @classmethod
@@ -645,6 +692,15 @@ class NequIPEnergyModel(torch.nn.Module):
         dst = edge_index[0]
         csr = ops.csr_cache.get(dst if dst.dtype == torch.int64 else dst.long().contiguous(), num_nodes)
         return ops.edge_pairs(edge_index, shift, edge_embedding, csr)
+
+    def _edge_type_kwargs(self, types) -> dict:
+        """Keyword arguments of the edge embedding for the per-edge-type cutoffs ({} without a table)."""
+        if self.per_edge_type_cutoff is None:
+            return {}
+        return dict(types=types, edge_type_recip=self.rmax_recip)
+
+    def _pair_kwargs(self) -> dict:
+        return {} if self.per_edge_type_cutoff is None else dict(edge_type_recip=self.rmax_recip)
 
     @staticmethod
     def _reduce_energy(e_atom: torch.Tensor, data: Dict[str, torch.Tensor]) -> torch.Tensor:
@@ -675,13 +731,18 @@ class NequIPEnergyModel(torch.nn.Module):
         sink = data.get("_edge_grad_sink")
         if EDGE_VECTORS_KEY in data:
             # the caller (LAMMPS ML-IAP) supplies the edge vectors: with_edge_vectors_ keeps them (nn/utils.py:68-118)
+            # the types of an edge come from the real edge_index (the kernel's own index list names made-up positions)
+            et = self._edge_type_kwargs(types)
+            if et:
+                et["edge_index"] = edge_index
             edge_attrs, edge_embedding = ops.edge_embed_from_vectors(
                 data[EDGE_VECTORS_KEY], lmax=self.l_max, num_bessel=self.num_bessels, r_max=self.r_max,
-                poly_p=self.poly_p, prefactor=pre, out_dtype=self.model_dtype)
+                poly_p=self.poly_p, prefactor=pre, out_dtype=self.model_dtype, **et)
         else:
             _vec, edge_attrs, edge_embedding = ops.edge_embed(
                 pos, edge_index, shift, cell, lmax=self.l_max, num_bessel=self.num_bessels, r_max=self.r_max,
-                poly_p=self.poly_p, prefactor=pre, out_dtype=self.model_dtype, edge_grad_sink=sink)
+                poly_p=self.poly_p, prefactor=pre, out_dtype=self.model_dtype, edge_grad_sink=sink,
+                **self._edge_type_kwargs(types))
         pairs = self._edge_pairs(edge_index, None if EDGE_VECTORS_KEY in data else shift, edge_embedding, types.numel())
         for layer in self.layers:
             x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight, pairs=pairs)
@@ -692,10 +753,11 @@ class NequIPEnergyModel(torch.nn.Module):
             e_atom = e_atom + self.shifts[types]
         if self.pair_potential is not None:
             if EDGE_VECTORS_KEY in data:
-                e_pair = self.pair_potential(types, edge_index, self.r_max, edge_vectors=data[EDGE_VECTORS_KEY])
+                e_pair = self.pair_potential(types, edge_index, self.r_max, edge_vectors=data[EDGE_VECTORS_KEY],
+                                             **self._pair_kwargs())
             else:
                 e_pair = self.pair_potential(types, edge_index, self.r_max, pos=pos, shift=shift, cell=cell,
-                                             edge_grad_sink=sink)
+                                             edge_grad_sink=sink, **self._pair_kwargs())
             e_atom = e_atom + e_pair
         data[PER_ATOM_ENERGY_KEY] = e_atom
         data[TOTAL_ENERGY_KEY] = self._reduce_energy(e_atom, data)
@@ -713,7 +775,8 @@ class NequIPEnergyModel(torch.nn.Module):
             shift = None
         _vec, edge_attrs, edge_embedding = ops.edge_embed(
             pos, edge_index, shift, cell, lmax=self.l_max, num_bessel=self.num_bessels, r_max=self.r_max,
-            poly_p=self.poly_p, prefactor=(2 * math.pi) / (self.r_max * self.r_max), out_dtype=self.model_dtype)
+            poly_p=self.poly_p, prefactor=(2 * math.pi) / (self.r_max * self.r_max), out_dtype=self.model_dtype,
+            **self._edge_type_kwargs(types))
         pairs = self._edge_pairs(edge_index, shift, edge_embedding, types.numel())
         for layer in self.layers:
             x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight, n_own, halo,
@@ -726,7 +789,8 @@ class NequIPEnergyModel(torch.nn.Module):
             e_atom = e_atom + self.shifts[t_own]
         if self.pair_potential is not None:
             # every edge's centre is owned: the owned rows are complete, the ghost rows (no edges) are 0
-            e_atom = e_atom + self.pair_potential(types, edge_index, self.r_max, pos=pos, shift=shift, cell=cell)[:n_own]
+            e_atom = e_atom + self.pair_potential(types, edge_index, self.r_max, pos=pos, shift=shift, cell=cell,
+                                                  **self._pair_kwargs())[:n_own]
         return e_atom
 
     def forward(self, data: Dict[str, torch.Tensor], compute_forces: bool = True,

@@ -92,12 +92,13 @@ class ZBL(torch.nn.Module):
         return self._table[1]
 
     def forward(self, types, edge_index, r_max: float, pos=None, shift=None, cell=None, edge_vectors=None,
-                edge_grad_sink=None) -> torch.Tensor:
-        """Per-atom ZBL energies [N, 1] f64 (N = number of atom types given)."""
+                edge_grad_sink=None, **edge_type) -> torch.Tensor:
+        """Per-atom ZBL energies [N, 1] f64 (N = number of atom types given).  ``edge_type_recip=`` [T * T]: the
+        model's per-edge-type cutoffs (``ops.zbl_energy``)."""
         dev = types.device
         return ops.zbl_energy(pos, edge_index, types, self.table(dev), shift=shift, cell=cell,
                               edge_vectors=edge_vectors, r_max=r_max, poly_p=self.poly_p,
-                              cutoff_dtype=self.model_dtype, edge_grad_sink=edge_grad_sink)
+                              cutoff_dtype=self.model_dtype, edge_grad_sink=edge_grad_sink, **edge_type)
 
     def extra_repr(self) -> str:
         return f"units={self.units}, chemical_species={self.chemical_species}, polynomial_cutoff_p={self.poly_p}"

@@ -455,28 +455,38 @@ def spherical_harmonics(vec: torch.Tensor, lmax: int, out_dtype=torch.float32) -
 
 class _EdgeEmbedFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, pos, edge_index, shift, cell, lmax, num_bessel, r_max, poly_p, prefactor, out_dtype, sink=None):
+    def forward(ctx, pos, edge_index, shift, cell, lmax, num_bessel, r_max, poly_p, prefactor, out_dtype, sink=None,
+                types=None, recip=None):
         L = _capi.lib()
         N, E = pos.shape[0], edge_index.shape[1]
         dev = pos.device
         vec = torch.empty((E, 3), dtype=torch.float64, device=dev)
         y = torch.empty((E, (lmax + 1) ** 2), dtype=out_dtype, device=dev)
         emb = torch.empty((E, num_bessel), dtype=out_dtype, device=dev)
-        _capi.check(
-            L.nqb_edge_embed_fwd(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(pos), _ptr(edge_index), _ptr(shift),
-                                 _ptr(cell), N, E, _DT[out_dtype], _ptr(vec), _ptr(y), _ptr(emb), _stream()),
-            "nqb_edge_embed_fwd",
-        )
+        if recip is None:
+            _capi.check(
+                L.nqb_edge_embed_fwd(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(pos), _ptr(edge_index), _ptr(shift),
+                                     _ptr(cell), N, E, _DT[out_dtype], _ptr(vec), _ptr(y), _ptr(emb), _stream()),
+                "nqb_edge_embed_fwd",
+            )
+        else:
+            _capi.check(
+                L.nqb_edge_embed_fwd_typed(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(pos), _ptr(edge_index),
+                                           _ptr(shift), _ptr(cell), N, E, _ptr(types), _ptr(edge_index), _ptr(recip),
+                                           _edge_type_count(recip), _DT[out_dtype], _ptr(vec), _ptr(y), _ptr(emb),
+                                           _stream()),
+                "nqb_edge_embed_fwd_typed",
+            )
         ctx.args = (lmax, num_bessel, r_max, poly_p, prefactor, out_dtype, N)
         ctx.sink = sink
-        ctx.save_for_backward(vec, edge_index)
+        ctx.save_for_backward(vec, edge_index, types, recip)
         ctx.mark_non_differentiable(vec)
         return vec, y, emb
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, _gvec, gy, gemb):
-        vec, edge_index = ctx.saved_tensors
+        vec, edge_index, types, recip = ctx.saved_tensors
         lmax, num_bessel, r_max, poly_p, prefactor, out_dtype, N = ctx.args
         L = _capi.lib()
         E = vec.shape[0]
@@ -486,14 +496,22 @@ class _EdgeEmbedFn(torch.autograd.Function):
         # the per-edge gradient dE/d(edge vector) is what the virial is made of (sum_e r_e (x) g_e): keep it
         # when the caller asked for it
         gvec = torch.empty_like(vec) if ctx.sink is not None else None
-        _capi.check(
-            L.nqb_edge_embed_bwd(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(vec), _ptr(edge_index), N, E,
-                                 _DT[out_dtype], _ptr(gy), _ptr(gemb), _ptr(gpos), _ptr(gvec), _stream()),
-            "nqb_edge_embed_bwd",
-        )
+        if recip is None:
+            _capi.check(
+                L.nqb_edge_embed_bwd(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(vec), _ptr(edge_index), N, E,
+                                     _DT[out_dtype], _ptr(gy), _ptr(gemb), _ptr(gpos), _ptr(gvec), _stream()),
+                "nqb_edge_embed_bwd",
+            )
+        else:
+            _capi.check(
+                L.nqb_edge_embed_bwd_typed(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(vec), _ptr(edge_index), N, E,
+                                           _ptr(types), _ptr(edge_index), _ptr(recip), _edge_type_count(recip),
+                                           _DT[out_dtype], _ptr(gy), _ptr(gemb), _ptr(gpos), _ptr(gvec), _stream()),
+                "nqb_edge_embed_bwd_typed",
+            )
         if ctx.sink is not None:
             ctx.sink["edge_vectors"], ctx.sink["edge_vector_grad"] = vec, gvec
-        return gpos, None, None, None, None, None, None, None, None, None, None
+        return gpos, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 class _EdgeEmbedVecFn(torch.autograd.Function):
@@ -501,7 +519,8 @@ class _EdgeEmbedVecFn(torch.autograd.Function):
     nequip/nn/grad_output.py:270-296); backward = dE/d(edge vectors)."""
 
     @staticmethod
-    def forward(ctx, vec, lmax, num_bessel, r_max, poly_p, prefactor, out_dtype):
+    def forward(ctx, vec, lmax, num_bessel, r_max, poly_p, prefactor, out_dtype, types=None, type_index=None,
+                recip=None):
         L = _capi.lib()
         E = vec.shape[0]
         dev = vec.device
@@ -512,48 +531,101 @@ class _EdgeEmbedVecFn(torch.autograd.Function):
         vec_out = torch.empty((E, 3), dtype=torch.float64, device=dev)
         y = torch.empty((E, (lmax + 1) ** 2), dtype=out_dtype, device=dev)
         emb = torch.empty((E, num_bessel), dtype=out_dtype, device=dev)
-        _capi.check(
-            L.nqb_edge_embed_fwd(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(pos), _ptr(edge_index), 0, 0, E + 1, E,
-                                 _DT[out_dtype], _ptr(vec_out), _ptr(y), _ptr(emb), _stream()),
-            "nqb_edge_embed_fwd",
-        )
+        if recip is None:
+            _capi.check(
+                L.nqb_edge_embed_fwd(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(pos), _ptr(edge_index), 0, 0, E + 1,
+                                     E, _DT[out_dtype], _ptr(vec_out), _ptr(y), _ptr(emb), _stream()),
+                "nqb_edge_embed_fwd",
+            )
+        else:
+            # the types come from the real edge list, not from the made-up positions' index list
+            _capi.check(
+                L.nqb_edge_embed_fwd_typed(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(pos), _ptr(edge_index), 0, 0,
+                                           E + 1, E, _ptr(types), _ptr(type_index), _ptr(recip), _edge_type_count(recip),
+                                           _DT[out_dtype], _ptr(vec_out), _ptr(y), _ptr(emb), _stream()),
+                "nqb_edge_embed_fwd_typed",
+            )
         ctx.args = (lmax, num_bessel, r_max, poly_p, prefactor, out_dtype)
-        ctx.save_for_backward(vec_out, edge_index)
+        ctx.save_for_backward(vec_out, edge_index, types, type_index, recip)
         return y, emb
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, gy, gemb):
-        vec, edge_index = ctx.saved_tensors
+        vec, edge_index, types, type_index, recip = ctx.saved_tensors
         lmax, num_bessel, r_max, poly_p, prefactor, out_dtype = ctx.args
         E = vec.shape[0]
         gvec = torch.empty_like(vec)
         gy = None if gy is None else gy.to(out_dtype).contiguous()
         gemb = None if gemb is None else gemb.to(out_dtype).contiguous()
-        _capi.check(
-            _capi.lib().nqb_edge_embed_bwd(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(vec), _ptr(edge_index), E + 1, E,
-                                           _DT[out_dtype], _ptr(gy), _ptr(gemb), 0, _ptr(gvec), _stream()),
-            "nqb_edge_embed_bwd",
-        )
-        return gvec, None, None, None, None, None, None
+        if recip is None:
+            _capi.check(
+                _capi.lib().nqb_edge_embed_bwd(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(vec), _ptr(edge_index),
+                                               E + 1, E, _DT[out_dtype], _ptr(gy), _ptr(gemb), 0, _ptr(gvec), _stream()),
+                "nqb_edge_embed_bwd",
+            )
+        else:
+            _capi.check(
+                _capi.lib().nqb_edge_embed_bwd_typed(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(vec),
+                                                     _ptr(edge_index), E + 1, E, _ptr(types), _ptr(type_index),
+                                                     _ptr(recip), _edge_type_count(recip), _DT[out_dtype], _ptr(gy),
+                                                     _ptr(gemb), 0, _ptr(gvec), _stream()),
+                "nqb_edge_embed_bwd_typed",
+            )
+        return gvec, None, None, None, None, None, None, None, None, None
+
+
+def _edge_type_count(recip: torch.Tensor) -> int:
+    """T of a [T * T] reciprocal-cutoff table."""
+    T = int(round(recip.numel() ** 0.5))
+    if T < 1 or T * T != recip.numel():
+        raise ValueError(f"edge_type_recip must hold T * T values, got {recip.numel()}")
+    return T
+
+
+def _edge_type_args(types, edge_type_recip, what: str):
+    """(types, recip) checked and laid out for the ``_typed`` kernels, or (None, None) without a table."""
+    if (types is None) != (edge_type_recip is None):
+        raise ValueError(f"{what}: types and edge_type_recip must be given together")
+    if edge_type_recip is None:
+        return None, None
+    _require_cuda(types, edge_type_recip)
+    recip = edge_type_recip.to(torch.float64).reshape(-1).contiguous()
+    _edge_type_count(recip)
+    return types.view(-1).long().contiguous(), recip
 
 
 def edge_embed_from_vectors(vec, *, lmax: int, num_bessel: int = 8, r_max: float, poly_p: float = 6.0,
-                            prefactor: float = 1.0, out_dtype=torch.float32):
+                            prefactor: float = 1.0, out_dtype=torch.float32, types=None, edge_index=None,
+                            edge_type_recip=None):
     """``(edge_attrs [E,(lmax+1)^2], edge_embedding [E,num_bessel])`` of given ``[E,3]`` edge vectors,
-    differentiable w.r.t. the vectors."""
+    differentiable w.r.t. the vectors.
+
+    Per-edge-type cutoffs: ``edge_type_recip`` [T * T] f64 holds ``1 / rc[source, target]`` and the normalised length
+    of edge e is ``|vec_e| * edge_type_recip[T * types[edge_index[0, e]] + types[edge_index[1, e]]]``; ``types`` [N]
+    and the edge list ``edge_index`` [2, E] the vectors belong to must come with it."""
     _require_cuda(vec)
+    types, recip = _edge_type_args(types, edge_type_recip, "edge_embed_from_vectors")
+    if recip is not None:
+        if edge_index is None or tuple(edge_index.shape) != (2, vec.shape[0]):
+            raise ValueError(f"edge_embed_from_vectors: edge_type_recip needs edge_index [2, {vec.shape[0]}]")
+        _require_cuda(edge_index)
+        edge_index = edge_index.long().contiguous()
     return _EdgeEmbedVecFn.apply(vec.double().contiguous(), int(lmax), int(num_bessel), float(r_max), float(poly_p),
-                                 float(prefactor), out_dtype)
+                                 float(prefactor), out_dtype, types, None if recip is None else edge_index, recip)
 
 
 def edge_embed(pos, edge_index, shift=None, cell=None, *, lmax: int, num_bessel: int = 8, r_max: float,
-               poly_p: float = 6.0, prefactor: float = 1.0, out_dtype=torch.float32, edge_grad_sink=None):
+               poly_p: float = 6.0, prefactor: float = 1.0, out_dtype=torch.float32, edge_grad_sink=None,
+               types=None, edge_type_recip=None):
     """Edge vectors, harmonics and Bessel x cutoff embedding in one kernel.
 
     Returns ``(edge_vectors [E,3] f64, edge_attrs [E,(lmax+1)^2], edge_embedding [E,num_bessel])``.
     Differentiable w.r.t. ``pos`` (forces).  ``edge_grad_sink`` (a dict): the backward pass also stores the
-    edge vectors and dE/d(edge vector) in it, from which the virial / cell gradient follows."""
+    edge vectors and dE/d(edge vector) in it, from which the virial / cell gradient follows.
+    ``types`` [N] + ``edge_type_recip`` [T * T] f64: per-edge-type cutoffs, the normalised length of edge e is
+    ``r_e * edge_type_recip[T * types[edge_index[0, e]] + types[edge_index[1, e]]]`` instead of ``r_e / r_max``
+    (``prefactor`` is the caller's)."""
     _require_cuda(pos, edge_index)
     pos = pos.double().contiguous()
     edge_index = edge_index.long().contiguous()
@@ -562,8 +634,12 @@ def edge_embed(pos, edge_index, shift=None, cell=None, *, lmax: int, num_bessel:
     if shift is not None:
         shift = shift.double().contiguous()
         cell = cell.double().reshape(3, 3).contiguous()
+    types, recip = _edge_type_args(types, edge_type_recip, "edge_embed")
+    if recip is None:
+        return _EdgeEmbedFn.apply(pos, edge_index, shift, cell, int(lmax), int(num_bessel), float(r_max),
+                                  float(poly_p), float(prefactor), out_dtype, edge_grad_sink)
     return _EdgeEmbedFn.apply(pos, edge_index, shift, cell, int(lmax), int(num_bessel), float(r_max),
-                              float(poly_p), float(prefactor), out_dtype, edge_grad_sink)
+                              float(poly_p), float(prefactor), out_dtype, edge_grad_sink, types, recip)
 
 
 # ---------------------------------------------------------------------------------------
@@ -571,26 +647,35 @@ def edge_embed(pos, edge_index, shift=None, cell=None, *, lmax: int, num_bessel:
 # ---------------------------------------------------------------------------------------
 class _ZBLFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, geom, edge_index, shift, cell, types, table, r_max, poly_p, cutoff_f32, from_vectors, sink):
+    def forward(ctx, geom, edge_index, shift, cell, types, table, r_max, poly_p, cutoff_f32, from_vectors, sink,
+                recip=None):
         N, E, T = types.numel(), edge_index.shape[1], table.shape[0]
         csr = csr_cache.get(edge_index[0], N)  # the CSR the first interaction layer already built
         pos, vec = (None, geom) if from_vectors else (geom, None)
         e_atom = torch.empty((N, 1), dtype=torch.float64, device=types.device)
-        _capi.check(
-            _capi.lib().nqb_zbl_fwd(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(vec), _ptr(types),
-                                    _ptr(table), T, _ptr(csr.row_ptr), _ptr(csr.perm), N, E, r_max, poly_p,
-                                    int(cutoff_f32), _ptr(e_atom), _stream()),
-            "nqb_zbl_fwd",
-        )
+        if recip is None:
+            _capi.check(
+                _capi.lib().nqb_zbl_fwd(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(vec), _ptr(types),
+                                        _ptr(table), T, _ptr(csr.row_ptr), _ptr(csr.perm), N, E, r_max, poly_p,
+                                        int(cutoff_f32), _ptr(e_atom), _stream()),
+                "nqb_zbl_fwd",
+            )
+        else:
+            _capi.check(
+                _capi.lib().nqb_zbl_fwd_typed(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(vec),
+                                              _ptr(types), _ptr(table), T, _ptr(csr.row_ptr), _ptr(csr.perm), N, E,
+                                              r_max, poly_p, int(cutoff_f32), _ptr(recip), _ptr(e_atom), _stream()),
+                "nqb_zbl_fwd_typed",
+            )
         ctx.args = (r_max, poly_p, cutoff_f32, from_vectors)
         ctx.sink = sink
-        ctx.save_for_backward(geom, edge_index, shift, cell, types, table)
+        ctx.save_for_backward(geom, edge_index, shift, cell, types, table, recip)
         return e_atom
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, ge):
-        geom, edge_index, shift, cell, types, table = ctx.saved_tensors
+        geom, edge_index, shift, cell, types, table, recip = ctx.saved_tensors
         r_max, poly_p, cutoff_f32, from_vectors = ctx.args
         N, E = types.numel(), edge_index.shape[1]
         pos, vec = (None, geom) if from_vectors else (geom, None)
@@ -598,27 +683,37 @@ class _ZBLFn(torch.autograd.Function):
         gvec = torch.empty((E, 3), dtype=torch.float64, device=geom.device) \
             if from_vectors or ctx.sink is not None else None
         ge = ge.to(torch.float64).contiguous()
-        _capi.check(
-            _capi.lib().nqb_zbl_bwd(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(vec), _ptr(types),
-                                    _ptr(table), table.shape[0], N, E, r_max, poly_p, int(cutoff_f32), _ptr(ge),
-                                    _ptr(gpos), _ptr(gvec), _stream()),
-            "nqb_zbl_bwd",
-        )
+        if recip is None:
+            _capi.check(
+                _capi.lib().nqb_zbl_bwd(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(vec), _ptr(types),
+                                        _ptr(table), table.shape[0], N, E, r_max, poly_p, int(cutoff_f32), _ptr(ge),
+                                        _ptr(gpos), _ptr(gvec), _stream()),
+                "nqb_zbl_bwd",
+            )
+        else:
+            _capi.check(
+                _capi.lib().nqb_zbl_bwd_typed(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(vec),
+                                              _ptr(types), _ptr(table), table.shape[0], N, E, r_max, poly_p,
+                                              int(cutoff_f32), _ptr(recip), _ptr(ge), _ptr(gpos), _ptr(gvec), _stream()),
+                "nqb_zbl_bwd_typed",
+            )
         if ctx.sink is not None:
             # kept apart from the edge embedding's gradient: the stress assembly adds the two once both backwards ran
             ctx.sink["pair_edge_vector_grad"] = gvec
-        return (gvec if from_vectors else gpos), None, None, None, None, None, None, None, None, None, None
+        return (gvec if from_vectors else gpos), None, None, None, None, None, None, None, None, None, None, None
 
 
 def zbl_energy(pos, edge_index, types, table, *, shift=None, cell=None, edge_vectors=None, r_max: float,
-               poly_p: float = 6.0, cutoff_dtype=torch.float64, edge_grad_sink=None):
+               poly_p: float = 6.0, cutoff_dtype=torch.float64, edge_grad_sink=None, edge_type_recip=None):
     """ZBL per-atom energies ``[N, 1]`` f64 (``N = types.numel()``), summed onto the centre ``edge_index[0]``.
 
     ``table`` [T, T, 2] f64 holds ``0.5 * qqr2e * Z_i Z_j`` and ``Z_i^0.23 + Z_j^0.23`` per ordered type pair
     (``nn.pair.ZBL.table``).  The geometry comes from ``pos`` (+ ``shift``/``cell``) or, with ``pos=None``, from the
     given ``edge_vectors`` [E, 3] (the ML-IAP branch); the result is differentiable w.r.t. whichever was given.
     ``cutoff_dtype=torch.float32`` rounds the cutoff as a float32 model does.  ``edge_grad_sink`` (a dict): the backward
-    pass also stores dE/d(edge vector) in it under ``pair_edge_vector_grad``."""
+    pass also stores dE/d(edge vector) in it under ``pair_edge_vector_grad``.  ``edge_type_recip`` [T * T] f64
+    (``1 / rc[source, target]``): per-edge-type cutoffs, the envelope takes ``r * edge_type_recip[T * t_i + t_j]``
+    instead of ``r / r_max``."""
     _require_cuda(edge_index, types, table)
     edge_index = edge_index.long().contiguous()
     types = types.view(-1).long().contiguous()
@@ -644,8 +739,15 @@ def zbl_energy(pos, edge_index, types, table, *, shift=None, cell=None, edge_vec
         if shift is not None:
             shift = shift.double().contiguous()
             cell = cell.double().reshape(3, 3).contiguous()
+    if edge_type_recip is None:
+        return _ZBLFn.apply(geom, edge_index, shift, cell, types, table, float(r_max), float(poly_p),
+                            cutoff_dtype == torch.float32, from_vectors, edge_grad_sink)
+    _require_cuda(edge_type_recip)
+    recip = edge_type_recip.to(torch.float64).reshape(-1).contiguous()
+    if recip.numel() != table.shape[0] * table.shape[0]:
+        raise ValueError(f"zbl_energy: edge_type_recip must hold T * T = {table.shape[0] ** 2} values")
     return _ZBLFn.apply(geom, edge_index, shift, cell, types, table, float(r_max), float(poly_p),
-                        cutoff_dtype == torch.float32, from_vectors, edge_grad_sink)
+                        cutoff_dtype == torch.float32, from_vectors, edge_grad_sink, recip)
 
 
 # ---------------------------------------------------------------------------------------
@@ -1010,11 +1112,38 @@ def _nl_scratch(N: int, nbins: int, dev) -> Dict[str, torch.Tensor]:
     }
 
 
+class _NlTypes:
+    """Per-edge-type cutoffs of the device list: atom types [N] and ``rc2 = rc * rc`` [T * T] (float64, computed on
+    the host) on the device; the pair (i, j) is a neighbour when ``d2 < rc2[T * types[i] + types[j]]``."""
+
+    def __init__(self, atom_types, edge_type_cutoff, r_max: float, num_atoms: int, device):
+        import numpy as np
+
+        rc = (edge_type_cutoff.detach().cpu().double().numpy() if torch.is_tensor(edge_type_cutoff)
+              else np.asarray(edge_type_cutoff, dtype=np.float64))
+        if rc.ndim != 2 or rc.shape[0] != rc.shape[1] or rc.shape[0] < 1:
+            raise ValueError(f"edge_type_cutoff must be a [T, T] table, got shape {tuple(rc.shape)}")
+        if not (np.all(rc > 0) and np.all(rc <= r_max)):
+            raise ValueError(f"edge_type_cutoff: every entry must satisfy 0 < rc <= r_max = {r_max}")
+        if atom_types is None:
+            raise ValueError("edge_type_cutoff needs atom_types")
+        types = torch.as_tensor(atom_types).view(-1)
+        if types.numel() != num_atoms:
+            raise ValueError(f"atom_types must hold {num_atoms} types, got {types.numel()}")
+        T = rc.shape[0]
+        if num_atoms and (int(types.min()) < 0 or int(types.max()) >= T):
+            raise ValueError(f"atom_types must lie in [0, {T})")
+        self.T = T
+        # a copy the list owns: a captured graph keeps its pointer
+        self.types = types.to(device=device, dtype=torch.int64).contiguous().clone()
+        self.rc2 = torch.from_numpy((rc * rc).reshape(-1)).to(device)
+
+
 def _nl_rows(pos: torch.Tensor, a: _NlArgs, s: Dict[str, torch.Tensor],
-             params_dev: Optional[torch.Tensor] = None) -> None:
+             params_dev: Optional[torch.Tensor] = None, ty: Optional[_NlTypes] = None) -> None:
     """Bins, atoms sorted by bin, neighbours per atom and their exclusive scan into ``s["row_ptr"]``; all on the
     device, no host synchronisation.  ``params_dev``: read the cell-dependent arguments from this device parameter
-    block (``nqb_nl_params_pack``) instead of passing ``a``'s by value."""
+    block (``nqb_nl_params_pack``) instead of passing ``a``'s by value.  ``ty``: per-edge-type cutoffs."""
     L = _capi.lib()
     N = pos.shape[0]
     st = _stream()
@@ -1026,7 +1155,15 @@ def _nl_rows(pos: torch.Tensor, a: _NlArgs, s: Dict[str, torch.Tensor],
                                     _ptr(s["cidx"]), st), "nqb_nl_bin_dp")
     torch.sort(s["binid"], stable=True, out=(s["sorted_bin"], s["order"]))
     torch.searchsorted(s["sorted_bin"], s["bins"], out=s["bin_start"])
-    if params_dev is None:
+    if ty is not None and params_dev is None:
+        _capi.check(L.nqb_nl_count_typed(N, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, _ptr(s["wpos"]), _ptr(s["cidx"]),
+                                         _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(ty.types), _ptr(ty.rc2), ty.T,
+                                         _ptr(s["counts"]), st), "nqb_nl_count_typed")
+    elif ty is not None:
+        _capi.check(L.nqb_nl_count_dp_typed(N, _ptr(params_dev), _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["order"]),
+                                            _ptr(s["bin_start"]), _ptr(ty.types), _ptr(ty.rc2), ty.T, _ptr(s["counts"]),
+                                            st), "nqb_nl_count_dp_typed")
+    elif params_dev is None:
         _capi.check(L.nqb_nl_count(N, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, _ptr(s["wpos"]), _ptr(s["cidx"]),
                                    _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(s["counts"]), st), "nqb_nl_count")
     else:
@@ -1035,7 +1172,8 @@ def _nl_rows(pos: torch.Tensor, a: _NlArgs, s: Dict[str, torch.Tensor],
     torch.cumsum(s["counts"], 0, out=s["row_ptr"][1:])
 
 
-def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, transpose_perm: bool = False):
+def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, transpose_perm: bool = False,
+                  atom_types=None, edge_type_cutoff=None):
     """Full neighbour list within ``r_max`` built on the GPU (cell list), in the layout the convolution wants.
 
     ``pos`` [N,3] float64 CUDA; ``cell`` [3,3] (rows = lattice vectors; host or device) or None; ``pbc`` bool or 3
@@ -1044,7 +1182,10 @@ def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, tr
     [N+1] int64 (destination CSR: edges are sorted by (centre, neighbour)) and, on request,
     ``edge_transpose_perm`` [E] (argsort by (neighbour, centre), nequip/data/transforms/neighborlist.py:150-155).
     Same contract as the reference's host backends (nequip/data/_nl.py:60-152): both directions, no self edge in
-    the home image.  One host synchronisation (the edge count); ``NeighborListPlan`` has none."""
+    the home image.  One host synchronisation (the edge count); ``NeighborListPlan`` has none.
+
+    Per-edge-type cutoffs: ``edge_type_cutoff`` [T, T] (``rc[source, target]``, 0 < rc <= r_max) with ``atom_types``
+    [N] keeps the pair (i, j) when ``d2 < rc[t_i, t_j]^2`` (``rc * rc`` in float64); the bins are those of ``r_max``."""
     import numpy as np
 
     _require_cuda(pos)
@@ -1062,15 +1203,29 @@ def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, tr
             if not pbc[d]:
                 lo[d], width[d] = fmin[d], max(fmax[d] - fmin[d], 1e-9) * (1 + 1e-9)
     a = _NlArgs(N, cell_np, inv_np, pbc, r_max, lo, width)
+    ty = None
+    if edge_type_cutoff is not None:
+        ty = _NlTypes(atom_types, edge_type_cutoff, float(r_max), N, dev)
+    elif atom_types is not None:
+        raise ValueError("atom_types is only read with edge_type_cutoff")
     s = _nl_scratch(N, a.nbins, dev)
-    _nl_rows(pos, a, s)
+    if ty is None:
+        _nl_rows(pos, a, s)
+    else:
+        _nl_rows(pos, a, s, ty=ty)
     row_ptr = s["row_ptr"]
     E = int(row_ptr[-1].item())
     edge_index = torch.empty((2, E), dtype=torch.int64, device=dev)
     shifts = torch.empty((E, 3), dtype=torch.float64, device=dev)
-    _capi.check(L.nqb_nl_fill(N, E, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, _ptr(s["wpos"]), _ptr(s["cidx"]),
-                              _ptr(s["base"]), _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(row_ptr), _ptr(edge_index),
-                              _ptr(shifts), _stream()), "nqb_nl_fill")
+    if ty is None:
+        _capi.check(L.nqb_nl_fill(N, E, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, _ptr(s["wpos"]), _ptr(s["cidx"]),
+                                  _ptr(s["base"]), _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(row_ptr),
+                                  _ptr(edge_index), _ptr(shifts), _stream()), "nqb_nl_fill")
+    else:
+        _capi.check(L.nqb_nl_fill_typed(N, E, a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, _ptr(s["wpos"]),
+                                        _ptr(s["cidx"]), _ptr(s["base"]), _ptr(s["order"]), _ptr(s["bin_start"]),
+                                        _ptr(row_ptr), _ptr(ty.types), _ptr(ty.rc2), ty.T, _ptr(edge_index),
+                                        _ptr(shifts), _stream()), "nqb_nl_fill_typed")
     out = {"edge_index": edge_index, "edge_cell_shift": shifts, "row_ptr": row_ptr}
     if transpose_perm:
         out["edge_transpose_perm"] = torch.argsort(edge_index[1] * N + edge_index[0], stable=True)
@@ -1137,10 +1292,14 @@ class NeighborListPlan:
     padded destination CSR), ``num_edges`` [1] int64 (the true edge count E) and ``overflow`` [1] int32, all on the
     device and all overwritten by the next ``run``.  Row i holds its real edges in the order of ``neighbor_list``,
     then null edges (i, i, ``pad_shift``); each row gets floor or ceil of (capacity - E) / N of them.  When
-    E > capacity, ``overflow`` is 1 and every row holds only null edges: the list must not be used."""
+    E > capacity, ``overflow`` is 1 and every row holds only null edges: the list must not be used.
+
+    ``atom_types`` [N] + ``edge_type_cutoff`` [T, T]: per-edge-type cutoffs as in ``neighbor_list``.  The types are
+    fixed for the plan's lifetime (the plan keeps a device copy whose pointer captured graphs hold); the cutoff table
+    does not depend on the cell, so ``set_cell`` leaves it alone."""
 
     def __init__(self, num_atoms: int, cell, pbc, r_max: float, capacity: int, device=None,
-                 variable_cell: bool = False):
+                 variable_cell: bool = False, atom_types=None, edge_type_cutoff=None):
         import numpy as np
 
         if cell is None:
@@ -1161,6 +1320,11 @@ class NeighborListPlan:
             cell.device if torch.is_tensor(cell) and cell.is_cuda else torch.device("cuda"))
         self.device = dev
         self._a = _NlArgs(self.num_atoms, cell_np, inv_np, pbc, r_max, np.zeros(3), np.ones(3))
+        self._ty = None
+        if edge_type_cutoff is not None:
+            self._ty = _NlTypes(atom_types, edge_type_cutoff, self.r_max, self.num_atoms, dev)
+        elif atom_types is not None:
+            raise ValueError("NeighborListPlan: atom_types is only read with edge_type_cutoff")
         self._s = _nl_scratch(self.num_atoms, self._a.nbins, dev)
         N, cap = self.num_atoms, self.capacity
         self.edge_index = torch.empty((2, cap), dtype=torch.int64, device=dev)
@@ -1204,12 +1368,30 @@ class NeighborListPlan:
             raise ValueError(f"NeighborListPlan: pos must be [{self.num_atoms}, 3], got {tuple(pos.shape)}")
         pos = pos.detach().double().contiguous()
         L = _capi.lib()
-        a, s = self._a, self._s
-        _nl_rows(pos, a, s, self._params_dev)
+        a, s, ty = self._a, self._s, self._ty
+        if ty is None:
+            _nl_rows(pos, a, s, self._params_dev)
+        else:
+            _nl_rows(pos, a, s, self._params_dev, ty)
         st = _stream()
         _capi.check(L.nqb_nl_pad(self.num_atoms, self.capacity, _ptr(s["row_ptr"]), _ptr(self.row_ptr),
                                  _ptr(self.num_edges), _ptr(self.overflow), st), "nqb_nl_pad")
-        if self.variable_cell:
+        if ty is not None and self.variable_cell:
+            _capi.check(L.nqb_nl_fill_capacity_dp_typed(self.num_atoms, self.capacity, _ptr(self._params_dev),
+                                                        _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["base"]),
+                                                        _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(self.row_ptr),
+                                                        _ptr(self.overflow), _ptr(ty.types), _ptr(ty.rc2), ty.T,
+                                                        _ptr(self.edge_index), _ptr(self.edge_cell_shift), st),
+                        "nqb_nl_fill_capacity_dp_typed")
+        elif ty is not None:
+            _capi.check(L.nqb_nl_fill_capacity_typed(self.num_atoms, self.capacity, a.cell, a.inv, a.pbc, a.nb, a.sr,
+                                                     a.r_max, _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["base"]),
+                                                     _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(self.row_ptr),
+                                                     _ptr(self.overflow), self._pad_shift_c, _ptr(ty.types),
+                                                     _ptr(ty.rc2), ty.T, _ptr(self.edge_index),
+                                                     _ptr(self.edge_cell_shift), st),
+                        "nqb_nl_fill_capacity_typed")
+        elif self.variable_cell:
             _capi.check(L.nqb_nl_fill_capacity_dp(self.num_atoms, self.capacity, _ptr(self._params_dev),
                                                   _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["base"]), _ptr(s["order"]),
                                                   _ptr(s["bin_start"]), _ptr(self.row_ptr), _ptr(self.overflow),
