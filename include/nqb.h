@@ -262,6 +262,23 @@ int nqb_nl_fill_capacity_dp(int64_t N, int64_t capacity, const void* params_dev,
                             const int64_t* row_ptr_pad /* [N+1] */, const int32_t* overflow /* [1] */,
                             int64_t* edge_index /* [2,capacity] */, double* shifts /* [capacity,3] */,
                             nqb_stream_t st);
+/* Open directions (pbc[d] == 0) in a parameter block, so that a captured list follows a molecule or slab whose
+ * bounding box moves.  nqb_nl_params_pack_open fills out_host [nqb_nl_params_bytes()] fully, on the HOST, like
+ * nqb_nl_params_pack but accepting open directions: periodic directions get the values nqb_nl_params_pack gives them;
+ * an open direction's bounding box and grid are left for nqb_nl_bbox (a one-bin grid until it runs).  cap >= 1: most
+ * bins along an open direction (the caller's scratch grid); perp_host: 3 finite positive doubles, the distance between
+ * opposite faces of the cell along each lattice direction (1 / |column d of inv|); r_max finite and > 0.
+ * nqb_nl_bbox (N >= 0; nothing for N = 0) writes, in the DEVICE block params_dev and nowhere else in it, for each
+ * open direction d: lo = min over atoms of the fractional coordinate (computed as nqb_nl_bin_dp computes it),
+ * width = max(fmax - fmin, 1e-9) * (1 + 1e-9), nb = min(cap, max(1, floor(perp[d] * width / r_max))), search = 1.
+ * NaN coordinates are skipped; nb lies in [1, cap] for any input.  work [8] u64: zero before the first call, and
+ * every call leaves it zero again (one work buffer per stream; no host synchronisation, capturable).  Run it
+ * stream-ordered before nqb_nl_bin_dp; count, fill and the bin scratch then follow the device grid. */
+int nqb_nl_params_pack_open(const double* cell_host, const double* inv_host, const int* pbc, const int* nbins,
+                            const int* search, double r_max, const double* pad_shift_host, int cap,
+                            const double* perp_host, void* out_host);
+int nqb_nl_bbox(const double* pos /* [N,3] */, int64_t N, void* params_dev, uint64_t* work /* [8] */,
+                nqb_stream_t st);
 /* Per-edge-type cutoffs: count, fill and fill with capacity (by value and _dp) with the membership test
  * d2 < rc2[T * types[i] + types[j]] in place of d2 < r_max^2.  types [N] i64 in [0, T) and rc2 [T*T] f64 (rc * rc in
  * float64, every rc <= r_max) are device arrays; bins, search ranges and parameter blocks stay those of r_max, so

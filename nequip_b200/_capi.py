@@ -58,6 +58,8 @@ SIGNATURES = {
     "nqb_nl_bin_dp": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nqb_nl_count_dp": (_i32, [_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nqb_nl_fill_capacity_dp": (_i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nl_params_pack_open": (_i32, [_vp, _vp, _vp, _vp, _vp, _dbl, _vp, _i32, _vp, _vp]),
+    "nqb_nl_bbox": (_i32, [_vp, _i64, _vp, _vp, _vp]),
     "nqb_sh_fwd": (_i32, [_i32, _vp, _i64, _i32, _vp, _vp]),
     "nqb_sh_bwd": (_i32, [_i32, _vp, _i64, _i32, _vp, _vp, _vp]),
     "nqb_edge_embed_fwd": (

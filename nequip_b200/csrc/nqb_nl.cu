@@ -14,6 +14,7 @@
 // offsets, squared distance) is done in the same order as the host reference list (nequip_b200/data.py) with
 // explicitly rounded operations (no FMA contraction), so the edge set is bit-identical.
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -41,9 +42,15 @@ struct NlParams {
 // per launch) or a block in device memory, NlBlock* (variable cell: nqb_nl_params_pack fills it on the host and the
 // caller copies it in before a launch or a graph replay).  The block also holds the null-edge shift of the capacity
 // fill, which follows the cell.  One kernel body per kernel reads its parameters through nl_p / nl_pad_shift.
+// Open directions (nqb_nl_params_pack_open): the trailing fields are read by nqb_nl_bbox only, which writes the
+// bounding box (p.lo, p.width) and the grid (p.nb, p.sr) of every open direction into the block before the bins.
 struct NlBlock {
   NlParams p;
   double pad_shift[3];
+  int open[3];         // 1: the bounding box of this direction is found on the device
+  int cap;             // most bins along an open direction (the caller's scratch grid)
+  double perp[3];      // distance between opposite faces of the cell along each lattice direction
+  double r_max;
 };
 typedef const NlBlock* __restrict__ NlBlockPtr;
 
@@ -66,6 +73,17 @@ struct NlTypes {
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
 
+// fractional coordinates of one position: x / diag for an orthorhombic cell (as the host list), otherwise
+// pos @ inv with explicitly rounded operations; k_nl_bin and k_nl_bbox both call this, so the bounding box is that
+// of the coordinates that get binned
+__device__ __forceinline__ void nl_frac(const NlParams& p, double x, double y, double z, double f[3]) {
+  if (p.orthorhombic) {
+    f[0] = __ddiv_rn(x, p.diag[0]); f[1] = __ddiv_rn(y, p.diag[1]); f[2] = __ddiv_rn(z, p.diag[2]);
+  } else {
+    for (int d = 0; d < 3; ++d) f[d] = dadd(dadd(dmul(x, p.inv[d]), dmul(y, p.inv[3 + d])), dmul(z, p.inv[6 + d]));
+  }
+}
+
 // wrapped cartesian position, integer base shift (pos + base @ cell is the wrapped position) and bin of one atom
 template <class PS>
 __global__ void k_nl_bin(PS ps, const double* __restrict__ pos, int64_t N, double* __restrict__ wpos,
@@ -73,13 +91,8 @@ __global__ void k_nl_bin(PS ps, const double* __restrict__ pos, int64_t N, doubl
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   const NlParams& p = nl_p(ps);
-  const double x = pos[3 * i], y = pos[3 * i + 1], z = pos[3 * i + 2];
   double f[3];
-  if (p.orthorhombic) {
-    f[0] = __ddiv_rn(x, p.diag[0]); f[1] = __ddiv_rn(y, p.diag[1]); f[2] = __ddiv_rn(z, p.diag[2]);
-  } else {
-    for (int d = 0; d < 3; ++d) f[d] = dadd(dadd(dmul(x, p.inv[d]), dmul(y, p.inv[3 + d])), dmul(z, p.inv[6 + d]));
-  }
+  nl_frac(p, pos[3 * i], pos[3 * i + 1], pos[3 * i + 2], f);
   double w[3];
   int c[3];
   for (int d = 0; d < 3; ++d) {
@@ -230,6 +243,70 @@ __global__ void k_nl_pad(int64_t N, int64_t capacity, const int64_t* __restrict_
   }
 }
 
+// Bounding box of the open directions (nqb_nl_bbox).  Min / max of the fractional coordinates (nl_frac, the
+// arithmetic of k_nl_bin) per CTA, then one atomicMax per CTA and value into work[0..5] on an order-preserving 64-bit
+// key: work[d] = max of ~key(fmin_d), work[3 + d] = max of key(fmax_d), so 0 is the identity of all six.  fmin / fmax
+// skip NaN coordinates.  The CTA that takes the last ticket (work[6]) reads the six keys back with atomicExch(0),
+// writes lo / width / nb / sr of every open direction into the block, as ops.neighbor_list computes them on the host,
+// and resets the ticket: the work words are zero again for the next call or graph replay.  Min and max are exact, so
+// the result does not depend on the order in which CTAs arrive.
+constexpr int kBboxThreads = 256;
+constexpr int64_t kBboxMaxBlocks = 264;
+
+__device__ __forceinline__ unsigned long long nl_key(double v) {  // monotone: v < w => key(v) < key(w), -0 < +0
+  const unsigned long long b = (unsigned long long)__double_as_longlong(v);
+  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double nl_unkey(unsigned long long k) {
+  return __longlong_as_double((long long)((k >> 63) ? (k & 0x7FFFFFFFFFFFFFFFull) : ~k));
+}
+
+__global__ void __launch_bounds__(kBboxThreads)
+k_nl_bbox(NlBlock* __restrict__ b, const double* __restrict__ pos, int64_t N, unsigned long long* __restrict__ acc,
+          unsigned int* __restrict__ ticket) {
+  const NlParams& p = b->p;
+  double lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (int64_t)gridDim.x * blockDim.x) {
+    double f[3];
+    nl_frac(p, pos[3 * i], pos[3 * i + 1], pos[3 * i + 2], f);
+    for (int d = 0; d < 3; ++d) { lo[d] = fmin(lo[d], f[d]); hi[d] = fmax(hi[d], f[d]); }
+  }
+  for (int o = 16; o > 0; o >>= 1)
+    for (int d = 0; d < 3; ++d) {
+      lo[d] = fmin(lo[d], __shfl_xor_sync(0xffffffffu, lo[d], o));
+      hi[d] = fmax(hi[d], __shfl_xor_sync(0xffffffffu, hi[d], o));
+    }
+  __shared__ double s[kBboxThreads / 32][6];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0)
+    for (int d = 0; d < 3; ++d) { s[warp][d] = lo[d]; s[warp][3 + d] = hi[d]; }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (int w = 1; w < kBboxThreads / 32; ++w)
+    for (int d = 0; d < 3; ++d) { lo[d] = fmin(lo[d], s[w][d]); hi[d] = fmax(hi[d], s[w][3 + d]); }
+  for (int d = 0; d < 3; ++d) {
+    atomicMax(acc + d, ~nl_key(lo[d]));
+    atomicMax(acc + 3 + d, nl_key(hi[d]));
+  }
+  __threadfence();
+  if (atomicAdd(ticket, 1u) != gridDim.x - 1) return;
+  __threadfence();
+  for (int d = 0; d < 3; ++d) {
+    const double fmin_d = nl_unkey(~atomicExch(acc + d, 0ull)), fmax_d = nl_unkey(atomicExch(acc + 3 + d, 0ull));
+    if (!b->open[d]) continue;
+    // width = max(fmax - fmin, 1e-9) (1 + 1e-9); a NaN or -inf difference (no finite coordinate) takes 1e-9
+    double w = dadd(fmax_d, -fmin_d);
+    w = dmul(w > 1e-9 ? w : 1e-9, 1.0 + 1e-9);
+    // nb = min(cap, max(1, floor(perp * width / r_max))), in [1, cap] for any width (NaN gives 1, inf gives cap)
+    const double t = floor(__ddiv_rn(dmul(b->perp[d], w), b->r_max));
+    b->p.lo[d] = fmin_d;
+    b->p.width[d] = w;
+    b->p.nb[d] = t >= 1.0 ? (t < (double)b->cap ? (int)t : b->cap) : 1;
+    b->p.sr[d] = 1;
+  }
+  atomicExch(ticket, 0u);
+}
+
 }  // namespace
 
 // Step 1: bins.  cell/inv: row-major 3x3 on the HOST (9 doubles each); nbins/search: per direction.
@@ -359,6 +436,49 @@ extern "C" int nqb_nl_params_pack(const double* cell_host, const double* inv_hos
   for (int d = 0; d < 3; ++d) b.pad_shift[d] = pad_shift_host[d];
   memcpy(out_host, &b, sizeof(b));
   return 0;
+}
+
+static int nl_launch_done();
+
+// Open directions: the block of nqb_nl_params_pack with the directions where pbc[d] == 0 marked open.  Their
+// lo / width / nb / sr are left for nqb_nl_bbox (a valid one-bin grid until then); cap, perp and r_max are what it
+// derives the grid from.
+extern "C" int nqb_nl_params_pack_open(const double* cell_host, const double* inv_host, const int* pbc,
+                                       const int* nbins, const int* search, double r_max, const double* pad_shift_host,
+                                       int cap, const double* perp_host, void* out_host) {
+  if (!cell_host || !inv_host || !pbc || !nbins || !search || !pad_shift_host || !perp_host || !out_host)
+    return nqb_set_error("nqb_nl_params_pack_open: null pointer");
+  if (cap < 1 || !(r_max > 0.0) || !isfinite(r_max))
+    return nqb_set_error("nqb_nl_params_pack_open: needs cap >= 1 and a finite r_max > 0");
+  for (int d = 0; d < 3; ++d) {
+    if (pbc[d] && (nbins[d] < 1 || search[d] < 0)) return nqb_set_error("nqb_nl_params_pack_open: bad bin grid");
+    if (!(perp_host[d] > 0.0) || !isfinite(perp_host[d]))
+      return nqb_set_error("nqb_nl_params_pack_open: perpendicular widths must be finite and positive");
+  }
+  NlBlock b;
+  memset(&b, 0, sizeof(b));
+  nl_params(cell_host, inv_host, pbc, nbins, search, r_max, b.p);
+  for (int d = 0; d < 3; ++d) {
+    b.pad_shift[d] = pad_shift_host[d];
+    b.open[d] = pbc[d] ? 0 : 1;
+    if (!pbc[d]) { b.p.nb[d] = 1; b.p.sr[d] = 1; }
+    b.perp[d] = perp_host[d];
+  }
+  b.cap = cap;
+  b.r_max = r_max;
+  memcpy(out_host, &b, sizeof(b));
+  return 0;
+}
+
+extern "C" int nqb_nl_bbox(const double* pos, int64_t N, void* params_dev, uint64_t* work, nqb_stream_t st) {
+  if (N < 0) return nqb_set_error("nqb_nl_bbox: negative size");
+  if (N == 0) return 0;
+  if (!pos || !params_dev || !work) return nqb_set_error("nqb_nl_bbox: null pointer");
+  int64_t blocks = (N + kBboxThreads - 1) / kBboxThreads;
+  if (blocks > kBboxMaxBlocks) blocks = kBboxMaxBlocks;
+  k_nl_bbox<<<(unsigned)blocks, kBboxThreads, 0, (cudaStream_t)st>>>(
+      (NlBlock*)params_dev, pos, N, (unsigned long long*)work, (unsigned int*)(work + 6));
+  return nl_launch_done();
 }
 
 extern "C" int nqb_nl_bin_dp(const double* pos, int64_t N, const void* params_dev, double* wpos, int32_t* base,

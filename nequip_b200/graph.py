@@ -13,7 +13,8 @@ reference's neighbour lists produce, nequip/data/transforms/neighborlist.py:120-
 is computed inside the graph and verified when the results are read.  Anything else: use the eager
 ``model(data)`` call (same kernels, more launch overhead).
 
-``GraphedMDStep`` lifts the shape restriction for molecular dynamics in a fixed periodic cell: the device neighbour
+``GraphedMDStep`` lifts the shape restriction for molecular dynamics in a fixed cell (periodic, partly periodic
+like a slab, or none for a molecule in vacuum): the device neighbour
 list (``ops.NeighborListPlan``) is part of the graph and writes a list of fixed length ``capacity`` whose unused
 slots hold null edges, which contribute exactly zero (DESIGN.md section 4.8).  So one graph replays every step
 whatever the step's edge count, and a step that needs more than ``capacity`` edges is re-captured.  With
@@ -147,12 +148,17 @@ CAPACITY_SLACK = 0.02
 
 
 class GraphedMDStep(GraphedEnergyForces):
-    """One CUDA graph for a whole MD step in a periodic cell: positions -> device neighbour list -> energy -> forces.
+    """One CUDA graph for a whole MD step: positions -> device neighbour list -> energy -> forces.
     ``g = GraphedMDStep(model, example); out = g(pos)``.
 
-    ``example`` holds CUDA tensors ``pos`` [N,3], ``atom_types`` [N] and ``cell`` [3,3] (all three directions periodic).
-    By default the cell is captured (NVE / NVT).  ``capacity`` is the length of the edge buffer, by default
-    ``E0 + ceil(CAPACITY_SLACK * E0)`` with E0 the example's edge count; unused slots hold null edges.
+    ``example`` holds CUDA tensors ``pos`` [N,3], ``atom_types`` [N] and, for a periodic system, ``cell`` [3,3].
+    The periodicity is ``example["pbc"]`` ([3] or [1, 3] bools) when present; otherwise all three directions are
+    periodic with a cell and all open without one (a molecule in vacuum).  Along open directions the neighbour list
+    finds the positions' bounding box on the device at every replay (``ops.NeighborListPlan(open_boundaries=True)``),
+    and the captured model call reads the plan's cell (``plan.cell``, the identity without a cell), to which the null
+    edges' shift refers.  By default the cell is captured (NVE / NVT).  ``capacity`` is the length of the edge buffer,
+    by default ``E0 + ceil(CAPACITY_SLACK * E0)`` with E0 the example's edge count (``ops.neighbor_list`` with the
+    example's cell and periodicity); unused slots hold null edges.
 
     ``g(pos)`` takes host (pinned) or device positions and returns ``total_energy`` [1,1], ``atomic_energy`` [N,1],
     ``forces`` [N,3] and ``num_edges`` [1] -- views of static buffers that the next call overwrites.  Every call
@@ -168,16 +174,21 @@ class GraphedMDStep(GraphedEnergyForces):
     costs one device-to-host read).  It is copied into the static ``cell`` input the model reads and handed to the
     neighbour list (``ops.NeighborListPlan.set_cell``) before the replay.  The captured call is
     ``model(d, compute_stress=True)``, so the outputs also hold ``stress`` and ``virial`` [1,3,3].  A re-capture
-    happens at the current cell, with a bin grid chosen for it."""
+    happens at the current cell, with a bin grid chosen for it.  ``variable_cell`` needs all three directions periodic
+    (``ValueError`` otherwise)."""
 
     def __init__(self, model, example: Dict[str, torch.Tensor], capacity: Optional[int] = None, warmup: int = 3,
                  variable_cell: bool = False):
+        cell = example.get("cell")
+        self.pbc = self._periodicity(example)
+        if cell is None and any(self.pbc):
+            raise ValueError("GraphedMDStep: a periodic direction needs a cell")
+        if variable_cell and not all(self.pbc):
+            raise ValueError("GraphedMDStep: variable_cell needs all three directions periodic")
         if example["pos"].device.type != "cuda":
             raise RuntimeError("GraphedMDStep needs CUDA tensors (there is no CPU path)")
-        if example.get("cell") is None:
-            raise ValueError("GraphedMDStep needs a periodic cell")
         if capacity is None:
-            e0 = int(ops.neighbor_list(example["pos"], example["cell"], True, model.r_max,
+            e0 = int(ops.neighbor_list(example["pos"], cell, self.pbc, model.r_max,
                                        **self._edge_type_args(model, example))["edge_index"].shape[1])
             capacity = e0 + math.ceil(CAPACITY_SLACK * e0)
         self.variable_cell = bool(variable_cell)
@@ -185,7 +196,22 @@ class GraphedMDStep(GraphedEnergyForces):
         self._warmup = warmup
         self._num_edges_host = torch.zeros(1, dtype=torch.int64).pin_memory()
         self._overflow_host = torch.zeros(1, dtype=torch.int32).pin_memory()
-        self._capture(model, {k: example[k] for k in ("pos", "atom_types", "cell")}, int(capacity))
+        self._capture(model, {k: example[k] for k in ("pos", "atom_types", "cell") if example.get(k) is not None},
+                      int(capacity))
+
+    @staticmethod
+    def _periodicity(example: Dict[str, torch.Tensor]) -> tuple:
+        """3 bools: ``example["pbc"]`` ([3] or [1, 3], or one bool) when present, else all periodic with a cell and
+        all open without one."""
+        pbc = example.get("pbc")
+        if pbc is None:
+            return (example.get("cell") is not None,) * 3
+        flags = [bool(b) for b in torch.as_tensor(pbc).reshape(-1).tolist()]
+        if len(flags) == 1:
+            flags *= 3
+        if len(flags) != 3:
+            raise ValueError(f"GraphedMDStep: pbc must hold 3 flags, got {len(flags)}")
+        return tuple(flags)
 
     @staticmethod
     def _edge_type_args(model, example: Dict[str, torch.Tensor]) -> dict:
@@ -195,9 +221,13 @@ class GraphedMDStep(GraphedEnergyForces):
 
     def _capture(self, model, example: Dict[str, torch.Tensor], capacity: int) -> None:
         self.capacity = capacity
-        self.plan = ops.NeighborListPlan(example["pos"].shape[0], example["cell"], True, model.r_max, capacity,
+        is_open = not all(self.pbc)
+        self.plan = ops.NeighborListPlan(example["pos"].shape[0], example.get("cell"), self.pbc, model.r_max, capacity,
                                          device=example["pos"].device, variable_cell=self.variable_cell,
-                                         **self._edge_type_args(model, example))
+                                         **self._edge_type_args(model, example), open_boundaries=is_open)
+        if is_open:
+            # the null edges' shift refers to plan.cell (the identity without a cell): the model must see it
+            example = dict(example, cell=self.plan.cell)
         super().__init__(model, example, warmup=self._warmup)
         ops.src_csr_cache.clear()  # like csr_cache: an entry made during the capture lives in the graph's pool
         out, self._out = self._out, None

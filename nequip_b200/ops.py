@@ -1067,6 +1067,18 @@ def _nl_cell(cell, pbc):
     return pbc, cell_np, np.linalg.inv(cell_np)
 
 
+def _nl_bin_cap(N: int) -> int:
+    """Most bins per direction of the device list: round((4 N)^(1/3)), at least 1."""
+    return max(1, int(round((4 * max(N, 1)) ** (1.0 / 3.0))))
+
+
+def _nl_perp(inv_np):
+    """Distance between opposite faces along each lattice direction = 1 / |column d of the inverse| (3 floats)."""
+    import numpy as np
+
+    return 1.0 / np.linalg.norm(inv_np, axis=0)
+
+
 class _NlArgs:
     """Host-side arguments of the nqb_nl_* calls: cell, inverse, periodicity, bin grid and search range.
 
@@ -1076,11 +1088,10 @@ class _NlArgs:
     def __init__(self, N: int, cell_np, inv_np, pbc, r_max: float, lo, width, nb=None):
         import numpy as np
 
-        # distance between opposite faces along each lattice direction = 1 / |column d of the inverse|
-        perp = 1.0 / np.linalg.norm(inv_np, axis=0)
+        perp = _nl_perp(inv_np)
         fixed = nb is not None
         nb, sr = ([int(n) for n in nb] if fixed else [1, 1, 1]), [1, 1, 1]
-        cap = max(1, int(round((4 * max(N, 1)) ** (1.0 / 3.0))))
+        cap = _nl_bin_cap(N)
         for d in range(3):
             extent = perp[d] * (1.0 if pbc[d] else width[d])
             if not fixed:
@@ -1248,21 +1259,30 @@ def null_edge_shift(cell, r_max: float):
     return shift
 
 
+def _nl_check_cell(cell, what: str):
+    """``cell`` ([3,3] or [1,3,3]) as a [3, 3] float64 host array; ``ValueError`` for another shape, a non-finite or a
+    singular cell."""
+    import numpy as np
+
+    c = cell.detach().cpu().double().numpy() if torch.is_tensor(cell) else np.asarray(cell, dtype=np.float64)
+    if c.shape not in ((3, 3), (1, 3, 3)):
+        raise ValueError(f"{what}: cell must be [3, 3] or [1, 3, 3], got {tuple(c.shape)}")
+    c = c.reshape(3, 3)
+    if not np.all(np.isfinite(c)):
+        raise ValueError(f"{what}: cell is not finite")
+    vol = abs(float(np.linalg.det(c)))
+    if not vol > 1e-12 * float(np.prod(np.linalg.norm(c, axis=1))):
+        raise ValueError(f"{what}: cell is singular")
+    return c
+
+
 def _nl_cell_block(cell, r_max: float, nb, num_atoms: int):
     """Host part of ``NeighborListPlan.set_cell``: checks ``cell`` ([3,3] or [1,3,3], finite, non-singular) and returns
     the ``_NlArgs`` of this cell on the fixed bin grid ``nb`` (inverse as in ``neighbor_list``, search range for this
     cell), its null-edge shift and the packed device parameter block (``nqb_nl_params_pack``, ctypes buffer)."""
     import numpy as np
 
-    c = cell.detach().cpu().double().numpy() if torch.is_tensor(cell) else np.asarray(cell, dtype=np.float64)
-    if c.shape not in ((3, 3), (1, 3, 3)):
-        raise ValueError(f"set_cell: cell must be [3, 3] or [1, 3, 3], got {tuple(c.shape)}")
-    c = c.reshape(3, 3)
-    if not np.all(np.isfinite(c)):
-        raise ValueError("set_cell: cell is not finite")
-    vol = abs(float(np.linalg.det(c)))
-    if not vol > 1e-12 * float(np.prod(np.linalg.norm(c, axis=1))):
-        raise ValueError("set_cell: cell is singular")
+    c = _nl_check_cell(cell, "set_cell")
     pbc, cell_np, inv_np = _nl_cell(c, True)
     a = _NlArgs(num_atoms, cell_np, inv_np, pbc, r_max, np.zeros(3), np.ones(3), nb=nb)
     pad_shift = null_edge_shift(cell_np, r_max)
@@ -1278,9 +1298,8 @@ class NeighborListPlan:
     synchronisation, so it can be captured in a CUDA graph (``graph.GraphedMDStep``).
 
     All host work (inverse cell, bin grid, search range, the null-edge shift) and every allocation happen here; the
-    cell is fixed for the plan's lifetime unless ``variable_cell``.  The cell must be given and periodic in all three directions: a
-    non-periodic direction needs the positions' bounding box on the host at every call.  A molecule in vacuum can use
-    a large periodic box.
+    cell is fixed for the plan's lifetime unless ``variable_cell``.  The cell must be given and periodic in all three
+    directions unless ``open_boundaries`` (below).
 
     ``variable_cell=True`` (constant-pressure MD): the kernels read the cell-dependent arguments from a parameter
     block in device memory, and ``set_cell(cell)`` replaces them between runs (or graph replays) without touching
@@ -1296,20 +1315,41 @@ class NeighborListPlan:
 
     ``atom_types`` [N] + ``edge_type_cutoff`` [T, T]: per-edge-type cutoffs as in ``neighbor_list``.  The types are
     fixed for the plan's lifetime (the plan keeps a device copy whose pointer captured graphs hold); the cutoff table
-    does not depend on the cell, so ``set_cell`` leaves it alone."""
+    does not depend on the cell, so ``set_cell`` leaves it alone.
+
+    ``open_boundaries=True`` (molecules in vacuum, slabs): any ``pbc`` is accepted, and ``cell=None`` when no direction
+    is periodic (the identity then serves as the cell, as in ``neighbor_list``).  A plan with an open direction reads
+    its arguments from a device parameter block (``nqb_nl_params_pack_open``), and ``run`` first finds the bounding box
+    of the positions along the open directions on the device (``nqb_nl_bbox``), with the grid ``neighbor_list``
+    derives from it on the host: ``nb = min(cap, max(1, floor(perp * width / r_max)))``, cap = round((4 N)^(1/3)).
+    The rows are those of ``neighbor_list(pos, cell, pbc)``.  ``plan.cell`` ([3, 3] float64, on the device) is the cell
+    the shifts refer to: the caller must give it to the model as ``cell``, since the null edges (i, i, pad_shift)
+    only have their length r_max + |a_d| through it; real edges along open directions have shift 0.  The cell must be
+    finite and non-singular, and ``variable_cell`` needs all three directions periodic."""
 
     def __init__(self, num_atoms: int, cell, pbc, r_max: float, capacity: int, device=None,
-                 variable_cell: bool = False, atom_types=None, edge_type_cutoff=None):
+                 variable_cell: bool = False, atom_types=None, edge_type_cutoff=None, *,
+                 open_boundaries: bool = False):
         import numpy as np
 
-        if cell is None:
-            raise ValueError("NeighborListPlan needs a cell")
         if isinstance(pbc, bool):
             pbc = (pbc,) * 3
         pbc = [bool(b) for b in (pbc.tolist() if torch.is_tensor(pbc) else pbc)]
-        if len(pbc) != 3 or not all(pbc):
-            raise ValueError("NeighborListPlan needs all three directions periodic (the bounding box of a "
-                             "non-periodic direction is found on the host at every call); use a large periodic box")
+        if not open_boundaries:
+            if cell is None:
+                raise ValueError("NeighborListPlan needs a cell")
+            if len(pbc) != 3 or not all(pbc):
+                raise ValueError("NeighborListPlan needs all three directions periodic unless built with "
+                                 "open_boundaries=True")
+        else:
+            if len(pbc) != 3:
+                raise ValueError(f"NeighborListPlan: pbc must be a bool or 3 bools, got {pbc}")
+            if cell is None and any(pbc):
+                raise ValueError("NeighborListPlan: a periodic direction needs a cell")
+            if variable_cell and not all(pbc):
+                raise ValueError("NeighborListPlan: variable_cell needs all three directions periodic")
+            if cell is not None:
+                _nl_check_cell(cell, "NeighborListPlan")
         if int(num_atoms) < 1 or int(capacity) < 0:
             raise ValueError("NeighborListPlan needs num_atoms >= 1 and capacity >= 0")
         self.num_atoms, self.capacity, self.r_max = int(num_atoms), int(capacity), float(r_max)
@@ -1320,6 +1360,22 @@ class NeighborListPlan:
             cell.device if torch.is_tensor(cell) and cell.is_cuda else torch.device("cuda"))
         self.device = dev
         self._a = _NlArgs(self.num_atoms, cell_np, inv_np, pbc, r_max, np.zeros(3), np.ones(3))
+        self._open = not all(pbc)
+        if open_boundaries:
+            self.cell = torch.from_numpy(cell_np.copy()).to(dev)
+        if self._open:
+            # scratch grid: cap bins along every open direction; nqb_nl_bbox picks at most that many per run
+            cap = _nl_bin_cap(self.num_atoms)
+            nb = [n if p else cap for n, p in zip(self._a.nb, pbc)]
+            self._a = _NlArgs(self.num_atoms, cell_np, inv_np, pbc, r_max, np.zeros(3), np.ones(3), nb=nb)
+            L = _capi.lib()
+            block = C.create_string_buffer(int(L.nqb_nl_params_bytes()))
+            a = self._a
+            _capi.check(L.nqb_nl_params_pack_open(a.cell, a.inv, a.pbc, a.nb, a.sr, a.r_max, self._pad_shift_c, cap,
+                                                  (C.c_double * 3)(*_nl_perp(inv_np)), block),
+                        "nqb_nl_params_pack_open")
+            open_block = torch.frombuffer(bytearray(block.raw), dtype=torch.uint8).to(dev)
+            self._bbox_work = torch.zeros((8,), dtype=torch.int64, device=dev)  # left zero by every nqb_nl_bbox
         self._ty = None
         if edge_type_cutoff is not None:
             self._ty = _NlTypes(atom_types, edge_type_cutoff, self.r_max, self.num_atoms, dev)
@@ -1341,6 +1397,8 @@ class NeighborListPlan:
             self._params_host = torch.empty((nbytes,), dtype=torch.uint8).pin_memory()
             self._params_event: Optional[torch.cuda.Event] = None
             self.set_cell(cell)
+        elif self._open:
+            self._params_dev = open_block
 
     def set_cell(self, cell) -> None:
         """Make the following ``run`` calls (and replays of graphs that captured them) use ``cell`` ([3,3] or
@@ -1369,6 +1427,9 @@ class NeighborListPlan:
         pos = pos.detach().double().contiguous()
         L = _capi.lib()
         a, s, ty = self._a, self._s, self._ty
+        if self._open:
+            _capi.check(L.nqb_nl_bbox(_ptr(pos), self.num_atoms, _ptr(self._params_dev), _ptr(self._bbox_work),
+                                      _stream()), "nqb_nl_bbox")
         if ty is None:
             _nl_rows(pos, a, s, self._params_dev)
         else:
@@ -1376,7 +1437,7 @@ class NeighborListPlan:
         st = _stream()
         _capi.check(L.nqb_nl_pad(self.num_atoms, self.capacity, _ptr(s["row_ptr"]), _ptr(self.row_ptr),
                                  _ptr(self.num_edges), _ptr(self.overflow), st), "nqb_nl_pad")
-        if ty is not None and self.variable_cell:
+        if ty is not None and self._params_dev is not None:
             _capi.check(L.nqb_nl_fill_capacity_dp_typed(self.num_atoms, self.capacity, _ptr(self._params_dev),
                                                         _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["base"]),
                                                         _ptr(s["order"]), _ptr(s["bin_start"]), _ptr(self.row_ptr),
@@ -1391,7 +1452,7 @@ class NeighborListPlan:
                                                      _ptr(ty.rc2), ty.T, _ptr(self.edge_index),
                                                      _ptr(self.edge_cell_shift), st),
                         "nqb_nl_fill_capacity_typed")
-        elif self.variable_cell:
+        elif self._params_dev is not None:
             _capi.check(L.nqb_nl_fill_capacity_dp(self.num_atoms, self.capacity, _ptr(self._params_dev),
                                                   _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["base"]), _ptr(s["order"]),
                                                   _ptr(s["bin_start"]), _ptr(self.row_ptr), _ptr(self.overflow),
