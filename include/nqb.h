@@ -172,6 +172,17 @@ int nqb_edge_embed_bwd_typed(int lmax, int num_bessel, double r_max, double poly
                              const int64_t* types, const int64_t* type_index, const double* recip, int T,
                              int out_dtype, const void* grad_y, const void* grad_emb, double* grad_pos,
                              double* grad_vec, nqb_stream_t st);
+/* A batch of frames (nequip/nn/utils.py:96-106, the cell of an edge is cell[batch[edge_index[0]]]): as
+ * nqb_edge_embed_fwd with shift [E,3], cells [F,3,3] and frame [N] i64 in [0, F) (the frame of each atom), all
+ * device arrays and all required; edge e takes cells + 9 * frame[edge_index[0][e]] in the same shift expression, so
+ * each frame's outputs are bitwise those of nqb_edge_embed_fwd with that frame's cell.  types / type_index / recip /
+ * T as nqb_edge_embed_fwd_typed, or all three NULL for the untyped embedding.  Same write contracts.  The backward
+ * reads the stored edge vectors only: nqb_edge_embed_bwd(_typed) serves framed edges unchanged. */
+int nqb_edge_embed_fwd_frames(int lmax, int num_bessel, double r_max, double poly_p, double prefactor,
+                              const double* pos, const int64_t* edge_index, const double* shift, const double* cells,
+                              const int64_t* frame, int64_t N, int64_t E, const int64_t* types,
+                              const int64_t* type_index, const double* recip, int T, int out_dtype, double* vec,
+                              void* y, void* emb, nqb_stream_t st);
 
 /* ZBL pair energy (nequip/nn/pair_potential.py:230-386), everything in fp64.  Per edge e = (i -> j), i =
  * edge_index[0][e]:  eps_e = A[ti,tj] / r * psi((S[ti,tj] * r) / a0) * f_c(r / r_max),  psi = the four-exponential
@@ -203,6 +214,17 @@ int nqb_zbl_bwd_typed(const double* pos, const int64_t* edge_index, const double
                       const double* vec, const int64_t* types, const double* table, int T, int64_t N, int64_t E,
                       double r_max, double poly_p, int cutoff_f32, const double* recip, const double* grad_e_atom,
                       double* grad_pos, double* grad_vec, nqb_stream_t st);
+/* A batch of frames: as nqb_zbl_fwd / nqb_zbl_bwd on positions, with shift [E,3], cells [F,3,3] and frame [N] i64
+ * in [0, F) (device arrays, required when E > 0); edge e takes cells + 9 * frame[edge_index[0][e]].  recip as the
+ * _typed calls, or NULL for the untyped envelope.  Same write contracts. */
+int nqb_zbl_fwd_frames(const double* pos, const int64_t* edge_index, const double* shift, const double* cells,
+                       const int64_t* frame, const int64_t* types, const double* table, int T, const int64_t* row_ptr,
+                       const int64_t* perm, int64_t N, int64_t E, double r_max, double poly_p, int cutoff_f32,
+                       const double* recip, double* e_atom, nqb_stream_t st);
+int nqb_zbl_bwd_frames(const double* pos, const int64_t* edge_index, const double* shift, const double* cells,
+                       const int64_t* frame, const int64_t* types, const double* table, int T, int64_t N, int64_t E,
+                       double r_max, double poly_p, int cutoff_f32, const double* recip, const double* grad_e_atom,
+                       double* grad_pos, double* grad_vec, nqb_stream_t st);
 
 /* Neighbour list on the device (cell list; full list, both directions, periodic images, no self edge in the home
  * image) -- replaces the host construction of nequip/data/_nl.py:60-152,292-361 and emits what
@@ -308,6 +330,30 @@ int nqb_nl_fill_capacity_dp_typed(int64_t N, int64_t capacity, const void* param
                                   const int32_t* overflow /* [1] */, const int64_t* types, const double* rc2, int T,
                                   int64_t* edge_index /* [2,capacity] */, double* shifts /* [capacity,3] */,
                                   nqb_stream_t st);
+/* A batch of independent frames in one exact list (the nvalchemiops batch_cell_list contract of
+ * nequip/data/_nl.py:212-289): atoms of frame f are a contiguous range, batch [N] i64 is non-decreasing in [0, F).
+ * nqb_nl_frames_pack fills out_host [F * nqb_nl_params_bytes()] on the HOST with one block per frame, from per-frame
+ * arrays laid out as the by-value calls take them (cell / inv [F,9], pbc / nbins / search [F,3], lo / width [F,3]):
+ * block f holds exactly what nqb_nl_bin, nqb_nl_count and nqb_nl_fill derive from frame f's arguments.  The caller
+ * copies the blocks to the device.  bin_base [F+1] i64 (device) is the exclusive scan of the frames' bin counts: frame
+ * f's bins are [bin_base[f], bin_base[f+1]) of one global range, so bin [N] holds global bin ids and order / bin_start
+ * ([bin_base[F] + 1]) come from one sort and one searchsorted over all frames.  An atom only meets atoms of its own
+ * frame.  types / rc2 / T as the _typed calls, or types and rc2 NULL for the r_max test.  Write contracts of
+ * nqb_nl_bin, nqb_nl_count and nqb_nl_fill; each frame's rows are those of a single-frame list of that frame, with
+ * atom indices global. */
+int nqb_nl_frames_pack(int F, const double* cell_host, const double* inv_host, const int* pbc, const int* nbins,
+                       const int* search, const double* lo, const double* width, double r_max, void* out_host);
+int nqb_nl_bin_frames(const double* pos, int64_t N, const void* blocks_dev, const int64_t* batch,
+                      const int64_t* bin_base, double* wpos /* [N,3] */, int32_t* base /* [N,3] */,
+                      int64_t* bin /* [N] */, int32_t* cidx /* [N,3] */, nqb_stream_t st);
+int nqb_nl_count_frames(int64_t N, const void* blocks_dev, const int64_t* batch, const int64_t* bin_base,
+                        const double* wpos, const int32_t* cidx, const int64_t* order, const int64_t* bin_start,
+                        const int64_t* types, const double* rc2, int T, int64_t* counts /* [N] */, nqb_stream_t st);
+int nqb_nl_fill_frames(int64_t N, int64_t E, const void* blocks_dev, const int64_t* batch, const int64_t* bin_base,
+                       const double* wpos, const int32_t* cidx, const int32_t* base, const int64_t* order,
+                       const int64_t* bin_start, const int64_t* row_ptr /* [N+1] */, const int64_t* types,
+                       const double* rc2, int T, int64_t* edge_index /* [2,E] */, double* shifts /* [E,3] */,
+                       nqb_stream_t st);
 
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).

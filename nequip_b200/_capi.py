@@ -88,6 +88,18 @@ SIGNATURES = {
     "nqb_nl_count_dp_typed": (_i32, [_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp]),
     "nqb_nl_fill_capacity_dp_typed": (
         _i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "nqb_nl_frames_pack": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp]),
+    "nqb_nl_bin_frames": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nl_count_frames": (_i32, [_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp]),
+    "nqb_nl_fill_frames": (
+        _i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "nqb_edge_embed_fwd_frames": (
+        _i32, [_i32, _i32, _dbl, _dbl, _dbl, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _vp,
+               _vp, _vp]),
+    "nqb_zbl_fwd_frames": (
+        _i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _i64, _dbl, _dbl, _i32, _vp, _vp, _vp]),
+    "nqb_zbl_bwd_frames": (
+        _i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _dbl, _dbl, _i32, _vp, _vp, _vp, _vp, _vp]),
     "nqb_mlp_hidden_fwd": (_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_fwd_rows": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),

@@ -54,12 +54,27 @@ struct NlBlock {
 };
 typedef const NlBlock* __restrict__ NlBlockPtr;
 
-__device__ __forceinline__ const NlParams& nl_p(const NlParams& p) { return p; }
-__device__ __forceinline__ const NlParams& nl_p(NlBlockPtr b) { return b->p; }
+// A batch of independent frames (PS = NlFrames, nqb_nl_*_frames): one block per frame, and atom i reads its
+// parameters from blocks[batch[i]].  The bins of all frames lie in one global range: frame f owns
+// [bin_base[f], bin_base[f + 1]), and nl_bin0 offsets atom i's bins by its frame's base, so the atoms of a frame only
+// ever meet the atoms of that frame.  For the other parameter sources nl_bin0 is 0.
+struct NlFrames {
+  const NlBlock* blocks;    // [F]
+  const int64_t* batch;     // [N] frame of each atom
+  const int64_t* bin_base;  // [F + 1]
+};
+
+__device__ __forceinline__ const NlParams& nl_p(const NlParams& p, int64_t) { return p; }
+__device__ __forceinline__ const NlParams& nl_p(NlBlockPtr b, int64_t) { return b->p; }
+__device__ __forceinline__ const NlParams& nl_p(const NlFrames& f, int64_t i) { return f.blocks[f.batch[i]].p; }
+__device__ __forceinline__ int64_t nl_bin0(const NlParams&, int64_t) { return 0; }
+__device__ __forceinline__ int64_t nl_bin0(NlBlockPtr, int64_t) { return 0; }
+__device__ __forceinline__ int64_t nl_bin0(const NlFrames& f, int64_t i) { return f.bin_base[f.batch[i]]; }
 __device__ __forceinline__ double3 nl_pad_shift(const NlParams&, double3 pad_shift) { return pad_shift; }
 __device__ __forceinline__ double3 nl_pad_shift(NlBlockPtr b, double3) {
   return make_double3(b->pad_shift[0], b->pad_shift[1], b->pad_shift[2]);
 }
+__device__ __forceinline__ double3 nl_pad_shift(const NlFrames&, double3 pad_shift) { return pad_shift; }
 
 // Per-edge-type cutoffs (kTyped): the pair (i, j) is a neighbour when d2 < rc2[T * types[i] + types[j]] instead of
 // d2 < r2.  rc2 = rc * rc is computed on the host in float64; the bins stay sized by the global r_max >= every rc.
@@ -90,7 +105,7 @@ __global__ void k_nl_bin(PS ps, const double* __restrict__ pos, int64_t N, doubl
                          int32_t* __restrict__ base, int64_t* __restrict__ bin, int32_t* __restrict__ cidx) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  const NlParams& p = nl_p(ps);
+  const NlParams& p = nl_p(ps, i);
   double f[3];
   nl_frac(p, pos[3 * i], pos[3 * i + 1], pos[3 * i + 2], f);
   double w[3];
@@ -116,7 +131,7 @@ __global__ void k_nl_bin(PS ps, const double* __restrict__ pos, int64_t N, doubl
     for (int d = 0; d < 3; ++d)
       wpos[3 * i + d] = dadd(dadd(dmul(w[0], p.cell[d]), dmul(w[1], p.cell[3 + d])), dmul(w[2], p.cell[6 + d]));
   }
-  bin[i] = ((int64_t)c[2] * p.nb[1] + c[1]) * p.nb[0] + c[0];
+  bin[i] = nl_bin0(ps, i) + ((int64_t)c[2] * p.nb[1] + c[1]) * p.nb[0] + c[0];
 }
 
 // visit every (neighbour atom j, image) candidate of atom i; F(j, img[3], within cutoff)
@@ -170,7 +185,8 @@ __global__ void k_nl_count(PS ps, int64_t N, const double* __restrict__ wpos, co
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   int64_t n = 0;
-  nl_visit<kTyped>(nl_p(ps), ty, i, wpos, cidx, order, bin_start, [&](int64_t, int, int, int) { ++n; });
+  nl_visit<kTyped>(nl_p(ps, i), ty, i, wpos, cidx, order, bin_start + nl_bin0(ps, i),
+                   [&](int64_t, int, int, int) { ++n; });
   counts[i] = n;
 }
 
@@ -199,7 +215,8 @@ __global__ void k_nl_fill(PS ps, int64_t N, const double* __restrict__ wpos, con
   int64_t n = 0;
   int64_t* ej = edge_index + E;  // neighbours (row 1)
   if (!kCapacity || *overflow == 0) {
-    nl_visit<kTyped>(nl_p(ps), ty, i, wpos, cidx, order, bin_start, [&](int64_t j, int ix, int iy, int iz) {
+    nl_visit<kTyped>(nl_p(ps, i), ty, i, wpos, cidx, order, bin_start + nl_bin0(ps, i),
+                     [&](int64_t j, int ix, int iy, int iz) {
       // insertion into the sorted prefix of the row (rows hold a few dozen neighbours)
       double s[3] = {(double)(ix + base[3 * j] - base[3 * i]), (double)(iy + base[3 * j + 1] - base[3 * i + 1]),
                      (double)(iz + base[3 * j + 2] - base[3 * i + 2])};
@@ -627,5 +644,98 @@ extern "C" int nqb_nl_fill_capacity_dp_typed(int64_t N, int64_t capacity, const 
   k_nl_fill<true, NlBlockPtr, true><<<(unsigned)((N + 63) / 64), 64, 0, (cudaStream_t)st>>>(
       (const NlBlock*)params_dev, N, wpos, cidx, base, order, bin_start, row_ptr_pad, capacity, edge_index, shifts,
       overflow, make_double3(0.0, 0.0, 0.0), ty);
+  return nl_launch_done();
+}
+
+// A batch of frames: bin, count and fill of the exact list with the parameters of atom i read from
+// blocks[batch[i]] and its bins offset by bin_base[batch[i]] (NlFrames).  batch [N] i64 is non-decreasing in [0, F),
+// bin_base [F + 1] i64 the exclusive scan of the frames' bin counts; the sort, searchsorted and scan between the
+// steps run once over the global bin range.  Per-edge-type cutoffs when types / rc2 are given (T >= 1), none when
+// both are NULL.  The blocks come from nqb_nl_frames_pack and are copied to the device by the caller.
+extern "C" int nqb_nl_frames_pack(int F, const double* cell_host, const double* inv_host, const int* pbc,
+                                  const int* nbins, const int* search, const double* lo, const double* width,
+                                  double r_max, void* out_host) {
+  if (F < 0) return nqb_set_error("nqb_nl_frames_pack: negative frame count");
+  if (F > 0 && (!cell_host || !inv_host || !pbc || !nbins || !search || !lo || !width || !out_host))
+    return nqb_set_error("nqb_nl_frames_pack: null pointer");
+  for (int f = 0; f < F; ++f) {
+    NlBlock b;
+    memset(&b, 0, sizeof(b));
+    for (int d = 0; d < 3; ++d)
+      if (nbins[3 * f + d] < 1 || search[3 * f + d] < 0) return nqb_set_error("nqb_nl_frames_pack: bad bin grid");
+    // the fields nqb_nl_bin (lo / width) and nqb_nl_count / nqb_nl_fill (the rest) build for this frame
+    nl_params(cell_host + 9 * f, inv_host + 9 * f, pbc + 3 * f, nbins + 3 * f, search + 3 * f, r_max, b.p);
+    for (int d = 0; d < 3; ++d) { b.p.lo[d] = lo[3 * f + d]; b.p.width[d] = width[3 * f + d]; }
+    memcpy((char*)out_host + (size_t)f * sizeof(NlBlock), &b, sizeof(b));
+  }
+  return 0;
+}
+
+static int nl_frames(const char* what, const void* blocks_dev, const int64_t* batch, const int64_t* bin_base,
+                     NlFrames& fr) {
+  if (!blocks_dev || !batch || !bin_base) {
+    static thread_local char msg[160];
+    snprintf(msg, sizeof(msg), "%s: null blocks / batch / bin_base", what);
+    return nqb_set_error(msg);
+  }
+  fr = NlFrames{(const NlBlock*)blocks_dev, batch, bin_base};
+  return 0;
+}
+
+static int nl_types_opt(const char* what, const int64_t* types, const double* rc2, int T, NlTypes& ty) {
+  if (!types && !rc2) { ty = NlTypes{}; return 0; }
+  return nl_types(what, types, rc2, T, ty);
+}
+
+extern "C" int nqb_nl_bin_frames(const double* pos, int64_t N, const void* blocks_dev, const int64_t* batch,
+                                 const int64_t* bin_base, double* wpos, int32_t* base, int64_t* bin, int32_t* cidx,
+                                 nqb_stream_t st) {
+  if (N < 0) return nqb_set_error("nqb_nl_bin_frames: negative size");
+  if (N == 0) return 0;
+  if (!pos || !wpos || !base || !bin || !cidx) return nqb_set_error("nqb_nl_bin_frames: null pointer");
+  NlFrames fr;
+  if (int rc = nl_frames("nqb_nl_bin_frames", blocks_dev, batch, bin_base, fr)) return rc;
+  k_nl_bin<NlFrames><<<(unsigned)((N + 127) / 128), 128, 0, (cudaStream_t)st>>>(fr, pos, N, wpos, base, bin, cidx);
+  return nl_launch_done();
+}
+
+extern "C" int nqb_nl_count_frames(int64_t N, const void* blocks_dev, const int64_t* batch, const int64_t* bin_base,
+                                   const double* wpos, const int32_t* cidx, const int64_t* order,
+                                   const int64_t* bin_start, const int64_t* types, const double* rc2, int T,
+                                   int64_t* counts, nqb_stream_t st) {
+  if (N <= 0) return 0;
+  if (!wpos || !cidx || !order || !bin_start || !counts) return nqb_set_error("nqb_nl_count_frames: null pointer");
+  NlFrames fr;
+  if (int rc = nl_frames("nqb_nl_count_frames", blocks_dev, batch, bin_base, fr)) return rc;
+  NlTypes ty;
+  if (int rc = nl_types_opt("nqb_nl_count_frames", types, rc2, T, ty)) return rc;
+  const unsigned blocks = (unsigned)((N + 63) / 64);
+  if (ty.types)
+    k_nl_count<NlFrames, true><<<blocks, 64, 0, (cudaStream_t)st>>>(fr, N, wpos, cidx, order, bin_start, counts, ty);
+  else
+    k_nl_count<NlFrames><<<blocks, 64, 0, (cudaStream_t)st>>>(fr, N, wpos, cidx, order, bin_start, counts, ty);
+  return nl_launch_done();
+}
+
+extern "C" int nqb_nl_fill_frames(int64_t N, int64_t E, const void* blocks_dev, const int64_t* batch,
+                                  const int64_t* bin_base, const double* wpos, const int32_t* cidx,
+                                  const int32_t* base, const int64_t* order, const int64_t* bin_start,
+                                  const int64_t* row_ptr, const int64_t* types, const double* rc2, int T,
+                                  int64_t* edge_index, double* shifts, nqb_stream_t st) {
+  if (N <= 0 || E <= 0) return 0;
+  if (!wpos || !cidx || !base || !order || !bin_start || !row_ptr || !edge_index || !shifts)
+    return nqb_set_error("nqb_nl_fill_frames: null pointer");
+  NlFrames fr;
+  if (int rc = nl_frames("nqb_nl_fill_frames", blocks_dev, batch, bin_base, fr)) return rc;
+  NlTypes ty;
+  if (int rc = nl_types_opt("nqb_nl_fill_frames", types, rc2, T, ty)) return rc;
+  const unsigned blocks = (unsigned)((N + 63) / 64);
+  const double3 zero = make_double3(0.0, 0.0, 0.0);
+  if (ty.types)
+    k_nl_fill<false, NlFrames, true><<<blocks, 64, 0, (cudaStream_t)st>>>(
+        fr, N, wpos, cidx, base, order, bin_start, row_ptr, E, edge_index, shifts, nullptr, zero, ty);
+  else
+    k_nl_fill<false, NlFrames><<<blocks, 64, 0, (cudaStream_t)st>>>(
+        fr, N, wpos, cidx, base, order, bin_start, row_ptr, E, edge_index, shifts, nullptr, zero, ty);
   return nl_launch_done();
 }

@@ -52,8 +52,10 @@ struct ZblParams {
   int T;
 };
 
-__device__ __forceinline__ void edge_vector(const ZblGeom& g, int64_t e, int64_t i0, int64_t i1, double& vx,
-                                            double& vy, double& vz) {
+// kFramed (nqb_zbl_*_frames): g.cell is [F, 3, 3] and edge e takes the cell of its centre's frame, frame[i0]
+template <bool kFramed>
+__device__ __forceinline__ void edge_vector(const ZblGeom& g, int64_t e, int64_t i0, int64_t i1,
+                                            const int64_t* __restrict__ frame, double& vx, double& vy, double& vz) {
   if (g.vec != nullptr) {
     vx = g.vec[3 * e]; vy = g.vec[3 * e + 1]; vz = g.vec[3 * e + 2];
     return;
@@ -64,7 +66,7 @@ __device__ __forceinline__ void edge_vector(const ZblGeom& g, int64_t e, int64_t
   vz = g.pos[3 * i1 + 2] - g.pos[3 * i0 + 2];
   if (g.shift != nullptr && g.cell != nullptr) {
     const double s0 = g.shift[3 * e], s1 = g.shift[3 * e + 1], s2 = g.shift[3 * e + 2];
-    const double* c = g.cell;
+    const double* c = kFramed ? g.cell + 9 * frame[i0] : g.cell;
     vx += s0 * c[0] + s1 * c[3] + s2 * c[6];
     vy += s0 * c[1] + s1 * c[4] + s2 * c[7];
     vz += s0 * c[2] + s1 * c[5] + s2 * c[8];
@@ -101,10 +103,11 @@ __device__ __forceinline__ double zbl_edge(double r, double A, double S, const Z
   return A * inv_r * psi * fc;
 }
 
-template <bool kTyped = false>
+template <bool kTyped = false, bool kFramed = false>
 __global__ void k_zbl_fwd(ZblGeom g, ZblParams q, const int64_t* __restrict__ types, const double* __restrict__ table,
                           const int64_t* __restrict__ row_ptr, const int64_t* __restrict__ perm, int64_t N,
-                          double* __restrict__ e_atom, const double* __restrict__ recip) {
+                          double* __restrict__ e_atom, const double* __restrict__ recip,
+                          const int64_t* __restrict__ frame) {
   const int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= N) return;  // uniform over the warp
@@ -118,7 +121,7 @@ __global__ void k_zbl_fwd(ZblGeom g, ZblParams q, const int64_t* __restrict__ ty
       const int64_t e = perm ? perm[n] : n;
       const int64_t i0 = g.eidx[e], i1 = g.eidx[g.E + e];
       double vx, vy, vz;
-      edge_vector(g, e, i0, i1, vx, vy, vz);
+      edge_vector<kFramed>(g, e, i0, i1, frame, vx, vy, vz);
       const double r = sqrt(vx * vx + vy * vy + vz * vz);
       const int64_t tt = ti * q.T + types[i1];
       const double* t = table + 2 * tt;
@@ -130,15 +133,15 @@ __global__ void k_zbl_fwd(ZblGeom g, ZblParams q, const int64_t* __restrict__ ty
   if (lane == 0) e_atom[row] = s;
 }
 
-template <bool kTyped = false>
+template <bool kTyped = false, bool kFramed = false>
 __global__ void k_zbl_bwd(ZblGeom g, ZblParams q, const int64_t* __restrict__ types, const double* __restrict__ table,
                           const double* __restrict__ grad_e, double* __restrict__ gpos, double* __restrict__ gvec,
-                          const double* __restrict__ recip) {
+                          const double* __restrict__ recip, const int64_t* __restrict__ frame) {
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= g.E) return;
   const int64_t i0 = g.eidx[e], i1 = g.eidx[g.E + e];
   double vx, vy, vz;
-  edge_vector(g, e, i0, i1, vx, vy, vz);
+  edge_vector<kFramed>(g, e, i0, i1, frame, vx, vy, vz);
   const double r = sqrt(vx * vx + vy * vy + vz * vz);
   const int64_t tt = types[i0] * q.T + types[i1];
   const double* t = table + 2 * tt;
@@ -185,7 +188,7 @@ extern "C" int nqb_zbl_fwd(const double* pos, const int64_t* edge_index, const d
   ZblGeom g{pos, edge_index, shift, cell, vec, E};
   ZblParams q{r_max, poly_p, cutoff_f32 ? 1 : 0, T};
   const unsigned blocks = (unsigned)((N + 3) / 4);  // 4 rows (warps) per 128-thread block
-  k_zbl_fwd<<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, row_ptr, perm, N, e_atom, nullptr);
+  k_zbl_fwd<<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, row_ptr, perm, N, e_atom, nullptr, nullptr);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -204,7 +207,7 @@ extern "C" int nqb_zbl_bwd(const double* pos, const int64_t* edge_index, const d
   ZblGeom g{pos, edge_index, shift, cell, vec, E};
   ZblParams q{r_max, poly_p, cutoff_f32 ? 1 : 0, T};
   const unsigned blocks = (unsigned)((E + 127) / 128);
-  k_zbl_bwd<<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, grad_e_atom, grad_pos, grad_vec, nullptr);
+  k_zbl_bwd<<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, grad_e_atom, grad_pos, grad_vec, nullptr, nullptr);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -225,7 +228,7 @@ extern "C" int nqb_zbl_fwd_typed(const double* pos, const int64_t* edge_index, c
   ZblGeom g{pos, edge_index, shift, cell, vec, E};
   ZblParams q{r_max, poly_p, cutoff_f32 ? 1 : 0, T};
   const unsigned blocks = (unsigned)((N + 3) / 4);
-  k_zbl_fwd<true><<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, row_ptr, perm, N, e_atom, recip);
+  k_zbl_fwd<true><<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, row_ptr, perm, N, e_atom, recip, nullptr);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
@@ -246,7 +249,62 @@ extern "C" int nqb_zbl_bwd_typed(const double* pos, const int64_t* edge_index, c
   ZblGeom g{pos, edge_index, shift, cell, vec, E};
   ZblParams q{r_max, poly_p, cutoff_f32 ? 1 : 0, T};
   const unsigned blocks = (unsigned)((E + 127) / 128);
-  k_zbl_bwd<true><<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, grad_e_atom, grad_pos, grad_vec, recip);
+  k_zbl_bwd<true><<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, grad_e_atom, grad_pos, grad_vec, recip, nullptr);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+// A batch of frames: as nqb_zbl_fwd / nqb_zbl_bwd on positions with cells [F, 3, 3] (device) and frame [N] i64 (the
+// frame of each atom); edge e takes the cell of frame[edge_index[0][e]].  Per-edge-type cutoffs when recip is given
+// (as nqb_zbl_*_typed), none when it is NULL.
+extern "C" int nqb_zbl_fwd_frames(const double* pos, const int64_t* edge_index, const double* shift,
+                                  const double* cells, const int64_t* frame, const int64_t* types, const double* table,
+                                  int T, const int64_t* row_ptr, const int64_t* perm, int64_t N, int64_t E,
+                                  double r_max, double poly_p, int cutoff_f32, const double* recip, double* e_atom,
+                                  nqb_stream_t st) {
+  if (int rc = check_common("nqb_zbl_fwd_frames", pos, edge_index, shift, cells, nullptr, types, table, T, N, E, r_max,
+                            poly_p))
+    return rc;
+  if (N == 0) return 0;
+  if (!row_ptr || !e_atom) return nqb_set_error("nqb_zbl_fwd_frames: null row_ptr / e_atom");
+  if (E > 0 && (!shift || !frame)) return nqb_set_error("nqb_zbl_fwd_frames: null shift / cells / frame");
+  ZblGeom g{pos, edge_index, shift, cells, nullptr, E};
+  ZblParams q{r_max, poly_p, cutoff_f32 ? 1 : 0, T};
+  const unsigned blocks = (unsigned)((N + 3) / 4);
+  if (recip)
+    k_zbl_fwd<true, true><<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, row_ptr, perm, N, e_atom, recip,
+                                                                 frame);
+  else
+    k_zbl_fwd<false, true><<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, row_ptr, perm, N, e_atom, recip,
+                                                                  frame);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int nqb_zbl_bwd_frames(const double* pos, const int64_t* edge_index, const double* shift,
+                                  const double* cells, const int64_t* frame, const int64_t* types, const double* table,
+                                  int T, int64_t N, int64_t E, double r_max, double poly_p, int cutoff_f32,
+                                  const double* recip, const double* grad_e_atom, double* grad_pos, double* grad_vec,
+                                  nqb_stream_t st) {
+  if (int rc = check_common("nqb_zbl_bwd_frames", pos, edge_index, shift, cells, nullptr, types, table, T, N, E, r_max,
+                            poly_p))
+    return rc;
+  if (E == 0) return 0;
+  if (!grad_e_atom || (!grad_pos && !grad_vec)) return nqb_set_error("nqb_zbl_bwd_frames: null grad_e_atom / outputs");
+  if (!shift || !frame) return nqb_set_error("nqb_zbl_bwd_frames: null shift / cells / frame");
+  ZblGeom g{pos, edge_index, shift, cells, nullptr, E};
+  ZblParams q{r_max, poly_p, cutoff_f32 ? 1 : 0, T};
+  const unsigned blocks = (unsigned)((E + 127) / 128);
+  if (recip)
+    k_zbl_bwd<true, true><<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, grad_e_atom, grad_pos, grad_vec,
+                                                                 recip, frame);
+  else
+    k_zbl_bwd<false, true><<<blocks, 128, 0, (cudaStream_t)st>>>(g, q, types, table, grad_e_atom, grad_pos, grad_vec,
+                                                                  recip, frame);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));

@@ -581,10 +581,15 @@ __device__ __forceinline__ double edge_recip(const EdgeTypes& et, int64_t E, int
   return et.recip[et.T * et.types[et.tidx[e]] + et.types[et.tidx[E + e]]];
 }
 
-template <int LMAX, typename TO, bool kTyped = false>
+// kFramed (nqb_edge_embed_fwd_frames): a batch of frames, cell [F, 3, 3]; edge e takes the cell of its centre's
+// frame, cell + 9 * frame[eidx[0][e]], in the same shift expression.  Unframed variants do not read the trailing frame
+// parameter (appended, so their code is unchanged).  The backward reads the stored edge vectors only and needs no
+// framed variant.
+template <int LMAX, typename TO, bool kTyped = false, bool kFramed = false>
 __global__ void k_edge_embed_fwd(EmbedParams prm, const double* __restrict__ pos, const int64_t* __restrict__ eidx,
                                  const double* __restrict__ shift, const double* __restrict__ cell, int64_t E,
-                                 double* __restrict__ vec, TO* __restrict__ yout, TO* __restrict__ emb, EdgeTypes et) {
+                                 double* __restrict__ vec, TO* __restrict__ yout, TO* __restrict__ emb, EdgeTypes et,
+                                 const int64_t* __restrict__ frame) {
   constexpr int S = (LMAX + 1) * (LMAX + 1);
   int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
@@ -594,9 +599,10 @@ __global__ void k_edge_embed_fwd(EmbedParams prm, const double* __restrict__ pos
   double vz = pos[3 * i1 + 2] - pos[3 * i0 + 2];
   if (shift != nullptr && cell != nullptr) {
     const double s0 = shift[3 * e], s1 = shift[3 * e + 1], s2 = shift[3 * e + 2];
-    vx += s0 * cell[0] + s1 * cell[3] + s2 * cell[6];
-    vy += s0 * cell[1] + s1 * cell[4] + s2 * cell[7];
-    vz += s0 * cell[2] + s1 * cell[5] + s2 * cell[8];
+    const double* c = kFramed ? cell + 9 * frame[i0] : cell;
+    vx += s0 * c[0] + s1 * c[3] + s2 * c[6];
+    vy += s0 * c[1] + s1 * c[4] + s2 * c[7];
+    vz += s0 * c[2] + s1 * c[5] + s2 * c[8];
   }
   vec[3 * e] = vx; vec[3 * e + 1] = vy; vec[3 * e + 2] = vz;
   const double r = sqrt(vx * vx + vy * vy + vz * vz);
@@ -680,7 +686,7 @@ extern "C" int nqb_edge_embed_fwd(int lmax, int num_bessel, double r_max, double
   EmbedParams prm{num_bessel, r_max, poly_p, prefactor};
   unsigned blocks = (unsigned)((E + 127) / 128);
   cudaStream_t s = (cudaStream_t)st;
-#define EE_FWD(L, TT) k_edge_embed_fwd<L, TT><<<blocks, 128, 0, s>>>(prm, pos, edge_index, shift, cell, E, vec, (TT*)y, (TT*)emb, EdgeTypes{})
+#define EE_FWD(L, TT) k_edge_embed_fwd<L, TT><<<blocks, 128, 0, s>>>(prm, pos, edge_index, shift, cell, E, vec, (TT*)y, (TT*)emb, EdgeTypes{}, nullptr)
   if (out_dtype == NQB_F32) {
     switch (lmax) { case 0: EE_FWD(0, float); break; case 1: EE_FWD(1, float); break; case 2: EE_FWD(2, float); break; case 3: EE_FWD(3, float); break; default: EE_FWD(4, float); break; }
   } else {
@@ -743,7 +749,7 @@ extern "C" int nqb_edge_embed_fwd_typed(int lmax, int num_bessel, double r_max, 
   const EdgeTypes et{types, type_index, recip, T};
   unsigned blocks = (unsigned)((E + 127) / 128);
   cudaStream_t s = (cudaStream_t)st;
-#define EE_FWD(L, TT) k_edge_embed_fwd<L, TT, true><<<blocks, 128, 0, s>>>(prm, pos, edge_index, shift, cell, E, vec, (TT*)y, (TT*)emb, et)
+#define EE_FWD(L, TT) k_edge_embed_fwd<L, TT, true><<<blocks, 128, 0, s>>>(prm, pos, edge_index, shift, cell, E, vec, (TT*)y, (TT*)emb, et, nullptr)
   if (out_dtype == NQB_F32) {
     switch (lmax) { case 0: EE_FWD(0, float); break; case 1: EE_FWD(1, float); break; case 2: EE_FWD(2, float); break; case 3: EE_FWD(3, float); break; default: EE_FWD(4, float); break; }
   } else {
@@ -780,6 +786,45 @@ extern "C" int nqb_edge_embed_bwd_typed(int lmax, int num_bessel, double r_max, 
   }
 #undef EE_BWD
   NQB_LAUNCH_CHECK("nqb_edge_embed_bwd_typed");
+  return 0;
+}
+
+// A batch of frames: as nqb_edge_embed_fwd with cells [F, 3, 3] (device) and frame [N] i64 (the frame of each atom);
+// edge e takes the cell of frame[edge_index[0][e]].  Per-edge-type cutoffs as nqb_edge_embed_fwd_typed when types,
+// type_index and recip are given, none when all three are NULL.  The backward is nqb_edge_embed_bwd(_typed).
+extern "C" int nqb_edge_embed_fwd_frames(int lmax, int num_bessel, double r_max, double poly_p, double prefactor,
+                                         const double* pos, const int64_t* edge_index, const double* shift,
+                                         const double* cells, const int64_t* frame, int64_t N, int64_t E,
+                                         const int64_t* types, const int64_t* type_index, const double* recip, int T,
+                                         int out_dtype, double* vec, void* y, void* emb, nqb_stream_t st) {
+  (void)N;
+  if (lmax < 0 || lmax > 4) return fail("nqb_edge_embed_fwd_frames: lmax=%d unsupported (0..4)", lmax);
+  if (num_bessel < 1 || num_bessel > NQB_MAX_BESSEL) return fail("nqb_edge_embed_fwd_frames: bad num_bessel %d", num_bessel);
+  if (out_dtype != NQB_F32 && out_dtype != NQB_F64) return fail("nqb_edge_embed_fwd_frames: bad dtype");
+  if (!(r_max > 0.0) || !(poly_p >= 2.0)) return fail("nqb_edge_embed_fwd_frames: need r_max > 0 and p >= 2");
+  if (E < 0) return fail("nqb_edge_embed_fwd_frames: negative size");
+  if (E == 0) return 0;
+  if (!pos || !edge_index || !shift || !cells || !frame || !vec || !y || !emb)
+    return fail("nqb_edge_embed_fwd_frames: null pointer");
+  const bool typed = types || type_index || recip;
+  if (typed)
+    if (int rc = check_edge_types("nqb_edge_embed_fwd_frames", types, type_index, recip, T)) return rc;
+  EmbedParams prm{num_bessel, r_max, poly_p, prefactor};
+  const EdgeTypes et{types, type_index, recip, T};
+  unsigned blocks = (unsigned)((E + 127) / 128);
+  cudaStream_t s = (cudaStream_t)st;
+#define EE_FWD(L, TT)                                                                                                  \
+  (typed ? k_edge_embed_fwd<L, TT, true, true><<<blocks, 128, 0, s>>>(prm, pos, edge_index, shift, cells, E, vec,      \
+                                                                      (TT*)y, (TT*)emb, et, frame)                     \
+         : k_edge_embed_fwd<L, TT, false, true><<<blocks, 128, 0, s>>>(prm, pos, edge_index, shift, cells, E, vec,     \
+                                                                       (TT*)y, (TT*)emb, et, frame))
+  if (out_dtype == NQB_F32) {
+    switch (lmax) { case 0: EE_FWD(0, float); break; case 1: EE_FWD(1, float); break; case 2: EE_FWD(2, float); break; case 3: EE_FWD(3, float); break; default: EE_FWD(4, float); break; }
+  } else {
+    switch (lmax) { case 0: EE_FWD(0, double); break; case 1: EE_FWD(1, double); break; case 2: EE_FWD(2, double); break; case 3: EE_FWD(3, double); break; default: EE_FWD(4, double); break; }
+  }
+#undef EE_FWD
+  NQB_LAUNCH_CHECK("nqb_edge_embed_fwd_frames");
   return 0;
 }
 

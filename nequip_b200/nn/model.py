@@ -703,6 +703,15 @@ class NequIPEnergyModel(torch.nn.Module):
         return {} if self.per_edge_type_cutoff is None else dict(edge_type_recip=self.rmax_recip)
 
     @staticmethod
+    def _frame_kwargs(data: Dict[str, torch.Tensor], cell) -> dict:
+        """``batch=`` for the edge embedding and ZBL when a batch comes with one cell per frame ([F, 3, 3], F > 1);
+        {} otherwise, so that a single frame and frames sharing one cell take the single-cell kernels."""
+        batch = data.get(BATCH_KEY)
+        if batch is None or cell is None or cell.dim() != 3 or cell.shape[0] == 1:
+            return {}
+        return dict(batch=batch)
+
+    @staticmethod
     def _reduce_energy(e_atom: torch.Tensor, data: Dict[str, torch.Tensor]) -> torch.Tensor:
         """AtomwiseReduce (atomwise.py:92-113): per-graph sum -> [num_graphs, 1]; one frame without ``batch``."""
         batch = data.get(BATCH_KEY)
@@ -742,7 +751,7 @@ class NequIPEnergyModel(torch.nn.Module):
             _vec, edge_attrs, edge_embedding = ops.edge_embed(
                 pos, edge_index, shift, cell, lmax=self.l_max, num_bessel=self.num_bessels, r_max=self.r_max,
                 poly_p=self.poly_p, prefactor=pre, out_dtype=self.model_dtype, edge_grad_sink=sink,
-                **self._edge_type_kwargs(types))
+                **self._edge_type_kwargs(types), **self._frame_kwargs(data, cell))
         pairs = self._edge_pairs(edge_index, None if EDGE_VECTORS_KEY in data else shift, edge_embedding, types.numel())
         for layer in self.layers:
             x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight, pairs=pairs)
@@ -757,7 +766,8 @@ class NequIPEnergyModel(torch.nn.Module):
                                              **self._pair_kwargs())
             else:
                 e_pair = self.pair_potential(types, edge_index, self.r_max, pos=pos, shift=shift, cell=cell,
-                                             edge_grad_sink=sink, **self._pair_kwargs())
+                                             edge_grad_sink=sink, **self._pair_kwargs(),
+                                             **self._frame_kwargs(data, cell))
             e_atom = e_atom + e_pair
         data[PER_ATOM_ENERGY_KEY] = e_atom
         data[TOTAL_ENERGY_KEY] = self._reduce_energy(e_atom, data)
@@ -793,13 +803,30 @@ class NequIPEnergyModel(torch.nn.Module):
                                                   **self._pair_kwargs())[:n_own]
         return e_atom
 
+    @staticmethod
+    def _frame_stress(vec: torch.Tensor, g_edge: torch.Tensor, data: Dict[str, torch.Tensor]):
+        """(stress, virial) [F, 3, 3] of a batch: dE/d(eps_f) = sym(sum over the edges e whose centre is in frame f of
+        r_e (x) g_e), divided by |det cell_f| (one cell serves every frame).  F is the row count of the energy."""
+        F = data[TOTAL_ENERGY_KEY].shape[0]
+        cell = data[CELL_KEY].double().reshape(-1, 3, 3)
+        if cell.shape[0] not in (1, F):
+            raise ValueError(f"compute_stress: {cell.shape[0]} cells for {F} frames")
+        frame_e = data[BATCH_KEY].view(-1).long()[data[EDGE_INDEX_KEY][0].long()]
+        rg = (vec.unsqueeze(2) * g_edge.unsqueeze(1)).reshape(-1, 9)
+        v = torch.zeros((F, 9), dtype=torch.float64, device=vec.device).index_add_(0, frame_e, rg).view(F, 3, 3)
+        v = 0.5 * (v + v.transpose(1, 2))
+        vol = torch.linalg.det(cell).abs().view(-1, 1, 1)
+        return v / vol, torch.neg(v)
+
     def forward(self, data: Dict[str, torch.Tensor], compute_forces: bool = True,
                 compute_stress: bool = False) -> Dict[str, torch.Tensor]:
         """``ForceStressOutput.forward`` (nequip/nn/grad_output.py:107-298):
 
         * positions given: ``forces = -dE/dpos``; with ``compute_stress`` (needs ``cell``) also
           ``stress = (1/|det cell|) dE/d(eps)`` and ``virial = -dE/d(eps)`` ([1,3,3]) for the symmetric strain
-          ``eps`` applied to positions and cell.  The cell/strain gradient is not taken through a displaced
+          ``eps`` applied to positions and cell.  With ``batch`` (a batch of frames, ``cell`` [F,3,3] or one cell for
+          all) each frame has its own strain: ``stress`` and ``virial`` are [F,3,3], frame f sums the edges whose
+          centre is in f and divides by its own ``|det cell_f|`` (grad_output.py:117-260).  The cell/strain gradient is not taken through a displaced
           copy of the inputs: every edge vector transforms as ``r -> r (1 + eps)``, so
           ``dE/d(eps) = sym( sum_e r_e (x) dE/dr_e )`` and the per-edge gradients are a by-product of the
           edge-embedding backward kernel;
@@ -836,11 +863,14 @@ class NequIPEnergyModel(torch.nn.Module):
             g_edge = sink["edge_vector_grad"]
             if "pair_edge_vector_grad" in sink:  # the pair potential's share of dE/d(edge vector)
                 g_edge = g_edge + sink["pair_edge_vector_grad"]
-            v = torch.einsum("ea,eb->ab", sink["edge_vectors"], g_edge)
-            v = 0.5 * (v + v.t())
-            vol = torch.linalg.det(data[CELL_KEY].double().view(3, 3)).abs()
-            data[STRESS_KEY] = (v / vol).view(1, 3, 3)
-            data[VIRIAL_KEY] = torch.neg(v).view(1, 3, 3)
+            if data.get(BATCH_KEY) is None:
+                v = torch.einsum("ea,eb->ab", sink["edge_vectors"], g_edge)
+                v = 0.5 * (v + v.t())
+                vol = torch.linalg.det(data[CELL_KEY].double().view(3, 3)).abs()
+                data[STRESS_KEY] = (v / vol).view(1, 3, 3)
+                data[VIRIAL_KEY] = torch.neg(v).view(1, 3, 3)
+            else:
+                data[STRESS_KEY], data[VIRIAL_KEY] = self._frame_stress(sink["edge_vectors"], g_edge, data)
         data[POSITIONS_KEY] = pos.detach()
         data[TOTAL_ENERGY_KEY] = data[TOTAL_ENERGY_KEY].detach()
         data[PER_ATOM_ENERGY_KEY] = data[PER_ATOM_ENERGY_KEY].detach()

@@ -456,14 +456,23 @@ def spherical_harmonics(vec: torch.Tensor, lmax: int, out_dtype=torch.float32) -
 class _EdgeEmbedFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pos, edge_index, shift, cell, lmax, num_bessel, r_max, poly_p, prefactor, out_dtype, sink=None,
-                types=None, recip=None):
+                types=None, recip=None, frame=None):
         L = _capi.lib()
         N, E = pos.shape[0], edge_index.shape[1]
         dev = pos.device
         vec = torch.empty((E, 3), dtype=torch.float64, device=dev)
         y = torch.empty((E, (lmax + 1) ** 2), dtype=out_dtype, device=dev)
         emb = torch.empty((E, num_bessel), dtype=out_dtype, device=dev)
-        if recip is None:
+        if frame is not None:
+            _capi.check(
+                L.nqb_edge_embed_fwd_frames(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(pos), _ptr(edge_index),
+                                            _ptr(shift), _ptr(cell), _ptr(frame), N, E, _ptr(types),
+                                            0 if recip is None else _ptr(edge_index), _ptr(recip),
+                                            0 if recip is None else _edge_type_count(recip), _DT[out_dtype], _ptr(vec),
+                                            _ptr(y), _ptr(emb), _stream()),
+                "nqb_edge_embed_fwd_frames",
+            )
+        elif recip is None:
             _capi.check(
                 L.nqb_edge_embed_fwd(lmax, num_bessel, r_max, poly_p, prefactor, _ptr(pos), _ptr(edge_index), _ptr(shift),
                                      _ptr(cell), N, E, _DT[out_dtype], _ptr(vec), _ptr(y), _ptr(emb), _stream()),
@@ -511,7 +520,7 @@ class _EdgeEmbedFn(torch.autograd.Function):
             )
         if ctx.sink is not None:
             ctx.sink["edge_vectors"], ctx.sink["edge_vector_grad"] = vec, gvec
-        return gpos, None, None, None, None, None, None, None, None, None, None, None, None
+        return gpos, None, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 class _EdgeEmbedVecFn(torch.autograd.Function):
@@ -615,9 +624,31 @@ def edge_embed_from_vectors(vec, *, lmax: int, num_bessel: int = 8, r_max: float
                                  float(prefactor), out_dtype, types, None if recip is None else edge_index, recip)
 
 
+def _frame_cells(cell, batch, num_atoms: int, what: str):
+    """(cells [F, 3, 3] f64, frame [N] i64) of a batch of frames for the ``_frames`` kernels; ``ValueError`` for a
+    malformed ``batch`` or a frame index outside [0, F) (one host synchronisation)."""
+    _require_cuda(cell, batch)
+    if cell.dim() != 3 or tuple(cell.shape[1:]) != (3, 3):
+        raise ValueError(f"{what}: cell must be [F, 3, 3] with batch, got {tuple(cell.shape)}")
+    frame = batch.view(-1).long().contiguous()
+    if frame.numel() != num_atoms:
+        raise ValueError(f"{what}: batch must hold {num_atoms} frame indices, got {frame.numel()}")
+    if num_atoms:
+        lo, hi = (int(v) for v in torch.aminmax(frame))
+        if lo < 0 or hi >= cell.shape[0]:
+            raise ValueError(f"{what}: batch holds frame indices outside [0, {cell.shape[0]})")
+    return cell.double().contiguous(), frame
+
+
+def _framed(cell, batch) -> bool:
+    """Whether a call takes the ``_frames`` kernels: a batch with more than one cell.  One cell ([3, 3] or [1, 3, 3])
+    serves every edge as it does without a batch."""
+    return batch is not None and cell is not None and cell.dim() == 3 and cell.shape[0] > 1
+
+
 def edge_embed(pos, edge_index, shift=None, cell=None, *, lmax: int, num_bessel: int = 8, r_max: float,
                poly_p: float = 6.0, prefactor: float = 1.0, out_dtype=torch.float32, edge_grad_sink=None,
-               types=None, edge_type_recip=None):
+               types=None, edge_type_recip=None, batch=None):
     """Edge vectors, harmonics and Bessel x cutoff embedding in one kernel.
 
     Returns ``(edge_vectors [E,3] f64, edge_attrs [E,(lmax+1)^2], edge_embedding [E,num_bessel])``.
@@ -625,16 +656,26 @@ def edge_embed(pos, edge_index, shift=None, cell=None, *, lmax: int, num_bessel:
     edge vectors and dE/d(edge vector) in it, from which the virial / cell gradient follows.
     ``types`` [N] + ``edge_type_recip`` [T * T] f64: per-edge-type cutoffs, the normalised length of edge e is
     ``r_e * edge_type_recip[T * types[edge_index[0, e]] + types[edge_index[1, e]]]`` instead of ``r_e / r_max``
-    (``prefactor`` is the caller's)."""
+    (``prefactor`` is the caller's).
+    A batch of frames: ``cell`` [F, 3, 3] with ``batch`` [N] (the frame of each atom); edge e takes the cell of frame
+    ``batch[edge_index[0, e]]`` (nequip/nn/utils.py:96-106) and its outputs are bitwise those of a call on its frame
+    alone.  A single cell with or without ``batch`` takes the single-cell kernels."""
     _require_cuda(pos, edge_index)
     pos = pos.double().contiguous()
     edge_index = edge_index.long().contiguous()
     if (shift is None) != (cell is None):
         raise ValueError("shift and cell must be given together")
+    frame = None
     if shift is not None:
         shift = shift.double().contiguous()
-        cell = cell.double().reshape(3, 3).contiguous()
+        if _framed(cell, batch):
+            cell, frame = _frame_cells(cell, batch, pos.shape[0], "edge_embed")
+        else:
+            cell = cell.double().reshape(3, 3).contiguous()
     types, recip = _edge_type_args(types, edge_type_recip, "edge_embed")
+    if frame is not None:
+        return _EdgeEmbedFn.apply(pos, edge_index, shift, cell, int(lmax), int(num_bessel), float(r_max),
+                                  float(poly_p), float(prefactor), out_dtype, edge_grad_sink, types, recip, frame)
     if recip is None:
         return _EdgeEmbedFn.apply(pos, edge_index, shift, cell, int(lmax), int(num_bessel), float(r_max),
                                   float(poly_p), float(prefactor), out_dtype, edge_grad_sink)
@@ -648,12 +689,19 @@ def edge_embed(pos, edge_index, shift=None, cell=None, *, lmax: int, num_bessel:
 class _ZBLFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, geom, edge_index, shift, cell, types, table, r_max, poly_p, cutoff_f32, from_vectors, sink,
-                recip=None):
+                recip=None, frame=None):
         N, E, T = types.numel(), edge_index.shape[1], table.shape[0]
         csr = csr_cache.get(edge_index[0], N)  # the CSR the first interaction layer already built
         pos, vec = (None, geom) if from_vectors else (geom, None)
         e_atom = torch.empty((N, 1), dtype=torch.float64, device=types.device)
-        if recip is None:
+        if frame is not None:
+            _capi.check(
+                _capi.lib().nqb_zbl_fwd_frames(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(frame),
+                                               _ptr(types), _ptr(table), T, _ptr(csr.row_ptr), _ptr(csr.perm), N, E,
+                                               r_max, poly_p, int(cutoff_f32), _ptr(recip), _ptr(e_atom), _stream()),
+                "nqb_zbl_fwd_frames",
+            )
+        elif recip is None:
             _capi.check(
                 _capi.lib().nqb_zbl_fwd(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(vec), _ptr(types),
                                         _ptr(table), T, _ptr(csr.row_ptr), _ptr(csr.perm), N, E, r_max, poly_p,
@@ -669,13 +717,13 @@ class _ZBLFn(torch.autograd.Function):
             )
         ctx.args = (r_max, poly_p, cutoff_f32, from_vectors)
         ctx.sink = sink
-        ctx.save_for_backward(geom, edge_index, shift, cell, types, table, recip)
+        ctx.save_for_backward(geom, edge_index, shift, cell, types, table, recip, frame)
         return e_atom
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, ge):
-        geom, edge_index, shift, cell, types, table, recip = ctx.saved_tensors
+        geom, edge_index, shift, cell, types, table, recip, frame = ctx.saved_tensors
         r_max, poly_p, cutoff_f32, from_vectors = ctx.args
         N, E = types.numel(), edge_index.shape[1]
         pos, vec = (None, geom) if from_vectors else (geom, None)
@@ -683,7 +731,15 @@ class _ZBLFn(torch.autograd.Function):
         gvec = torch.empty((E, 3), dtype=torch.float64, device=geom.device) \
             if from_vectors or ctx.sink is not None else None
         ge = ge.to(torch.float64).contiguous()
-        if recip is None:
+        if frame is not None:
+            _capi.check(
+                _capi.lib().nqb_zbl_bwd_frames(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(frame),
+                                               _ptr(types), _ptr(table), table.shape[0], N, E, r_max, poly_p,
+                                               int(cutoff_f32), _ptr(recip), _ptr(ge), _ptr(gpos), _ptr(gvec),
+                                               _stream()),
+                "nqb_zbl_bwd_frames",
+            )
+        elif recip is None:
             _capi.check(
                 _capi.lib().nqb_zbl_bwd(_ptr(pos), _ptr(edge_index), _ptr(shift), _ptr(cell), _ptr(vec), _ptr(types),
                                         _ptr(table), table.shape[0], N, E, r_max, poly_p, int(cutoff_f32), _ptr(ge),
@@ -700,11 +756,11 @@ class _ZBLFn(torch.autograd.Function):
         if ctx.sink is not None:
             # kept apart from the edge embedding's gradient: the stress assembly adds the two once both backwards ran
             ctx.sink["pair_edge_vector_grad"] = gvec
-        return (gvec if from_vectors else gpos), None, None, None, None, None, None, None, None, None, None, None
+        return (gvec if from_vectors else gpos), None, None, None, None, None, None, None, None, None, None, None, None
 
 
 def zbl_energy(pos, edge_index, types, table, *, shift=None, cell=None, edge_vectors=None, r_max: float,
-               poly_p: float = 6.0, cutoff_dtype=torch.float64, edge_grad_sink=None, edge_type_recip=None):
+               poly_p: float = 6.0, cutoff_dtype=torch.float64, edge_grad_sink=None, edge_type_recip=None, batch=None):
     """ZBL per-atom energies ``[N, 1]`` f64 (``N = types.numel()``), summed onto the centre ``edge_index[0]``.
 
     ``table`` [T, T, 2] f64 holds ``0.5 * qqr2e * Z_i Z_j`` and ``Z_i^0.23 + Z_j^0.23`` per ordered type pair
@@ -713,7 +769,8 @@ def zbl_energy(pos, edge_index, types, table, *, shift=None, cell=None, edge_vec
     ``cutoff_dtype=torch.float32`` rounds the cutoff as a float32 model does.  ``edge_grad_sink`` (a dict): the backward
     pass also stores dE/d(edge vector) in it under ``pair_edge_vector_grad``.  ``edge_type_recip`` [T * T] f64
     (``1 / rc[source, target]``): per-edge-type cutoffs, the envelope takes ``r * edge_type_recip[T * t_i + t_j]``
-    instead of ``r / r_max``."""
+    instead of ``r / r_max``.  ``cell`` [F, 3, 3] with ``batch`` [N]: a batch of frames, edge e takes the cell of frame
+    ``batch[edge_index[0, e]]`` (as ``edge_embed``)."""
     _require_cuda(edge_index, types, table)
     edge_index = edge_index.long().contiguous()
     types = types.view(-1).long().contiguous()
@@ -736,16 +793,25 @@ def zbl_energy(pos, edge_index, types, table, *, shift=None, cell=None, edge_vec
         geom, from_vectors = pos.double().contiguous(), False
         if geom.shape != (types.numel(), 3):
             raise ValueError(f"zbl_energy: pos must be [{types.numel()}, 3], got {tuple(geom.shape)}")
-        if shift is not None:
-            shift = shift.double().contiguous()
+    frame = None
+    if shift is not None:
+        shift = shift.double().contiguous()
+        if _framed(cell, batch):
+            cell, frame = _frame_cells(cell, batch, types.numel(), "zbl_energy")
+        else:
             cell = cell.double().reshape(3, 3).contiguous()
+    recip = None
+    if edge_type_recip is not None:
+        _require_cuda(edge_type_recip)
+        recip = edge_type_recip.to(torch.float64).reshape(-1).contiguous()
+        if recip.numel() != table.shape[0] * table.shape[0]:
+            raise ValueError(f"zbl_energy: edge_type_recip must hold T * T = {table.shape[0] ** 2} values")
+    if frame is not None:
+        return _ZBLFn.apply(geom, edge_index, shift, cell, types, table, float(r_max), float(poly_p),
+                            cutoff_dtype == torch.float32, from_vectors, edge_grad_sink, recip, frame)
     if edge_type_recip is None:
         return _ZBLFn.apply(geom, edge_index, shift, cell, types, table, float(r_max), float(poly_p),
                             cutoff_dtype == torch.float32, from_vectors, edge_grad_sink)
-    _require_cuda(edge_type_recip)
-    recip = edge_type_recip.to(torch.float64).reshape(-1).contiguous()
-    if recip.numel() != table.shape[0] * table.shape[0]:
-        raise ValueError(f"zbl_energy: edge_type_recip must hold T * T = {table.shape[0] ** 2} values")
     return _ZBLFn.apply(geom, edge_index, shift, cell, types, table, float(r_max), float(poly_p),
                         cutoff_dtype == torch.float32, from_vectors, edge_grad_sink, recip)
 
@@ -1184,7 +1250,7 @@ def _nl_rows(pos: torch.Tensor, a: _NlArgs, s: Dict[str, torch.Tensor],
 
 
 def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, transpose_perm: bool = False,
-                  atom_types=None, edge_type_cutoff=None):
+                  atom_types=None, edge_type_cutoff=None, batch=None):
     """Full neighbour list within ``r_max`` built on the GPU (cell list), in the layout the convolution wants.
 
     ``pos`` [N,3] float64 CUDA; ``cell`` [3,3] (rows = lattice vectors; host or device) or None; ``pbc`` bool or 3
@@ -1196,9 +1262,19 @@ def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, tr
     the home image.  One host synchronisation (the edge count); ``NeighborListPlan`` has none.
 
     Per-edge-type cutoffs: ``edge_type_cutoff`` [T, T] (``rc[source, target]``, 0 < rc <= r_max) with ``atom_types``
-    [N] keeps the pair (i, j) when ``d2 < rc[t_i, t_j]^2`` (``rc * rc`` in float64); the bins are those of ``r_max``."""
+    [N] keeps the pair (i, j) when ``d2 < rc[t_i, t_j]^2`` (``rc * rc`` in float64); the bins are those of ``r_max``.
+
+    A batch of independent frames (``batch`` [N] int, the frame of each atom, non-decreasing): ``cell`` [F, 3, 3] or
+    None (every frame open), ``pbc`` a bool, [3] or [F, 3]; F is the number of cells, else of ``pbc`` rows, else
+    ``batch.max() + 1``, and a frame may hold no atoms.  The result is the concatenation over frames of the single-frame
+    lists, bit for bit, with atom indices offset by each frame's first atom (``row_ptr`` [N+1] over all atoms).  A frame
+    open in every direction takes the identity cell, whatever its row of ``cell`` holds.  One set of launches for all
+    frames; host synchronisations for the checks of ``batch``, one read-back of the per-frame atom counts and bounding
+    boxes, and the edge count."""
     import numpy as np
 
+    if batch is not None:
+        return _neighbor_list_frames(pos, cell, pbc, r_max, transpose_perm, atom_types, edge_type_cutoff, batch)
     _require_cuda(pos)
     L = _capi.lib()
     pos = pos.detach().double().contiguous()
@@ -1239,6 +1315,126 @@ def neighbor_list(pos: torch.Tensor, cell=None, pbc=True, r_max: float = 5.0, tr
                                         _ptr(shifts), _stream()), "nqb_nl_fill_typed")
     out = {"edge_index": edge_index, "edge_cell_shift": shifts, "row_ptr": row_ptr}
     if transpose_perm:
+        out["edge_transpose_perm"] = torch.argsort(edge_index[1] * N + edge_index[0], stable=True)
+    return out
+
+
+def _nl_frame_args(cell, pbc, batch, num_atoms: int):
+    """Host checks of a batched ``neighbor_list``: (F, pbc [F, 3] bool, cells [F, 3, 3] float64) with the identity
+    as the cell of a frame open in every direction.  ``ValueError`` for a ``batch`` that is not [N] integers or
+    decreases or leaves [0, F), a cell that is not [F, 3, 3], a ``pbc`` of another shape or row count, and a periodic
+    frame without a cell."""
+    import numpy as np
+
+    b = torch.as_tensor(batch)
+    if b.dim() != 1 or b.numel() != num_atoms or b.dtype.is_floating_point or b.dtype == torch.bool:
+        raise ValueError(f"neighbor_list: batch must be [{num_atoms}] integers, got {tuple(b.shape)} {b.dtype}")
+    if num_atoms > 1 and bool((b[1:] < b[:-1]).any()):
+        raise ValueError("neighbor_list: batch must be non-decreasing (each frame is one contiguous range of atoms)")
+    F = None
+    if cell is not None:
+        c = cell.detach().cpu().double().numpy() if torch.is_tensor(cell) else np.asarray(cell, dtype=np.float64)
+        if c.ndim != 3 or c.shape[1:] != (3, 3):
+            raise ValueError(f"neighbor_list: with batch, cell must be [F, 3, 3], got {tuple(c.shape)}")
+        F = c.shape[0]
+    p = pbc.detach().cpu().numpy() if torch.is_tensor(pbc) else np.asarray(pbc)
+    if p.shape == ():
+        p = np.full(3, bool(p))
+    if p.shape == (3,):
+        if F is None:
+            F = int(b.max()) + 1 if num_atoms else 0
+        p = np.broadcast_to(p, (F, 3))
+    elif p.ndim == 2 and p.shape[1] == 3:
+        if F is not None and p.shape[0] != F:
+            raise ValueError(f"neighbor_list: pbc has {p.shape[0]} rows for {F} cells")
+        F = p.shape[0]
+    else:
+        raise ValueError(f"neighbor_list: with batch, pbc must be a bool, [3] or [F, 3], got shape {tuple(p.shape)}")
+    p = p.astype(bool)
+    if cell is None:
+        if p.any():
+            raise ValueError("Periodic boundary conditions requested but no cell was provided.")
+        c = np.zeros((F, 3, 3))
+    if num_atoms and (int(b.min()) < 0 or int(b.max()) >= F):
+        raise ValueError(f"neighbor_list: batch holds frame indices outside [0, {F})")
+    c = c.copy()
+    c[~p.any(axis=1)] = np.eye(3)  # an open frame's edges do not depend on its cell (nvalchemiops uses the identity)
+    return F, p, c
+
+
+def _neighbor_list_frames(pos, cell, pbc, r_max, transpose_perm, atom_types, edge_type_cutoff, batch):
+    """``neighbor_list`` of a batch of frames: the ``_NlArgs`` of each frame as the single-frame call builds them,
+    packed into one device block per frame (``nqb_nl_frames_pack``), and one bin / sort / count / scan / fill over
+    all frames with each frame's bins at ``bin_base[f]`` of one global range."""
+    import numpy as np
+
+    N = pos.shape[0]
+    F, pbc_np, cells = _nl_frame_args(cell, pbc, batch, N)
+    _require_cuda(pos)
+    L = _capi.lib()
+    pos = pos.detach().double().contiguous()
+    dev = pos.device
+    frame = torch.as_tensor(batch).to(device=dev, dtype=torch.int64).contiguous()
+    invs = np.linalg.inv(cells) if F else np.zeros((0, 3, 3))
+    # per-frame atom counts and, for frames with an open direction, the bounding box of the fractional coordinates:
+    # one segmented min / max on the device and one read-back
+    stats = torch.bincount(frame, minlength=F).double().view(F, 1)
+    if N and not pbc_np.all():
+        frac = torch.bmm(pos.view(N, 1, 3), torch.as_tensor(invs, device=dev)[frame]).view(N, 3)
+        idx = frame.view(N, 1).expand(N, 3)
+        fmin = torch.full((F, 3), float("inf"), dtype=torch.float64, device=dev).scatter_reduce(0, idx, frac, "amin")
+        fmax = torch.full((F, 3), float("-inf"), dtype=torch.float64, device=dev).scatter_reduce(0, idx, frac, "amax")
+        stats = torch.cat([stats, fmin, fmax], 1)
+    host = stats.cpu().numpy()
+    I3, D9, D3 = C.c_int * (3 * F), C.c_double * (9 * F), C.c_double * (3 * F)
+    cols = {k: [] for k in ("pbc", "nb", "sr", "lo", "width")}
+    nbins = [0]
+    for f in range(F):
+        nf = int(host[f, 0])
+        lo, width = np.zeros(3), np.ones(3)
+        if not pbc_np[f].all() and nf > 0:
+            for d in range(3):
+                if not pbc_np[f, d]:
+                    lo[d], width[d] = host[f, 1 + d], max(host[f, 4 + d] - host[f, 1 + d], 1e-9) * (1 + 1e-9)
+        a = _NlArgs(nf, cells[f], invs[f], [bool(v) for v in pbc_np[f]], r_max, lo, width)
+        for k in cols:
+            cols[k].extend(getattr(a, k))
+        nbins.append(a.nbins)
+    bin_base = np.cumsum(nbins)
+    block_bytes = int(L.nqb_nl_params_bytes())
+    blocks = C.create_string_buffer(max(1, F * block_bytes))
+    _capi.check(L.nqb_nl_frames_pack(F, D9(*cells.reshape(-1)), D9(*invs.reshape(-1)), I3(*cols["pbc"]),
+                                     I3(*cols["nb"]), I3(*cols["sr"]), D3(*cols["lo"]), D3(*cols["width"]),
+                                     float(r_max), blocks), "nqb_nl_frames_pack")
+    blocks_dev = torch.frombuffer(bytearray(blocks.raw), dtype=torch.uint8).to(dev)
+    bin_base_dev = torch.as_tensor(bin_base, dtype=torch.int64).to(dev)
+    ty = None
+    if edge_type_cutoff is not None:
+        ty = _NlTypes(atom_types, edge_type_cutoff, float(r_max), N, dev)
+    elif atom_types is not None:
+        raise ValueError("atom_types is only read with edge_type_cutoff")
+    types, rc2, T = (0, 0, 0) if ty is None else (_ptr(ty.types), _ptr(ty.rc2), ty.T)
+    s = _nl_scratch(N, int(bin_base[-1]), dev)
+    st = _stream()
+    fr = (_ptr(blocks_dev), _ptr(frame), _ptr(bin_base_dev))
+    _capi.check(L.nqb_nl_bin_frames(_ptr(pos), N, *fr, _ptr(s["wpos"]), _ptr(s["base"]), _ptr(s["binid"]),
+                                    _ptr(s["cidx"]), st), "nqb_nl_bin_frames")
+    torch.sort(s["binid"], stable=True, out=(s["sorted_bin"], s["order"]))
+    torch.searchsorted(s["sorted_bin"], s["bins"], out=s["bin_start"])
+    _capi.check(L.nqb_nl_count_frames(N, *fr, _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["order"]),
+                                      _ptr(s["bin_start"]), types, rc2, T, _ptr(s["counts"]), st),
+                "nqb_nl_count_frames")
+    row_ptr = s["row_ptr"]
+    torch.cumsum(s["counts"], 0, out=row_ptr[1:])
+    E = int(row_ptr[-1].item())
+    edge_index = torch.empty((2, E), dtype=torch.int64, device=dev)
+    shifts = torch.empty((E, 3), dtype=torch.float64, device=dev)
+    _capi.check(L.nqb_nl_fill_frames(N, E, *fr, _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["base"]), _ptr(s["order"]),
+                                     _ptr(s["bin_start"]), _ptr(row_ptr), types, rc2, T, _ptr(edge_index),
+                                     _ptr(shifts), st), "nqb_nl_fill_frames")
+    out = {"edge_index": edge_index, "edge_cell_shift": shifts, "row_ptr": row_ptr}
+    if transpose_perm:
+        # frames hold disjoint, increasing atom ranges: the global (neighbour, centre) order is the frames' orders
         out["edge_transpose_perm"] = torch.argsort(edge_index[1] * N + edge_index[0], stable=True)
     return out
 
