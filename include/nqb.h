@@ -354,6 +354,28 @@ int nqb_nl_fill_frames(int64_t N, int64_t E, const void* blocks_dev, const int64
                        const int64_t* bin_start, const int64_t* row_ptr /* [N+1] */, const int64_t* types,
                        const double* rc2, int T, int64_t* edge_index /* [2,E] */, double* shifts /* [E,3] */,
                        nqb_stream_t st);
+/* A batch of frames in a list of fixed length (NeighborListPlan with batch=).  nqb_nl_frames_pack_capacity fills
+ * out_host [F * nqb_nl_params_bytes()] on the HOST: block f is that of nqb_nl_frames_pack plus frame f's null-edge
+ * shift pad_shift [F,3] and the open-direction fields of nqb_nl_params_pack_open (open[d] = !pbc[3f+d], cap [F] >= 1,
+ * perp [F,3] finite and positive, r_max finite and > 0).
+ * nqb_nl_bbox_frames (capturable, no work buffer) runs one CTA per frame over its atoms [atom_ptr[f], atom_ptr[f+1])
+ * (atom_ptr [F+1] i64, device) and writes, in the DEVICE block f and nowhere else, lo / width / nb / search of each open
+ * direction as nqb_nl_bbox does for one block; a frame without an open direction or without atoms is left as packed.
+ * nqb_nl_fill_capacity_frames: nqb_nl_fill_capacity over frames (row_ptr_pad and overflow from nqb_nl_pad over all N
+ * atoms, one capacity for the batch); the null edges of atom i carry the pad_shift of blocks[batch[i]].  Write contract
+ * of nqb_nl_fill_capacity. */
+int nqb_nl_frames_pack_capacity(int F, const double* cell_host, const double* inv_host, const int* pbc,
+                                const int* nbins, const int* search, const double* lo, const double* width,
+                                double r_max, const double* pad_shift_host, const int* cap, const double* perp_host,
+                                void* out_host);
+int nqb_nl_bbox_frames(const double* pos /* [N,3] */, int F, const int64_t* atom_ptr /* [F+1] */, void* blocks_dev,
+                       nqb_stream_t st);
+int nqb_nl_fill_capacity_frames(int64_t N, int64_t capacity, const void* blocks_dev, const int64_t* batch,
+                                const int64_t* bin_base, const double* wpos, const int32_t* cidx, const int32_t* base,
+                                const int64_t* order, const int64_t* bin_start, const int64_t* row_ptr_pad /* [N+1] */,
+                                const int32_t* overflow /* [1] */, const int64_t* types, const double* rc2, int T,
+                                int64_t* edge_index /* [2,capacity] */, double* shifts /* [capacity,3] */,
+                                nqb_stream_t st);
 
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).

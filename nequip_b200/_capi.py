@@ -93,6 +93,10 @@ SIGNATURES = {
     "nqb_nl_count_frames": (_i32, [_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp]),
     "nqb_nl_fill_frames": (
         _i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "nqb_nl_frames_pack_capacity": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp]),
+    "nqb_nl_bbox_frames": (_i32, [_vp, _i32, _vp, _vp, _vp]),
+    "nqb_nl_fill_capacity_frames": (
+        _i32, [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "nqb_edge_embed_fwd_frames": (
         _i32, [_i32, _i32, _dbl, _dbl, _dbl, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _vp,
                _vp, _vp]),

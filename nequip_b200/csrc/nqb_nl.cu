@@ -70,11 +70,15 @@ __device__ __forceinline__ const NlParams& nl_p(const NlFrames& f, int64_t i) { 
 __device__ __forceinline__ int64_t nl_bin0(const NlParams&, int64_t) { return 0; }
 __device__ __forceinline__ int64_t nl_bin0(NlBlockPtr, int64_t) { return 0; }
 __device__ __forceinline__ int64_t nl_bin0(const NlFrames& f, int64_t i) { return f.bin_base[f.batch[i]]; }
-__device__ __forceinline__ double3 nl_pad_shift(const NlParams&, double3 pad_shift) { return pad_shift; }
-__device__ __forceinline__ double3 nl_pad_shift(NlBlockPtr b, double3) {
+__device__ __forceinline__ double3 nl_pad_shift(const NlParams&, int64_t, double3 pad_shift) { return pad_shift; }
+__device__ __forceinline__ double3 nl_pad_shift(NlBlockPtr b, int64_t, double3) {
   return make_double3(b->pad_shift[0], b->pad_shift[1], b->pad_shift[2]);
 }
-__device__ __forceinline__ double3 nl_pad_shift(const NlFrames&, double3 pad_shift) { return pad_shift; }
+// a null edge of atom i takes the shift of its own frame: one shift for every frame could be short in another cell
+__device__ __forceinline__ double3 nl_pad_shift(const NlFrames& f, int64_t i, double3) {
+  const NlBlock& b = f.blocks[f.batch[i]];
+  return make_double3(b.pad_shift[0], b.pad_shift[1], b.pad_shift[2]);
+}
 
 // Per-edge-type cutoffs (kTyped): the pair (i, j) is a neighbour when d2 < rc2[T * types[i] + types[j]] instead of
 // d2 < r2.  rc2 = rc * rc is computed on the host in float64; the bins stay sized by the global r_max >= every rc.
@@ -201,8 +205,8 @@ __device__ __forceinline__ bool nl_less(int64_t ja, const double* sa, int64_t jb
 // kCapacity = true (nqb_nl_fill_capacity): the row owns [row_ptr_pad[i], row_ptr_pad[i + 1]) of a list of E = capacity
 // slots; its real edges come first (same order and shifts as above, none when *overflow is set) and the remaining slots
 // hold null edges (i, i, pad_shift).  The trailing parameters are appended so the unpadded variant's code is unchanged.
-// With PS = NlBlockPtr (only with kCapacity) the null-edge shift comes from the block and the pad_shift argument is
-// not read.
+// With PS = NlBlockPtr or NlFrames (only with kCapacity) the null-edge shift comes from the block (of atom i's frame)
+// and the pad_shift argument is not read.
 template <bool kCapacity, class PS, bool kTyped = false>
 __global__ void k_nl_fill(PS ps, int64_t N, const double* __restrict__ wpos, const int32_t* __restrict__ cidx,
                           const int32_t* __restrict__ base, const int64_t* __restrict__ order,
@@ -234,7 +238,7 @@ __global__ void k_nl_fill(PS ps, int64_t N, const double* __restrict__ wpos, con
   }
   if (kCapacity) {
     const int64_t end = row_ptr[i + 1];
-    const double3 ps3 = nl_pad_shift(ps, pad_shift);
+    const double3 ps3 = nl_pad_shift(ps, i, pad_shift);
     for (int64_t q = beg + n; q < end; ++q) {
       edge_index[q] = i;
       ej[q] = i;
@@ -322,6 +326,47 @@ k_nl_bbox(NlBlock* __restrict__ b, const double* __restrict__ pos, int64_t N, un
     b->p.sr[d] = 1;
   }
   atomicExch(ticket, 0u);
+}
+
+// Bounding boxes of a batch of frames (nqb_nl_bbox_frames): CTA f reduces the fractional coordinates (nl_frac) of its
+// frame's atoms [atom_ptr[f], atom_ptr[f + 1]) and writes lo / width / nb / sr of every open direction of blocks[f]
+// with the formulas of k_nl_bbox.  One CTA owns one block, so there are no atomics and no work words, and the grid
+// depends on F only (capturable).  A frame without open directions or without atoms keeps its packed block.
+__global__ void __launch_bounds__(kBboxThreads)
+k_nl_bbox_frames(NlBlock* __restrict__ blocks, const double* __restrict__ pos, const int64_t* __restrict__ atom_ptr) {
+  NlBlock* b = blocks + blockIdx.x;
+  const int64_t beg = atom_ptr[blockIdx.x], end = atom_ptr[blockIdx.x + 1];
+  if (!(b->open[0] || b->open[1] || b->open[2]) || end <= beg) return;
+  const NlParams& p = b->p;
+  double lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+  for (int64_t i = beg + threadIdx.x; i < end; i += blockDim.x) {
+    double f[3];
+    nl_frac(p, pos[3 * i], pos[3 * i + 1], pos[3 * i + 2], f);
+    for (int d = 0; d < 3; ++d) { lo[d] = fmin(lo[d], f[d]); hi[d] = fmax(hi[d], f[d]); }
+  }
+  for (int o = 16; o > 0; o >>= 1)
+    for (int d = 0; d < 3; ++d) {
+      lo[d] = fmin(lo[d], __shfl_xor_sync(0xffffffffu, lo[d], o));
+      hi[d] = fmax(hi[d], __shfl_xor_sync(0xffffffffu, hi[d], o));
+    }
+  __shared__ double s[kBboxThreads / 32][6];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0)
+    for (int d = 0; d < 3; ++d) { s[warp][d] = lo[d]; s[warp][3 + d] = hi[d]; }
+  __syncthreads();  // every thread's reads of the block precede thread 0's writes
+  if (threadIdx.x != 0) return;
+  for (int w = 1; w < kBboxThreads / 32; ++w)
+    for (int d = 0; d < 3; ++d) { lo[d] = fmin(lo[d], s[w][d]); hi[d] = fmax(hi[d], s[w][3 + d]); }
+  for (int d = 0; d < 3; ++d) {
+    if (!b->open[d]) continue;
+    double w = dadd(hi[d], -lo[d]);
+    w = dmul(w > 1e-9 ? w : 1e-9, 1.0 + 1e-9);
+    const double t = floor(__ddiv_rn(dmul(b->perp[d], w), b->r_max));
+    b->p.lo[d] = lo[d];
+    b->p.width[d] = w;
+    b->p.nb[d] = t >= 1.0 ? (t < (double)b->cap ? (int)t : b->cap) : 1;
+    b->p.sr[d] = 1;
+  }
 }
 
 }  // namespace
@@ -737,5 +782,69 @@ extern "C" int nqb_nl_fill_frames(int64_t N, int64_t E, const void* blocks_dev, 
   else
     k_nl_fill<false, NlFrames><<<blocks, 64, 0, (cudaStream_t)st>>>(
         fr, N, wpos, cidx, base, order, bin_start, row_ptr, E, edge_index, shifts, nullptr, zero, ty);
+  return nl_launch_done();
+}
+
+// Capacity mode for a batch of frames (NeighborListPlan with batch=).  nqb_nl_frames_pack_capacity: the blocks of
+// nqb_nl_frames_pack, plus each frame's null-edge shift (pad_shift [F,3]) and the fields of nqb_nl_params_pack_open:
+// open[d] = !pbc[3f + d], cap [F] (most bins along frame f's open directions), perp [F,3], r_max.
+extern "C" int nqb_nl_frames_pack_capacity(int F, const double* cell_host, const double* inv_host, const int* pbc,
+                                           const int* nbins, const int* search, const double* lo, const double* width,
+                                           double r_max, const double* pad_shift_host, const int* cap,
+                                           const double* perp_host, void* out_host) {
+  if (F < 0) return nqb_set_error("nqb_nl_frames_pack_capacity: negative frame count");
+  if (F > 0 && (!pad_shift_host || !cap || !perp_host)) return nqb_set_error("nqb_nl_frames_pack_capacity: null pointer");
+  if (!(r_max > 0.0) || !isfinite(r_max)) return nqb_set_error("nqb_nl_frames_pack_capacity: needs a finite r_max > 0");
+  for (int f = 0; f < F; ++f) {
+    if (cap[f] < 1) return nqb_set_error("nqb_nl_frames_pack_capacity: needs cap >= 1");
+    for (int d = 0; d < 3; ++d)
+      if (!(perp_host[3 * f + d] > 0.0) || !isfinite(perp_host[3 * f + d]))
+        return nqb_set_error("nqb_nl_frames_pack_capacity: perpendicular widths must be finite and positive");
+  }
+  if (int rc = nqb_nl_frames_pack(F, cell_host, inv_host, pbc, nbins, search, lo, width, r_max, out_host)) return rc;
+  for (int f = 0; f < F; ++f) {
+    NlBlock* b = (NlBlock*)((char*)out_host + (size_t)f * sizeof(NlBlock));
+    for (int d = 0; d < 3; ++d) {
+      b->pad_shift[d] = pad_shift_host[3 * f + d];
+      b->open[d] = pbc[3 * f + d] ? 0 : 1;
+      b->perp[d] = perp_host[3 * f + d];
+    }
+    b->cap = cap[f];
+    b->r_max = r_max;
+  }
+  return 0;
+}
+
+extern "C" int nqb_nl_bbox_frames(const double* pos, int F, const int64_t* atom_ptr, void* blocks_dev,
+                                  nqb_stream_t st) {
+  if (F < 0) return nqb_set_error("nqb_nl_bbox_frames: negative frame count");
+  if (F == 0) return 0;
+  if (!pos || !atom_ptr || !blocks_dev) return nqb_set_error("nqb_nl_bbox_frames: null pointer");
+  k_nl_bbox_frames<<<(unsigned)F, kBboxThreads, 0, (cudaStream_t)st>>>((NlBlock*)blocks_dev, pos, atom_ptr);
+  return nl_launch_done();
+}
+
+extern "C" int nqb_nl_fill_capacity_frames(int64_t N, int64_t capacity, const void* blocks_dev, const int64_t* batch,
+                                           const int64_t* bin_base, const double* wpos, const int32_t* cidx,
+                                           const int32_t* base, const int64_t* order, const int64_t* bin_start,
+                                           const int64_t* row_ptr_pad, const int32_t* overflow, const int64_t* types,
+                                           const double* rc2, int T, int64_t* edge_index, double* shifts,
+                                           nqb_stream_t st) {
+  if (N <= 0 || capacity < 0) return nqb_set_error("nqb_nl_fill_capacity_frames: needs N > 0 and capacity >= 0");
+  if (capacity == 0) return 0;
+  if (!wpos || !cidx || !base || !order || !bin_start || !row_ptr_pad || !overflow || !edge_index || !shifts)
+    return nqb_set_error("nqb_nl_fill_capacity_frames: null pointer");
+  NlFrames fr;
+  if (int rc = nl_frames("nqb_nl_fill_capacity_frames", blocks_dev, batch, bin_base, fr)) return rc;
+  NlTypes ty;
+  if (int rc = nl_types_opt("nqb_nl_fill_capacity_frames", types, rc2, T, ty)) return rc;
+  const unsigned blocks = (unsigned)((N + 63) / 64);
+  const double3 zero = make_double3(0.0, 0.0, 0.0);
+  if (ty.types)
+    k_nl_fill<true, NlFrames, true><<<blocks, 64, 0, (cudaStream_t)st>>>(
+        fr, N, wpos, cidx, base, order, bin_start, row_ptr_pad, capacity, edge_index, shifts, overflow, zero, ty);
+  else
+    k_nl_fill<true, NlFrames><<<blocks, 64, 0, (cudaStream_t)st>>>(
+        fr, N, wpos, cidx, base, order, bin_start, row_ptr_pad, capacity, edge_index, shifts, overflow, zero, ty);
   return nl_launch_done();
 }

@@ -175,21 +175,38 @@ class GraphedMDStep(GraphedEnergyForces):
     neighbour list (``ops.NeighborListPlan.set_cell``) before the replay.  The captured call is
     ``model(d, compute_stress=True)``, so the outputs also hold ``stress`` and ``virial`` [1,3,3].  A re-capture
     happens at the current cell, with a bin grid chosen for it.  ``variable_cell`` needs all three directions periodic
-    (``ValueError`` otherwise)."""
+    (``ValueError`` otherwise).
+
+    A batch of independent frames (torch-sim's input): ``example`` also holds ``batch`` [N] (non-decreasing) and
+    ``num_atoms`` [F], ``cell`` is [F, 3, 3] or absent and ``pbc``, when present, is [F, 3] (or [3] for every frame).
+    One graph then holds the step of every frame: one batched device list of one ``capacity``
+    (``ops.NeighborListPlan(batch=)``, each frame with its own cell, grid and null-edge shift) and one model call on
+    ``plan.cell`` [F, 3, 3].  The default capacity is sized from the batched ``ops.neighbor_list`` count.  ``g(pos)``
+    returns ``total_energy`` [F, 1]; with ``variable_cell=True``, ``g(pos, cells)`` takes [F, 3, 3] and returns
+    ``stress`` and ``virial`` [F, 3, 3].  The frames and their atom counts are fixed for the graph (a different batch
+    needs a new ``GraphedMDStep``); ``batch`` and ``num_atoms`` are copied into the graph's static inputs, so the
+    captured model call reads the frame count without a host synchronisation."""
 
     def __init__(self, model, example: Dict[str, torch.Tensor], capacity: Optional[int] = None, warmup: int = 3,
                  variable_cell: bool = False):
         cell = example.get("cell")
         self.pbc = self._periodicity(example)
-        if cell is None and any(self.pbc):
+        if cell is None and any(self._flags()):
             raise ValueError("GraphedMDStep: a periodic direction needs a cell")
-        if variable_cell and not all(self.pbc):
+        if variable_cell and not all(self._flags()):
             raise ValueError("GraphedMDStep: variable_cell needs all three directions periodic")
         if example["pos"].device.type != "cuda":
             raise RuntimeError("GraphedMDStep needs CUDA tensors (there is no CPU path)")
+        self._frames = None
+        if example.get("batch") is not None:
+            dev = example["pos"].device
+            self._frames = {"batch": example["batch"].to(dev).view(-1).clone(),
+                            "num_atoms": torch.as_tensor(example["num_atoms"]).to(dev).view(-1).clone()}
         if capacity is None:
             e0 = int(ops.neighbor_list(example["pos"], cell, self.pbc, model.r_max,
-                                       **self._edge_type_args(model, example))["edge_index"].shape[1])
+                                       **self._edge_type_args(model, example),
+                                       **({} if self._frames is None else {"batch": self._frames["batch"]})
+                                       )["edge_index"].shape[1])
             capacity = e0 + math.ceil(CAPACITY_SLACK * e0)
         self.variable_cell = bool(variable_cell)
         self.recaptures = 0
@@ -199,13 +216,19 @@ class GraphedMDStep(GraphedEnergyForces):
         self._capture(model, {k: example[k] for k in ("pos", "atom_types", "cell") if example.get(k) is not None},
                       int(capacity))
 
+    def _flags(self) -> list:
+        """Every periodicity flag of the step (3, or 3 per frame of a batch)."""
+        return [b for row in self.pbc for b in (row if isinstance(row, tuple) else (row,))]
+
     @staticmethod
     def _periodicity(example: Dict[str, torch.Tensor]) -> tuple:
         """3 bools: ``example["pbc"]`` ([3] or [1, 3], or one bool) when present, else all periodic with a cell and
-        all open without one."""
+        all open without one.  A batch (``example["batch"]``) with ``pbc`` [F, 3]: F tuples of 3 bools."""
         pbc = example.get("pbc")
         if pbc is None:
             return (example.get("cell") is not None,) * 3
+        if example.get("batch") is not None and torch.as_tensor(pbc).dim() == 2:
+            return tuple(tuple(bool(b) for b in row) for row in torch.as_tensor(pbc).tolist())
         flags = [bool(b) for b in torch.as_tensor(pbc).reshape(-1).tolist()]
         if len(flags) == 1:
             flags *= 3
@@ -221,12 +244,17 @@ class GraphedMDStep(GraphedEnergyForces):
 
     def _capture(self, model, example: Dict[str, torch.Tensor], capacity: int) -> None:
         self.capacity = capacity
-        is_open = not all(self.pbc)
+        is_open = not all(self._flags())
+        frames = {}
+        if self._frames is not None:
+            example = dict(example, **self._frames)
+            frames = {"batch": self._frames["batch"]}
         self.plan = ops.NeighborListPlan(example["pos"].shape[0], example.get("cell"), self.pbc, model.r_max, capacity,
                                          device=example["pos"].device, variable_cell=self.variable_cell,
-                                         **self._edge_type_args(model, example), open_boundaries=is_open)
-        if is_open:
-            # the null edges' shift refers to plan.cell (the identity without a cell): the model must see it
+                                         **self._edge_type_args(model, example), open_boundaries=is_open, **frames)
+        if is_open or frames:
+            # the null edges' shift refers to plan.cell (the identity without a cell, [F, 3, 3] for a batch): the
+            # model must see it
             example = dict(example, cell=self.plan.cell)
         super().__init__(model, example, warmup=self._warmup)
         ops.src_csr_cache.clear()  # like csr_cache: an entry made during the capture lives in the graph's pool

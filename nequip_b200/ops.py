@@ -626,14 +626,17 @@ def edge_embed_from_vectors(vec, *, lmax: int, num_bessel: int = 8, r_max: float
 
 def _frame_cells(cell, batch, num_atoms: int, what: str):
     """(cells [F, 3, 3] f64, frame [N] i64) of a batch of frames for the ``_frames`` kernels; ``ValueError`` for a
-    malformed ``batch`` or a frame index outside [0, F) (one host synchronisation)."""
+    malformed ``batch`` or a frame index outside [0, F) (one host synchronisation, skipped while the stream is
+    capturing a CUDA graph)."""
     _require_cuda(cell, batch)
     if cell.dim() != 3 or tuple(cell.shape[1:]) != (3, 3):
         raise ValueError(f"{what}: cell must be [F, 3, 3] with batch, got {tuple(cell.shape)}")
     frame = batch.view(-1).long().contiguous()
     if frame.numel() != num_atoms:
         raise ValueError(f"{what}: batch must hold {num_atoms} frame indices, got {frame.numel()}")
-    if num_atoms:
+    if num_atoms and not torch.cuda.is_current_stream_capturing():
+        # a captured step (graph.GraphedMDStep) takes its batch from a NeighborListPlan that checked it when it was
+        # made, and a read-back cannot be captured
         lo, hi = (int(v) for v in torch.aminmax(frame))
         if lo < 0 or hi >= cell.shape[0]:
             raise ValueError(f"{what}: batch holds frame indices outside [0, {cell.shape[0]})")
@@ -1521,13 +1524,31 @@ class NeighborListPlan:
     The rows are those of ``neighbor_list(pos, cell, pbc)``.  ``plan.cell`` ([3, 3] float64, on the device) is the cell
     the shifts refer to: the caller must give it to the model as ``cell``, since the null edges (i, i, pad_shift)
     only have their length r_max + |a_d| through it; real edges along open directions have shift 0.  The cell must be
-    finite and non-singular, and ``variable_cell`` needs all three directions periodic."""
+    finite and non-singular, and ``variable_cell`` needs all three directions periodic.
+
+    ``batch`` [N] (a batch of independent frames, as in ``neighbor_list(..., batch=)``): ``cell`` [F, 3, 3] or None,
+    ``pbc`` a bool, [3] or [F, 3]; ``batch`` is checked once, here, and is fixed for the plan's lifetime, as are the
+    frames' atom counts.  Each frame gets its own parameter block (``nqb_nl_frames_pack_capacity``): its bin grid, fixed
+    here, with ``cap_f = round((4 N_f)^(1/3))`` bins along its open directions, and its own null-edge shift
+    (``pad_shift`` [F, 3]): one shift for all frames could be shorter than r_max in another frame's cell.  ``run`` finds
+    the bounding boxes of the frames with an open direction on the device (``nqb_nl_bbox_frames``, one CTA per frame),
+    then bins, counts and fills over all frames.  Row i holds the real edges of ``neighbor_list(pos, cell, pbc,
+    batch=)`` then null edges (i, i, pad_shift of i's frame); one ``capacity`` and one ``overflow`` flag serve the batch,
+    since every row only holds its own frame's edges.  ``plan.cell`` [F, 3, 3] (the identity for a frame open in every
+    direction) is the cell the model must be given.  A frame with an open direction needs ``open_boundaries``;
+    ``variable_cell`` needs every frame periodic in all three directions, and ``set_cell`` then takes [F, 3, 3]."""
+
+    _fr = None  # the frames of a batched plan (batch=); None for one frame
 
     def __init__(self, num_atoms: int, cell, pbc, r_max: float, capacity: int, device=None,
                  variable_cell: bool = False, atom_types=None, edge_type_cutoff=None, *,
-                 open_boundaries: bool = False):
+                 open_boundaries: bool = False, batch=None):
         import numpy as np
 
+        if batch is not None:
+            self._init_frames(num_atoms, cell, pbc, r_max, capacity, device, variable_cell, atom_types,
+                              edge_type_cutoff, open_boundaries, batch)
+            return
         if isinstance(pbc, bool):
             pbc = (pbc,) * 3
         pbc = [bool(b) for b in (pbc.tolist() if torch.is_tensor(pbc) else pbc)]
@@ -1596,6 +1617,90 @@ class NeighborListPlan:
         elif self._open:
             self._params_dev = open_block
 
+    def _init_frames(self, num_atoms, cell, pbc, r_max, capacity, device, variable_cell, atom_types, edge_type_cutoff,
+                     open_boundaries, batch) -> None:
+        import numpy as np
+
+        N = int(num_atoms)
+        if N < 1 or int(capacity) < 0:
+            raise ValueError("NeighborListPlan needs num_atoms >= 1 and capacity >= 0")
+        F, pbc_np, cells = _nl_frame_args(cell, pbc, batch, N)
+        open_f = ~pbc_np.all(axis=1)
+        if open_f.any() and not open_boundaries:
+            raise ValueError("NeighborListPlan: a frame with an open direction needs open_boundaries=True")
+        if variable_cell and open_f.any():
+            raise ValueError("NeighborListPlan: variable_cell needs every frame periodic in all three directions")
+        for f in range(F):
+            _nl_check_cell(cells[f], "NeighborListPlan")
+        self.num_atoms, self.capacity, self.r_max = N, int(capacity), float(r_max)
+        self.num_frames = F
+        frame = torch.as_tensor(batch).view(-1).to(torch.int64)
+        counts = torch.bincount(frame.cpu(), minlength=F).numpy()
+        dev = torch.device(device) if device is not None else (
+            frame.device if frame.is_cuda else torch.device("cuda"))
+        self.device = dev
+        invs = np.linalg.inv(cells)
+        self._counts = [int(n) for n in counts]
+        self._pbc = [[bool(v) for v in pbc_np[f]] for f in range(F)]
+        # the bin grid of every frame, fixed here: cap_f bins along open directions (nqb_nl_bbox_frames picks at most
+        # that many per run); the frames' ranges of one global bin range start at bin_base
+        self._caps = [_nl_bin_cap(n) for n in self._counts]
+        self._nbins = []
+        for f in range(F):
+            a = _NlArgs(self._counts[f], cells[f], invs[f], self._pbc[f], r_max, np.zeros(3), np.ones(3))
+            self._nbins.append([n if p else self._caps[f] for n, p in zip(a.nb, self._pbc[f])])
+        block = self._pack_frames(cells, invs)
+        self._fr = {
+            "frame": frame.to(dev).contiguous().clone(),
+            "bin_base": torch.as_tensor(np.cumsum([0] + [int(np.prod(nb)) for nb in self._nbins]),
+                                        dtype=torch.int64).to(dev),
+            "atom_ptr": torch.as_tensor(np.cumsum([0] + self._counts), dtype=torch.int64).to(dev),
+        }
+        self._open = bool(open_f.any())
+        self.cell = torch.from_numpy(cells.copy()).to(dev)
+        self._ty = None
+        if edge_type_cutoff is not None:
+            self._ty = _NlTypes(atom_types, edge_type_cutoff, self.r_max, N, dev)
+        elif atom_types is not None:
+            raise ValueError("NeighborListPlan: atom_types is only read with edge_type_cutoff")
+        self._s = _nl_scratch(N, int(self._fr["bin_base"][-1]), dev)
+        cap = self.capacity
+        self.edge_index = torch.empty((2, cap), dtype=torch.int64, device=dev)
+        self.edge_cell_shift = torch.empty((cap, 3), dtype=torch.float64, device=dev)
+        self.row_ptr = torch.empty((N + 1,), dtype=torch.int64, device=dev)
+        self.num_edges = torch.empty((1,), dtype=torch.int64, device=dev)
+        self.overflow = torch.empty((1,), dtype=torch.int32, device=dev)
+        self.variable_cell = bool(variable_cell)
+        self._params_dev = torch.frombuffer(bytearray(block.raw), dtype=torch.uint8).to(dev)
+        if self.variable_cell:
+            self._params_host = torch.empty((len(block),), dtype=torch.uint8).pin_memory()
+            self._params_event: Optional[torch.cuda.Event] = None
+
+    def _pack_frames(self, cells, invs):
+        """The frames' device parameter blocks (``nqb_nl_frames_pack_capacity``, ctypes buffer) for ``cells`` on the
+        plan's bin grids, each frame with the search range its cell needs and its own null-edge shift."""
+        import numpy as np
+
+        F = self.num_frames
+        cols = {k: [] for k in ("pbc", "nb", "sr", "lo", "width")}
+        pad, perp = [], []
+        for f in range(F):
+            a = _NlArgs(self._counts[f], cells[f], invs[f], self._pbc[f], self.r_max, np.zeros(3), np.ones(3),
+                        nb=self._nbins[f])
+            for k in cols:
+                cols[k].extend(getattr(a, k))
+            pad.extend(null_edge_shift(cells[f], self.r_max))
+            perp.extend(_nl_perp(invs[f]))
+        self.pad_shift = np.asarray(pad, dtype=np.float64).reshape(F, 3)
+        I3, D9, D3 = C.c_int * (3 * F), C.c_double * (9 * F), C.c_double * (3 * F)
+        L = _capi.lib()
+        block = C.create_string_buffer(F * int(L.nqb_nl_params_bytes()))
+        _capi.check(L.nqb_nl_frames_pack_capacity(F, D9(*cells.reshape(-1)), D9(*invs.reshape(-1)), I3(*cols["pbc"]),
+                                                  I3(*cols["nb"]), I3(*cols["sr"]), D3(*cols["lo"]),
+                                                  D3(*cols["width"]), self.r_max, D3(*pad), (C.c_int * F)(*self._caps),
+                                                  D3(*perp), block), "nqb_nl_frames_pack_capacity")
+        return block
+
     def set_cell(self, cell) -> None:
         """Make the following ``run`` calls (and replays of graphs that captured them) use ``cell`` ([3,3] or
         [1,3,3], rows = lattice vectors).  A host call, not captured: it computes the inverse (as ``neighbor_list``
@@ -1606,6 +1711,9 @@ class NeighborListPlan:
         singular cell and on a plan built without ``variable_cell``."""
         if not self.variable_cell:
             raise ValueError("NeighborListPlan.set_cell needs a plan built with variable_cell=True")
+        if self._fr is not None:
+            self._set_cells(cell)
+            return
         a, pad_shift, block = _nl_cell_block(cell, self.r_max, self.nbins, self.num_atoms)
         if self._params_event is not None:
             self._params_event.synchronize()
@@ -1616,11 +1724,61 @@ class NeighborListPlan:
             self._params_event.record()
         self._a, self.pad_shift = a, pad_shift
 
+    def _set_cells(self, cell) -> None:
+        """``set_cell`` of a batched plan: cells [F, 3, 3], each finite and non-singular; every frame's inverse,
+        search range on its fixed grid and null-edge shift, one pack of all blocks and one asynchronous copy from
+        pinned staging."""
+        import numpy as np
+
+        c = cell.detach().cpu().double().numpy() if torch.is_tensor(cell) else np.asarray(cell, dtype=np.float64)
+        if c.shape != (self.num_frames, 3, 3):
+            raise ValueError(f"set_cell: cell must be [{self.num_frames}, 3, 3], got {tuple(c.shape)}")
+        cells = np.stack([_nl_check_cell(c[f], "set_cell") for f in range(self.num_frames)])
+        block = self._pack_frames(cells, np.linalg.inv(cells))
+        if self._params_event is not None:
+            self._params_event.synchronize()
+        C.memmove(self._params_host.data_ptr(), block, len(block))
+        with torch.cuda.device(self.device):
+            self._params_dev.copy_(self._params_host, non_blocking=True)
+            self._params_event = torch.cuda.Event()
+            self._params_event.record()
+
+    def _run_frames(self, pos: torch.Tensor) -> None:
+        L = _capi.lib()
+        s, ty, fr = self._s, self._ty, self._fr
+        N, st = self.num_atoms, _stream()
+        blocks = (_ptr(self._params_dev), _ptr(fr["frame"]), _ptr(fr["bin_base"]))
+        types, rc2, T = (0, 0, 0) if ty is None else (_ptr(ty.types), _ptr(ty.rc2), ty.T)
+        if self._open:
+            _capi.check(L.nqb_nl_bbox_frames(_ptr(pos), self.num_frames, _ptr(fr["atom_ptr"]), _ptr(self._params_dev),
+                                             st), "nqb_nl_bbox_frames")
+        _capi.check(L.nqb_nl_bin_frames(_ptr(pos), N, *blocks, _ptr(s["wpos"]), _ptr(s["base"]), _ptr(s["binid"]),
+                                        _ptr(s["cidx"]), st), "nqb_nl_bin_frames")
+        torch.sort(s["binid"], stable=True, out=(s["sorted_bin"], s["order"]))
+        torch.searchsorted(s["sorted_bin"], s["bins"], out=s["bin_start"])
+        _capi.check(L.nqb_nl_count_frames(N, *blocks, _ptr(s["wpos"]), _ptr(s["cidx"]), _ptr(s["order"]),
+                                          _ptr(s["bin_start"]), types, rc2, T, _ptr(s["counts"]), st),
+                    "nqb_nl_count_frames")
+        torch.cumsum(s["counts"], 0, out=s["row_ptr"][1:])
+        _capi.check(L.nqb_nl_pad(N, self.capacity, _ptr(s["row_ptr"]), _ptr(self.row_ptr), _ptr(self.num_edges),
+                                 _ptr(self.overflow), st), "nqb_nl_pad")
+        _capi.check(L.nqb_nl_fill_capacity_frames(N, self.capacity, *blocks, _ptr(s["wpos"]), _ptr(s["cidx"]),
+                                                  _ptr(s["base"]), _ptr(s["order"]), _ptr(s["bin_start"]),
+                                                  _ptr(self.row_ptr), _ptr(self.overflow), types, rc2, T,
+                                                  _ptr(self.edge_index), _ptr(self.edge_cell_shift), st),
+                    "nqb_nl_fill_capacity_frames")
+
     def run(self, pos: torch.Tensor) -> Dict[str, torch.Tensor]:
         _require_cuda(pos)
         if tuple(pos.shape) != (self.num_atoms, 3):
             raise ValueError(f"NeighborListPlan: pos must be [{self.num_atoms}, 3], got {tuple(pos.shape)}")
         pos = pos.detach().double().contiguous()
+        if self._fr is not None:
+            self._run_frames(pos)
+            for t in (self.edge_index, self.edge_cell_shift, self.row_ptr, self.num_edges, self.overflow):
+                torch.autograd.graph.increment_version(t)
+            return {"edge_index": self.edge_index, "edge_cell_shift": self.edge_cell_shift, "row_ptr": self.row_ptr,
+                    "num_edges": self.num_edges, "overflow": self.overflow}
         L = _capi.lib()
         a, s, ty = self._a, self._s, self._ty
         if self._open:
