@@ -377,6 +377,40 @@ int nqb_nl_fill_capacity_frames(int64_t N, int64_t capacity, const void* blocks_
                                 int64_t* edge_index /* [2,capacity] */, double* shifts /* [capacity,3] */,
                                 nqb_stream_t st);
 
+/* Molecular dynamics on the device (nqb_md.cu, nequip_b200/md.py GraphedMD): velocity Verlet with the reference's
+ * Nose-Hoover thermostat (nequip/ase/nosehoover.py, NoseHoover.step) per frame f, all float64, in the reference's units
+ * (Angstrom, eV, amu; time in Angstrom sqrt(amu / eV)).  The atoms of frame f are [atom_ptr[f], atom_ptr[f+1])
+ * (atom_ptr [F+1] i64, device, non-decreasing).  The atom kernels run (nblk, F) CTAs of 256 threads; nblk in
+ * [1, 65535] is the caller's choice and sizes the workspaces part [F, nblk, 2] and ke_part [F, nblk].  No floating-point
+ * atomics: the sums over atoms are a fixed-order function of the inputs for a given nblk.  F <= 65535.
+ * nqb_md_kick_drift: a = forces/mass - zeta[f] v;  pos += dt v + dt^2/2 a;  vel = v + dt/2 a;
+ *   part[f, b] = {sum m v^2, sum m vel^2} over the atoms of CTA (b, f).  Writes pos and vel of every atom of the
+ *   frames and all of part, nothing else.
+ * nqb_md_bath (Nose-Hoover only): s0, s1 = sums of part[f, :, 0], part[f, :, 1] in index order;
+ *   zeta_h = zeta + dt/2 * (s0 - gkT) / 2 / Q;  zeta' = zeta_h + dt/2 * (s1 - gkT) / 2 / Q;
+ *   eta += dt/2 (zeta + zeta');  zeta = zeta'  (gkT = g_f k_B T_f with g_f = 3 N_f + 1, Q = nvt_q, both [F]).
+ *   Writes zeta [F] and eta [F], nothing else.
+ * nqb_md_kick: vel = (vel + dt/2 f_new/mass) / (1 + dt/2 zeta[f]);  forces = f_new;  ke_part[f, b] = sum m vel^2 of
+ *   CTA (b, f).  Writes vel and forces of every atom of the frames and all of ke_part, nothing else.
+ * nqb_md_log (one CTA): s = *step; row s % rows of log [rows, F, NQB_MD_LOG_FIELDS] gets, per frame,
+ *   {E_pot = e_pot[f], E_kin = sum_b ke_part[f, b] / 2, T = 2 E_kin / dof_kB[f], zeta, eta,
+ *    H = E_pot + E_kin + Q zeta^2 + gkT eta};  flags [4] i64 (sticky over the steps since the caller reset them to
+ *   {0, 0, -1, 0}): flags[0] |= overflow != 0, flags[1] |= sorted != 1, flags[2] = s at the first overflow,
+ *   flags[3] = max(flags[3], num_edges); then *step = s + 1.  Writes that log row, flags and step, nothing else. */
+#define NQB_MD_LOG_FIELDS 6
+int nqb_md_kick_drift(int F, int nblk, const int64_t* atom_ptr, const double* mass /* [N] */,
+                      const double* forces /* [N,3] */, const double* zeta /* [F] */, double dt, double* pos /* [N,3] */,
+                      double* vel /* [N,3] */, double* part /* [F,nblk,2] */, nqb_stream_t st);
+int nqb_md_bath(int F, int nblk, const double* part, const double* gkT, const double* Q, double dt, double* zeta,
+                double* eta, nqb_stream_t st);
+int nqb_md_kick(int F, int nblk, const int64_t* atom_ptr, const double* mass, const double* f_new /* [N,3] */,
+                const double* zeta, double dt, double* vel, double* forces, double* ke_part /* [F,nblk] */,
+                nqb_stream_t st);
+int nqb_md_log(int F, int nblk, const double* e_pot /* [F] */, const double* ke_part, const double* zeta,
+               const double* eta, const double* Q, const double* gkT, const double* dof_kB, const int64_t* num_edges,
+               const int32_t* overflow, const int32_t* sorted, int64_t rows, int64_t* step, double* log,
+               int64_t* flags /* [4] */, nqb_stream_t st);
+
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).
  * Together with nqb_gemm_grouped for the second layer this is ScalarMLPFunction (nequip/nn/mlp.py:80-195).

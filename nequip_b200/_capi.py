@@ -104,6 +104,10 @@ SIGNATURES = {
         _i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _i64, _dbl, _dbl, _i32, _vp, _vp, _vp]),
     "nqb_zbl_bwd_frames": (
         _i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _dbl, _dbl, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_md_kick_drift": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp]),
+    "nqb_md_bath": (_i32, [_i32, _i32, _vp, _vp, _vp, _dbl, _vp, _vp, _vp]),
+    "nqb_md_kick": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp]),
+    "nqb_md_log": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "nqb_mlp_hidden_fwd": (_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_fwd_rows": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
