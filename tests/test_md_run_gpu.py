@@ -30,13 +30,26 @@ def _ptr(t):
 # ------------------------------------------------------------------------------------------------------------------
 # kernels
 # ------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("counts", [[37], [5, 600, 1, 0, 80]], ids=["one_frame", "batch"])
+def _kernel_cases():
+    """(counts, nblk) with nblk in {1, 2, the driver's min(64, ceil(max N_f / 256))}: frames at the CTA size, frames
+    above 64 x 256 atoms (every CTA loops even at the driver's nblk) and empty frames.  nblk = 2 keeps the counts'
+    name as its id."""
+    named = [("one_frame", [37]), ("batch", [5, 600, 1, 0, 80]), ("cta_edges", [255, 256, 257]),
+             ("above_64_ctas", [16384, 1, 16385]), ("large_empty_small", [20000, 0, 3])]
+    cases = []
+    for name, counts in named:
+        driver = min(64, -(-max(counts) // 256))
+        for nblk in sorted({1, 2, driver}):
+            cases.append(pytest.param(counts, nblk, id=name if nblk == 2 else f"{name}-nblk{nblk}"))
+    return cases
+
+
+@pytest.mark.parametrize("counts,nblk", _kernel_cases())
 @pytest.mark.parametrize("thermostat", [False, True], ids=["nve", "nh"])
-def test_kernels_match_one_oracle_step_and_write_only_their_outputs(counts, thermostat):
+def test_kernels_match_one_oracle_step_and_write_only_their_outputs(counts, nblk, thermostat):
     g = torch.Generator().manual_seed(len(counts) + 10 * thermostat)
     F, N = len(counts), sum(counts)
     ptr = [0] + np.cumsum(counts).tolist()
-    nblk = 2  # frame 1 spans three CTAs' worth of atoms: each CTA loops
     pos = 10 * torch.rand(N, 3, generator=g, dtype=torch.float64)
     vel = torch.randn(N, 3, generator=g, dtype=torch.float64)
     frc = torch.randn(N, 3, generator=g, dtype=torch.float64)
