@@ -377,6 +377,15 @@ int nqb_nl_fill_capacity_frames(int64_t N, int64_t capacity, const void* blocks_
                                 int64_t* edge_index /* [2,capacity] */, double* shifts /* [capacity,3] */,
                                 nqb_stream_t st);
 
+/* Cells of a batched variable-cell plan packed on the device (NeighborListPlan.set_cell_device): thread f reads
+ * cells[f] ([F,3,3] float64, device, rows = lattice vectors) and rewrites in blocks[f] (device, F * nqb_nl_params_bytes())
+ * every field the host pack derives from the cell: cell, inverse (adjugate / determinant), diag and the orthorhombic
+ * test, perp, the search range sr = max(1, ceil(r_max / (perp_d / nb_d) - 1e-12)) on the block's grid, and the
+ * null-edge shift k e_d (d the first longest lattice vector, k = floor(r_max / |a_d|) + 2).  A non-finite cell or one
+ * with |det| <= 1e-12 |a_0| |a_1| |a_2| keeps its block and sets bad[f] = 1 (bad [F] int32, never cleared here).
+ * Writes those fields and bad, nothing else; no host synchronisation (capturable). */
+int nqb_nl_frames_set_cells(int F, const double* cells, void* blocks_dev, int32_t* bad, nqb_stream_t st);
+
 /* Molecular dynamics on the device (nqb_md.cu, nequip_b200/md.py GraphedMD): velocity Verlet with the reference's
  * Nose-Hoover thermostat (nequip/ase/nosehoover.py, NoseHoover.step) per frame f, all float64, in the reference's units
  * (Angstrom, eV, amu; time in Angstrom sqrt(amu / eV)).  The atoms of frame f are [atom_ptr[f], atom_ptr[f+1])
@@ -410,6 +419,43 @@ int nqb_md_log(int F, int nblk, const double* e_pot /* [F] */, const double* ke_
                const double* eta, const double* Q, const double* gkT, const double* dof_kB, const int64_t* num_edges,
                const int32_t* overflow, const int32_t* sorted, int64_t rows, int64_t* step, double* log,
                int64_t* flags /* [4] */, nqb_stream_t st);
+
+/* Structure relaxation on the device (nqb_relax.cu, nequip_b200/relax.py GraphedRelax): ASE's FIRE.step per frame f,
+ * optionally on the degrees of freedom of ASE's FrechetCellFilter (has_cell), all float64.  Atoms and CTAs as in the
+ * nqb_md kernels ((nblk, F) CTAs of 256 threads, nblk in [1, 65535], F <= 65535, no floating-point atomics).
+ * Per-frame state: fs [F,2] {dt, a}; is [F, NQB_RELAX_ISTATE] i64 {Nsteps, first, converged, failed, steps};
+ * a frame with converged or failed set is frozen.  Cell DOF (has_cell, all [F,9] row-major): Q = c log Fd, its
+ * velocity vcell and force gcell, Fd = exp(Q / c), the initial cell C0 and cell = C0 Fd^T; cfac [F] = c.
+ * nqb_relax_fire (one thread per frame): fire_host [7] = {maxstep, dtmax, finc, fdec, astart, fa, Nmin} on the HOST.
+ *   For an active frame, with vg, vv, gg = v.g, v.v, g.g over the frame's whole vector (part [F,nblk,4] in index
+ *   order, then the cell rows): first step v = 0; else v.g > 0 mixes v = (1-a) v + a |v| g / |g| (and dt, a grow
+ *   after Nmin steps, Nsteps += 1), v.g <= 0 resets v = 0, a = astart, dt *= fdec, Nsteps = 0; then v += dt g,
+ *   dr = dt v clipped to |dr| <= maxstep.  coef [F,4] = {cv, cg, sc, 1} so that v' = cv v + cg g, dr = sc v';
+ *   steps += 1; with has_cell it also moves vcell, Q, Fd and cell.  A frozen frame gets coef {1, 0, 0, 0} only.
+ *   Writes coef, fs, is and (has_cell) vcell, Q, Fd, cell of active frames, nothing else.
+ * nqb_relax_move: the atoms of active frames: vel = cv vel + cg g; s += sc vel; pos = s Fd^T (has_cell; without a
+ *   cell, s is not read and pos += sc vel).  Writes vel, s and pos of those atoms, nothing else.
+ * nqb_relax_gforce: g = forces Fd (has_cell) or forces; part[f, b] = {sum v.g, sum v.v, sum g.g, max |g_i|^2} of CTA
+ *   (b, f), a non-finite row counting +inf.  Writes g of every atom and all of part, nothing else.
+ * nqb_relax_finish (one CTA): per frame, with V = |det cell|: (has_cell) gcell = (1/c) D exp(L^T)[(virial - p V I)
+ *   Fd^-T], L = Q / c; m = the largest |g_i|^2 over part and the cell rows; a frame not frozen becomes failed if not
+ *   m <= fail_force^2, else converged if m < fmax^2; log row step % rows [rows, F, NQB_RELAX_LOG_FIELDS] =
+ *   {e_pot, e_pot + p V, sqrt(m), V}; flags [4] as in nqb_md_log; step += 1.  Writes gcell (has_cell), the
+ *   converged / failed words of is, that log row, flags and step, nothing else. */
+#define NQB_RELAX_ISTATE 5
+#define NQB_RELAX_LOG_FIELDS 4
+int nqb_relax_fire(int F, int nblk, const double* part, const double* fire_host, int has_cell, const double* cfac,
+                   const double* C0, const double* gcell, double* Q, double* vcell, double* Fd, double* cell,
+                   double* fs, int64_t* is, double* coef, nqb_stream_t st);
+int nqb_relax_move(int F, int nblk, const int64_t* atom_ptr, const double* coef, int has_cell, const double* Fd,
+                   const double* g, double* vel, double* s, double* pos, nqb_stream_t st);
+int nqb_relax_gforce(int F, int nblk, const int64_t* atom_ptr, int has_cell, const double* Fd, const double* forces,
+                     const double* vel, double* g, double* part, nqb_stream_t st);
+int nqb_relax_finish(int F, int nblk, const double* part, int has_cell, double pressure, const double* cfac,
+                     const double* Q, const double* Fd, const double* cell, const double* virial, const double* e_pot,
+                     double fmax, double fail_force, double* gcell, int64_t* is, const int64_t* num_edges,
+                     const int32_t* overflow, const int32_t* sorted, int64_t rows, int64_t* step, double* log,
+                     int64_t* flags, nqb_stream_t st);
 
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).

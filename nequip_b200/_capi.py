@@ -108,7 +108,14 @@ SIGNATURES = {
     "nqb_md_bath": (_i32, [_i32, _i32, _vp, _vp, _vp, _dbl, _vp, _vp, _vp]),
     "nqb_md_kick": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp, _dbl, _vp, _vp, _vp, _vp]),
     "nqb_md_log": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
-    "nqb_mlp_hidden_fwd": (_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
+    "nqb_nl_frames_set_cells": (_i32, [_i32, _vp, _vp, _vp, _vp]),
+    "nqb_relax_fire": (_i32, [_i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_relax_move": (_i32, [_i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_relax_gforce": (_i32, [_i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_relax_finish": (
+        _i32, [_i32, _i32, _vp, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _dbl, _vp, _vp, _vp, _vp, _vp, _i64,
+               _vp, _vp, _vp, _vp]),
+    "nqb_mlp_hidden_fwd":(_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_fwd_rows": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_edge_pairs_work_size": (_i64, [_i64]),

@@ -369,6 +369,67 @@ k_nl_bbox_frames(NlBlock* __restrict__ blocks, const double* __restrict__ pos, c
   }
 }
 
+// Cells of a batched variable-cell plan packed on the device (nqb_nl_frames_set_cells): thread f rewrites the fields of
+// blocks[f] that the host pack derives from the cell -- cell, inverse, diag / orthorhombic, perp, the search range on
+// the block's fixed grid and the null-edge shift -- with the host's formulas in the host's order of operations
+// (ops._NlArgs, ops.null_edge_shift; explicitly rounded, no FMA).  The inverse is the adjugate over the determinant,
+// so it may differ from the host's LU inverse by a few ulp.  A non-finite or singular cell (ops._nl_check_cell:
+// |det| <= 1e-12 |a_0| |a_1| |a_2|) leaves the block untouched and sets bad[f] = 1.
+__global__ void k_nl_frames_set_cells(int F, const double* __restrict__ cells, NlBlock* __restrict__ blocks,
+                                      int32_t* __restrict__ bad) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F) return;
+  double c[9];
+  bool finite = true;
+  for (int k = 0; k < 9; ++k) {
+    c[k] = cells[9 * (int64_t)f + k];
+    finite = finite && isfinite(c[k]);
+  }
+  double len[3];
+  for (int d = 0; d < 3; ++d)
+    len[d] = sqrt(dadd(dadd(dmul(c[3 * d], c[3 * d]), dmul(c[3 * d + 1], c[3 * d + 1])), dmul(c[3 * d + 2], c[3 * d + 2])));
+  // adjugate (transposed cofactors) and determinant
+  double adj[9];
+  adj[0] = dadd(dmul(c[4], c[8]), -dmul(c[5], c[7]));
+  adj[1] = dadd(dmul(c[2], c[7]), -dmul(c[1], c[8]));
+  adj[2] = dadd(dmul(c[1], c[5]), -dmul(c[2], c[4]));
+  adj[3] = dadd(dmul(c[5], c[6]), -dmul(c[3], c[8]));
+  adj[4] = dadd(dmul(c[0], c[8]), -dmul(c[2], c[6]));
+  adj[5] = dadd(dmul(c[2], c[3]), -dmul(c[0], c[5]));
+  adj[6] = dadd(dmul(c[3], c[7]), -dmul(c[4], c[6]));
+  adj[7] = dadd(dmul(c[1], c[6]), -dmul(c[0], c[7]));
+  adj[8] = dadd(dmul(c[0], c[4]), -dmul(c[1], c[3]));
+  const double det = dadd(dadd(dmul(c[0], adj[0]), dmul(c[1], adj[3])), dmul(c[2], adj[6]));
+  if (!finite || !(fabs(det) > dmul(1e-12, dmul(dmul(len[0], len[1]), len[2])))) {
+    bad[f] = 1;
+    return;
+  }
+  NlBlock* b = blocks + f;
+  NlParams& p = b->p;
+  bool ortho = true;
+  for (int k = 0; k < 9; ++k) {
+    p.cell[k] = c[k];
+    p.inv[k] = __ddiv_rn(adj[k], det);
+    if ((k % 4) != 0 && c[k] != 0.0) ortho = false;
+  }
+  p.orthorhombic = ortho ? 1 : 0;
+  int dmax = 0;
+  double lmax = len[0];
+  for (int d = 0; d < 3; ++d) {
+    p.diag[d] = c[4 * d];
+    const double* inv = p.inv;
+    const double nrm = sqrt(dadd(dadd(dmul(inv[d], inv[d]), dmul(inv[3 + d], inv[3 + d])), dmul(inv[6 + d], inv[6 + d])));
+    b->perp[d] = __ddiv_rn(1.0, nrm);
+    const double sr = ceil(dadd(__ddiv_rn(b->r_max, __ddiv_rn(b->perp[d], (double)p.nb[d])), -1e-12));
+    p.sr[d] = sr > 1.0 ? (int)sr : 1;
+    if (len[d] > lmax) {  // the first longest, as numpy's argmax
+      dmax = d;
+      lmax = len[d];
+    }
+  }
+  for (int d = 0; d < 3; ++d) b->pad_shift[d] = d == dmax ? floor(__ddiv_rn(b->r_max, lmax)) + 2.0 : 0.0;
+}
+
 }  // namespace
 
 // Step 1: bins.  cell/inv: row-major 3x3 on the HOST (9 doubles each); nbins/search: per direction.
@@ -821,6 +882,14 @@ extern "C" int nqb_nl_bbox_frames(const double* pos, int F, const int64_t* atom_
   if (F == 0) return 0;
   if (!pos || !atom_ptr || !blocks_dev) return nqb_set_error("nqb_nl_bbox_frames: null pointer");
   k_nl_bbox_frames<<<(unsigned)F, kBboxThreads, 0, (cudaStream_t)st>>>((NlBlock*)blocks_dev, pos, atom_ptr);
+  return nl_launch_done();
+}
+
+extern "C" int nqb_nl_frames_set_cells(int F, const double* cells, void* blocks_dev, int32_t* bad, nqb_stream_t st) {
+  if (F < 0) return nqb_set_error("nqb_nl_frames_set_cells: negative frame count");
+  if (F == 0) return 0;
+  if (!cells || !blocks_dev || !bad) return nqb_set_error("nqb_nl_frames_set_cells: null pointer");
+  k_nl_frames_set_cells<<<(unsigned)((F + 127) / 128), 128, 0, (cudaStream_t)st>>>(F, cells, (NlBlock*)blocks_dev, bad);
   return nl_launch_done();
 }
 

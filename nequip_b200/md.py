@@ -72,7 +72,107 @@ def maxwell_boltzmann(mass: torch.Tensor, temperature: torch.Tensor, seed: int =
     return z * torch.sqrt(KB * temperature / mass).unsqueeze(1)
 
 
-class GraphedMD(GraphedMDStep):
+class BlockDriver(GraphedMDStep):
+    """The block machinery that ``GraphedMD`` and ``relax.GraphedRelax`` share: a captured step that writes one row
+    of a device log ring per replay (row ``step % rows``) and keeps sticky flags [4] i64 {overflow, unsorted, first
+    overflowing step, largest edge count} (reset to {0, 0, -1, 0}), and ``_run_block(k)``, which replays the step k
+    times from a device-side snapshot of the state, reads the block's log rows, the flags and ``_block_reads()`` with
+    one host synchronisation, and rolls the block back and re-captures with ``capacity = ceil(1.02 * needed)`` when the
+    neighbour list overflowed.  A subclass sets ``LOG_FIELDS`` and ``num_frames``, lists its device state in
+    ``_state_list()``, calls ``_init_blocks`` before ``GraphedMDStep.__init__`` and writes the log from its captured
+    step."""
+
+    LOG_FIELDS: tuple = ()
+
+    def _init_blocks(self, dev) -> None:
+        self.host_reads = 0
+        self._step = torch.zeros(1, dtype=torch.int64, device=dev)
+        self._step_host = 0
+        self._sticky0 = torch.tensor([0, 0, -1, 0], dtype=torch.int64, device=dev)
+        self._sticky = self._sticky0.clone()
+        self._sticky_host = torch.zeros(4, dtype=torch.int64).pin_memory()
+        self._one = torch.ones(1, dtype=torch.int32, device=dev)
+        self._alloc_log(DEFAULT_LOG_ROWS)
+
+    def _state_list(self) -> list:
+        raise NotImplementedError
+
+    def _block_reads(self) -> list:
+        """(device tensor, pinned host tensor) pairs copied with every block's host read."""
+        return []
+
+    def _alloc_log(self, rows: int) -> None:
+        shape = (rows, self.num_frames, len(self.LOG_FIELDS))
+        self._log = torch.zeros(shape, dtype=torch.float64, device=self._step.device)
+        self._log_host = torch.zeros(shape, dtype=torch.float64).pin_memory()
+
+    def _sorted_flag(self) -> torch.Tensor:
+        """The captured step's "edges grouped by destination" flag (the capture's deferred flags)."""
+        flags = getattr(ops._sorted_tls, "flags", None)
+        return torch.stack([f.view(()) for f in flags]).min().view(1) if flags else self._one
+
+    def _capture(self, model, example: Dict[str, torch.Tensor], capacity: int) -> None:
+        # the warm-up before the capture executes the step: keep the state as it was
+        saved = [t.clone() for t in self._state_list()]
+        super()._capture(model, example, capacity)
+        for t, s in zip(self._state_list(), saved):
+            t.copy_(s)
+        self._sticky.copy_(self._sticky0)
+
+    def _read_block(self, k: int) -> torch.Tensor:
+        """The block's k log rows, the sticky flags and ``_block_reads()``, with one host synchronisation."""
+        R = self._log.shape[0]
+        a = self._step_host % R
+        n1 = min(k, R - a)
+        self._log_host[:n1].copy_(self._log[a:a + n1], non_blocking=True)
+        if n1 < k:
+            self._log_host[n1:k].copy_(self._log[:k - n1], non_blocking=True)
+        self._sticky_host.copy_(self._sticky, non_blocking=True)
+        for dev_t, host_t in self._block_reads():
+            host_t.copy_(dev_t, non_blocking=True)
+        done = torch.cuda.Event()
+        done.record()
+        done.synchronize()
+        self.host_reads += 1
+        return self._log_host[:k].clone()
+
+    def _fit_log(self, block: int) -> None:
+        """A log of at least ``block`` rows; the captured step holds the log's pointer and length, so a longer log
+        is a re-capture (not counted in ``recaptures``)."""
+        if block > self._log.shape[0]:
+            self._alloc_log(block)
+            n = self.recaptures
+            self._recapture(self.capacity)
+            self.recaptures = n
+
+    def _check_block(self) -> None:
+        """Raise for a block that must not be kept (after the overflow test)."""
+        if int(self._sticky_host[1]) != 0:
+            raise RuntimeError(f"{type(self).__name__}: a step's edge list was not grouped by destination; its "
+                               "forces are invalid")
+
+    def _run_block(self, k: int) -> torch.Tensor:
+        """Replay the step k times; returns the block's log rows [k, F, len(LOG_FIELDS)]."""
+        for s, t in zip(self._snap, self._state_list()):
+            s.copy_(t)
+        self._sticky.copy_(self._sticky0)
+        while True:
+            for _ in range(k):
+                self.graph.replay()
+            self.replays += k
+            got = self._read_block(k)
+            if int(self._sticky_host[0]) == 0:
+                break
+            for s, t in zip(self._snap, self._state_list()):
+                t.copy_(s)
+            self._sticky.copy_(self._sticky0)
+            self._recapture(max(self.capacity + 1, math.ceil(1.02 * int(self._sticky_host[3]))))
+        self._check_block()
+        self._step_host += k
+        return got
+
+
+class GraphedMD(BlockDriver):
     """A device-resident MD driver: ``md = GraphedMD(model, example, masses, timestep_fs); log = md.run(n_steps)``.
 
     ``example`` holds what ``GraphedMDStep`` takes: ``pos`` [N, 3], ``atom_types`` [N], ``cell`` or none, ``pbc``, and
@@ -100,6 +200,8 @@ class GraphedMD(GraphedMDStep):
 
     ``state`` holds the device buffers ``pos`` [N, 3], ``vel`` [N, 3], ``forces`` [N, 3] (all float64), ``zeta``
     and ``eta`` [F] and ``step`` [1] (int64); ``pos`` is the buffer the captured neighbour list reads."""
+
+    LOG_FIELDS = LOG_FIELDS
 
     def __init__(self, model, example: Dict[str, torch.Tensor], masses, timestep_fs: float,
                  thermostat: Optional[str] = None, temperature=None, nvt_q=None, velocities=None,
@@ -159,7 +261,7 @@ class GraphedMD(GraphedMDStep):
         self.thermostat = thermostat
         self.dt = float(timestep_fs) * FS
         self.num_frames = F
-        self.host_reads = 0
+        self._init_blocks(dev)
         self._nblk = max(1, min(_MAX_CTAS, -(-int(counts.max()) // _THREADS)))
         self._atom_ptr = atom_ptr.to(dev)
         self._mass = mass.to(dev)
@@ -174,15 +276,8 @@ class GraphedMD(GraphedMDStep):
         self._forces = torch.zeros(N, 3, dtype=torch.float64, device=dev)
         self._zeta = torch.zeros(F, dtype=torch.float64, device=dev)
         self._eta = torch.zeros(F, dtype=torch.float64, device=dev)
-        self._step = torch.zeros(1, dtype=torch.int64, device=dev)
-        self._step_host = 0
-        self._sticky0 = torch.tensor([0, 0, -1, 0], dtype=torch.int64, device=dev)
-        self._sticky = self._sticky0.clone()
-        self._sticky_host = torch.zeros(4, dtype=torch.int64).pin_memory()
         self._part = torch.zeros(F, self._nblk, 2, dtype=torch.float64, device=dev)
         self._ke_part = torch.zeros(F, self._nblk, dtype=torch.float64, device=dev)
-        self._one = torch.ones(1, dtype=torch.int32, device=dev)
-        self._alloc_log(DEFAULT_LOG_ROWS)
         self._snap = [t.clone() for t in self._state_list()]
         self._forces.copy_(self._eager_forces(model, example))
         super().__init__(model, dict(example, pos=self._pos), capacity=capacity, warmup=warmup)
@@ -195,10 +290,6 @@ class GraphedMD(GraphedMDStep):
     def state(self) -> Dict[str, torch.Tensor]:
         return {"pos": self._pos, "vel": self._vel, "forces": self._forces, "zeta": self._zeta, "eta": self._eta,
                 "step": self._step}
-
-    def _alloc_log(self, rows: int) -> None:
-        self._log = torch.zeros(rows, self.num_frames, len(LOG_FIELDS), dtype=torch.float64, device=self._pos.device)
-        self._log_host = torch.zeros(rows, self.num_frames, len(LOG_FIELDS), dtype=torch.float64).pin_memory()
 
     def _eager_forces(self, model, example) -> torch.Tensor:
         """F(0): one eager neighbour list and model call at the initial positions (any edge count)."""
@@ -218,14 +309,6 @@ class GraphedMD(GraphedMDStep):
         return model(d)["forces"].detach().double()
 
     # ---- the captured step --------------------------------------------------------------------------------------
-    def _capture(self, model, example: Dict[str, torch.Tensor], capacity: int) -> None:
-        # the warm-up before the capture executes the step: keep the state as it was
-        saved = [t.clone() for t in self._state_list()]
-        super()._capture(model, example, capacity)
-        for t, s in zip(self._state_list(), saved):
-            t.copy_(s)
-        self._sticky.copy_(self._sticky0)
-
     def _run(self):
         L, st = _capi.lib(), ops._stream()
         P = ops._ptr
@@ -241,8 +324,7 @@ class GraphedMD(GraphedMDStep):
         f_new = out["forces"].detach().double().contiguous()
         _capi.check(L.nqb_md_kick(F, nb, P(self._atom_ptr), P(self._mass), P(f_new), P(self._zeta), dt, P(self._vel),
                                   P(self._forces), P(self._ke_part), st), "nqb_md_kick")
-        flags = getattr(ops._sorted_tls, "flags", None)  # the capture's deferred sortedness flags
-        sorted_flag = torch.stack([f.view(()) for f in flags]).min().view(1) if flags else self._one
+        sorted_flag = self._sorted_flag()
         e_pot = out["total_energy"].detach().double().reshape(-1).contiguous()
         _capi.check(L.nqb_md_log(F, nb, P(e_pot), P(self._ke_part), P(self._zeta), P(self._eta), P(self._Q),
                                  P(self._gkT), P(self._dof_kB), P(self._out["num_edges"]), P(self._out["overflow"]),
@@ -250,54 +332,16 @@ class GraphedMD(GraphedMDStep):
                     "nqb_md_log")
         return out
 
-    # ---- blocks -------------------------------------------------------------------------------------------------
-    def _read_block(self, k: int) -> torch.Tensor:
-        """The block's k log rows and the sticky flags, with one host synchronisation."""
-        R = self._log.shape[0]
-        a = self._step_host % R
-        n1 = min(k, R - a)
-        self._log_host[:n1].copy_(self._log[a:a + n1], non_blocking=True)
-        if n1 < k:
-            self._log_host[n1:k].copy_(self._log[:k - n1], non_blocking=True)
-        self._sticky_host.copy_(self._sticky, non_blocking=True)
-        done = torch.cuda.Event()
-        done.record()
-        done.synchronize()
-        self.host_reads += 1
-        return self._log_host[:k].clone()
-
     def run(self, n_steps: int, block: int = 50,
             on_block: Optional[Callable[[Dict[str, torch.Tensor]], None]] = None) -> Dict[str, torch.Tensor]:
         if n_steps < 0 or block < 1:
             raise ValueError(f"GraphedMD.run: needs n_steps >= 0 and block >= 1, got {n_steps}, {block}")
-        if block > self._log.shape[0]:
-            # the captured log kernel holds the log's pointer and length
-            self._alloc_log(block)
-            n = self.recaptures
-            self._recapture(self.capacity)
-            self.recaptures = n
+        self._fit_log(block)
         rows = []
         done = 0
         while done < n_steps:
             k = min(block, n_steps - done)
-            for s, t in zip(self._snap, self._state_list()):
-                s.copy_(t)
-            self._sticky.copy_(self._sticky0)
-            while True:
-                for _ in range(k):
-                    self.graph.replay()
-                self.replays += k
-                got = self._read_block(k)
-                if int(self._sticky_host[0]) == 0:
-                    break
-                for s, t in zip(self._snap, self._state_list()):
-                    t.copy_(s)
-                self._sticky.copy_(self._sticky0)
-                self._recapture(max(self.capacity + 1, math.ceil(1.02 * int(self._sticky_host[3]))))
-            if int(self._sticky_host[1]) != 0:
-                raise RuntimeError("GraphedMD: a step's edge list was not grouped by destination; its forces are "
-                                   "invalid")
-            self._step_host += k
+            got = self._run_block(k)
             done += k
             rows.append(got)
             if on_block is not None:

@@ -1675,6 +1675,7 @@ class NeighborListPlan:
         if self.variable_cell:
             self._params_host = torch.empty((len(block),), dtype=torch.uint8).pin_memory()
             self._params_event: Optional[torch.cuda.Event] = None
+            self.cell_error = torch.zeros((F,), dtype=torch.int32, device=dev)
 
     def _pack_frames(self, cells, invs):
         """The frames' device parameter blocks (``nqb_nl_frames_pack_capacity``, ctypes buffer) for ``cells`` on the
@@ -1742,6 +1743,26 @@ class NeighborListPlan:
             self._params_dev.copy_(self._params_host, non_blocking=True)
             self._params_event = torch.cuda.Event()
             self._params_event.record()
+
+    def set_cell_device(self, cells: torch.Tensor) -> torch.Tensor:
+        """``set_cell`` of a batched variable-cell plan from device cells [F, 3, 3] (float64, on the plan's device),
+        packed on the device (``nqb_nl_frames_set_cells``, one thread per frame): a stream-ordered launch with no host
+        synchronisation, so it can be captured together with ``run`` and the cells can move inside a CUDA graph.
+        Each frame's cell, inverse, search range on its fixed grid and null-edge shift are those of the host pack (the
+        inverse to a few ulp); the host copy ``pad_shift`` is not updated.  A frame whose cell is non-finite or
+        singular keeps its previous parameters and gets ``cell_error[f] = 1``; ``cell_error`` [F] int32 is returned,
+        and only the caller clears it.  ``ValueError`` on a plan without ``batch`` and ``variable_cell``, or for cells
+        of another shape, dtype or device."""
+        if self._fr is None or not self.variable_cell:
+            raise ValueError("NeighborListPlan.set_cell_device needs a plan built with batch= and variable_cell=True")
+        if (not torch.is_tensor(cells) or tuple(cells.shape) != (self.num_frames, 3, 3)
+                or cells.dtype != torch.float64 or not cells.is_cuda
+                or (self.device.index is not None and cells.device.index != self.device.index)):
+            raise ValueError(f"set_cell_device: cells must be float64 [{self.num_frames}, 3, 3] on {self.device}")
+        cells = cells.contiguous()
+        _capi.check(_capi.lib().nqb_nl_frames_set_cells(self.num_frames, _ptr(cells), _ptr(self._params_dev),
+                                                        _ptr(self.cell_error), _stream()), "nqb_nl_frames_set_cells")
+        return self.cell_error
 
     def _run_frames(self, pos: torch.Tensor) -> None:
         L = _capi.lib()
