@@ -457,6 +457,54 @@ int nqb_relax_finish(int F, int nblk, const double* part, int has_cell, double p
                      const int32_t* overflow, const int32_t* sorted, int64_t rows, int64_t* step, double* log,
                      int64_t* flags, nqb_stream_t st);
 
+/* Constant-pressure MD on the device (nqb_npt.cu, nequip_b200/npt.py GraphedNPT): isotropic MTK with Nose-Hoover
+ * chains on the particles (M = tchain members, tloop sub-steps) and on the barostat (Mp = pchain, ploop), in the
+ * splitting of Tuckerman et al. (2006), per frame f, all float64, in the units of the nqb_md kernels.  Atoms and CTAs
+ * as in the nqb_md kernels ((nblk, F) CTAs of 256 threads, nblk in [1, 65535], F <= 65535, no floating-point atomics).
+ * M, Mp in [0, NQB_NPT_MAX_CHAIN] (0: no chain), tloop, ploop >= 1.
+ * prm [F, NQB_NPT_PARAMS] = {kT, P, W, N_f, V0, N_f k_B, Q[NQB_NPT_MAX_CHAIN], Q'[NQB_NPT_MAX_CHAIN]} (alpha =
+ *   1 + 3 / N_f).  state [F, NQB_NPT_STATE] = {eps, v_eps, K2 = sum m v^2, xi[8], v_xi[8], eta[8], v_eta[8]};
+ *   vir [F,9] the model's virial at the state's positions; cell [F,9] = C0 e^eps; err [F] int32 sticky error flags;
+ *   coef [F, NQB_NPT_COEF] = {s, e^{-alpha v_eps dt/2}, kick factor, e^{v_eps dt}, drift factor, active, final scale};
+ *   work [F, NQB_NPT_STATE] a workspace.  NHC(h) is the chain half-step of DESIGN.md section 4.16.
+ * nqb_npt_pre (one thread per frame): a frame with err set gets coef {1, 1, 0, 1, 0, 0, 1} only.  Otherwise
+ *   NHC_baro(dt/2) on (v_eps, W); NHC_part(dt/2) on K2 (scale s); v_eps += dt/2 (alpha K2 + tr vir - 3 P V0 e^{3 eps}) / W;
+ *   the coefficients; eps += dt v_eps; cell = C0 e^eps.  If any result is non-finite: err[f] = 1, coef as for err,
+ *   state and cell unchanged.  Writes coef, work and, for a frame that passes, its state row and cell, nothing else.
+ * nqb_npt_move: the atoms of active frames: v = s v; v = v e + kf forces/m; pos = pos e^{v_eps dt} + df v.  Writes pos
+ *   and vel of those atoms, nothing else.
+ * nqb_npt_kick: the atoms of active frames: vel = vel e + kf f_new/m; forces = f_new; part [F, nblk] = sum m vel^2 of
+ *   CTA (b, f) (0 for an inactive frame).  Writes vel and forces of those atoms and all of part, nothing else.
+ * nqb_npt_post (one thread per frame, frames with err set get coef[6] = 1 only): K2 = sum of part[f, :] in index
+ *   order; v_eps += dt/2 G_eps / W with vir_new; NHC_part(dt/2) (scale coef[6]); NHC_baro(dt/2).  If any result is
+ *   non-finite: err[f] = 1, coef[6] = 1, state and vir unchanged; else state row and vir = vir_new.  Writes coef[:, 6],
+ *   work, err and those rows, nothing else.
+ * nqb_npt_scale: the atoms of active frames: vel = coef[6] vel.  Writes those velocities, nothing else.
+ * nqb_npt_log (one CTA): log row step % rows [rows, F, NQB_NPT_LOG_FIELDS] = {E_pot, K2/2, K2 / (N_f k_B), V,
+ *   (K2 + tr vir) / (3 V), H} with H = E_pot + K2/2 + W v_eps^2/2 + P V + sum Q_k v_xi_k^2/2 + N_f kT xi_0
+ *   + kT sum_{k>=1} xi_k + sum Q'_k v_eta_k^2/2 + kT sum eta_k; flags [4] as in nqb_md_log; step += 1.  Writes that
+ *   log row, flags and step, nothing else. */
+#define NQB_NPT_MAX_CHAIN 8
+#define NQB_NPT_PARAMS 22
+#define NQB_NPT_STATE 35
+#define NQB_NPT_COEF 7
+#define NQB_NPT_LOG_FIELDS 6
+#define NQB_NPT_SINHC_TAYLOR 0.1
+int nqb_npt_pre(int F, int M, int Mp, int tloop, int ploop, double dt, const double* prm, const double* C0 /* [F,9] */,
+                const double* vir, double* state, double* cell, double* coef, int32_t* err, double* work,
+                nqb_stream_t st);
+int nqb_npt_move(int F, int nblk, const int64_t* atom_ptr, const double* mass, const double* forces,
+                 const double* coef, double* pos, double* vel, nqb_stream_t st);
+int nqb_npt_kick(int F, int nblk, const int64_t* atom_ptr, const double* mass, const double* f_new,
+                 const double* coef, double* vel, double* forces, double* part, nqb_stream_t st);
+int nqb_npt_post(int F, int nblk, int M, int Mp, int tloop, int ploop, double dt, const double* prm,
+                 const double* part, const double* vir_new /* [F,9] */, double* state, double* vir, double* coef,
+                 int32_t* err, double* work, nqb_stream_t st);
+int nqb_npt_scale(int F, int nblk, const int64_t* atom_ptr, const double* coef, double* vel, nqb_stream_t st);
+int nqb_npt_log(int F, int M, int Mp, const double* e_pot, const double* prm, const double* state, const double* vir,
+                const int64_t* num_edges, const int32_t* overflow, const int32_t* sorted, int64_t rows, int64_t* step,
+                double* log, int64_t* flags, nqb_stream_t st);
+
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).
  * Together with nqb_gemm_grouped for the second layer this is ScalarMLPFunction (nequip/nn/mlp.py:80-195).

@@ -115,6 +115,13 @@ SIGNATURES = {
     "nqb_relax_finish": (
         _i32, [_i32, _i32, _vp, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _dbl, _vp, _vp, _vp, _vp, _vp, _i64,
                _vp, _vp, _vp, _vp]),
+    "nqb_npt_pre": (_i32, [_i32, _i32, _i32, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_npt_move": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_npt_kick": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_npt_post": (
+        _i32, [_i32, _i32, _i32, _i32, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_npt_scale": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp]),
+    "nqb_npt_log": (_i32, [_i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "nqb_mlp_hidden_fwd":(_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_fwd_rows": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),

@@ -62,7 +62,7 @@ def ensure_runtime(force: bool = False) -> str:
     """Build (if stale) and return the path of libnqb.so."""
     out = runtime_lib_path()
     cus = [os.path.join(CSRC, n) for n in ("nqb_runtime.cu", "nqb_mlp.cu", "nqb_gemm.cu", "nqb_nl.cu",
-                                             "nqb_pair.cu", "nqb_md.cu", "nqb_relax.cu")]
+                                             "nqb_pair.cu", "nqb_md.cu", "nqb_relax.cu", "nqb_npt.cu")]
     srcs = cus + [os.path.join(INCLUDE, "nqb.h"), os.path.join(CSRC, "nqb_tc.cuh")]
     with _lock:
         if force or _newer(srcs, out):

@@ -184,7 +184,7 @@ class GraphedMD(BlockDriver):
     Maxwell-Boltzmann distribution at ``temperature`` (``seed``), or are zero without a temperature.  As the reference
     does, the initial velocities lose their rotation and then their centre-of-mass momentum, frame by frame.  The forces
     F(0) at the initial positions come from one eager neighbour list and model call.  ``variable_cell=True`` raises:
-    there is no barostat.  Invalid arguments raise ``ValueError`` before any CUDA work.
+    this driver has no barostat (constant-pressure MD is ``npt.GraphedNPT``).  Invalid arguments raise ``ValueError`` before any CUDA work.
 
     ``run(n_steps, block=50, on_block=None)`` advances the state by ``n_steps`` and returns the log, a dict of host
     float64 tensors [n_steps, F] named by ``LOG_FIELDS``: the potential energy (the model's ``total_energy``), the
