@@ -505,6 +505,51 @@ int nqb_npt_log(int F, int M, int Mp, const double* e_pot, const double* prm, co
                 const int64_t* num_edges, const int32_t* overflow, const int32_t* sorted, int64_t rows, int64_t* step,
                 double* log, int64_t* flags, nqb_stream_t st);
 
+/* The fully flexible cell (nqb_npt.cu, GraphedNPT(barostat="flexible"), DESIGN.md section 4.17): fully flexible MTK
+ * with a symmetric cell velocity v_g, chains, CTAs, err and the launch limits as above.  prm has the isotropic layout
+ * with W = W_g = (N_f + 3) kT tau_P^2 / 3 and Q'_1 = 6 kT tau_P^2 (V0 unused).  state [F, NQB_NPTF_STATE] = {v_g[9],
+ *   Kt[9] = sum m v (x) v, xi[8], v_xi[8], eta[8], v_eta[8]} (3x3 row-major, symmetric); cell [F,9] the cell (rows are
+ *   lattice vectors); coef [F, NQB_NPTF_COEF] = {s, active, final scale, E_v[9], K[9], E_r[9], D[9]}; work [F,
+ *   NQB_NPTF_STATE].  G_g = sym(Kt + vir) - P |det cell| I + (tr Kt / N_f) I; the barostat chain couples to W_g tr(v_g^2)
+ *   with 6 degrees of freedom; v_g = O diag(lambda) O^T by NQB_NPTF_JACOBI_SWEEPS cyclic Jacobi sweeps, mu = lambda +
+ *   tr(v_g) / N_f, E_v = O e^{-mu dt/2} O^T, K = O (dt/2) e^{-mu dt/4} sinhc(mu dt/4) O^T, E_r = O e^{lambda dt} O^T,
+ *   D = O dt e^{lambda dt/2} sinhc(lambda dt/2) O^T.
+ * nqb_nptf_pre (one thread per frame): a frame with err set gets coef {1, 0, 1, I, 0, I, 0} only.  Otherwise
+ *   NHC_baro(dt/2) (v_g scaled); NHC_part(dt/2) (Kt *= s^2); v_g += dt/2 G_g / W_g with vir and the cell; E_v, K, E_r, D;
+ *   cell = cell E_r.  If any result is non-finite: err[f] = 1, coef as for err, state and cell unchanged.  Writes coef,
+ *   work and, for a frame that passes, its state row and cell, nothing else.
+ * nqb_nptf_move: the atoms of active frames: v = s v; v = E_v v + K forces/m; pos = E_r pos + D v.  Writes pos and vel
+ *   of those atoms, nothing else.
+ * nqb_nptf_kick: the atoms of active frames: vel = E_v vel + K f_new/m; forces = f_new; part [F, nblk, 6] = sum m vel
+ *   (x) vel of CTA (b, f) as {xx, yy, zz, yz, xz, xy} (0 for an inactive frame).  Writes vel and forces of those atoms
+ *   and all of part, nothing else.
+ * nqb_nptf_post (one thread per frame, frames with err set get coef[2] = 1 only): Kt = sum of part[f, :, :] in index
+ *   order; v_g += dt/2 G_g / W_g with vir_new and the cell; NHC_part(dt/2) (scale coef[2], Kt *= s^2); NHC_baro(dt/2).
+ *   If any result is non-finite: err[f] = 1, coef[2] = 1, state and vir unchanged; else state row and vir = vir_new.
+ *   Writes coef[:, 2], work, err and those rows, nothing else.
+ * nqb_nptf_scale: the atoms of active frames: vel = coef[2] vel.  Writes those velocities, nothing else.
+ * nqb_nptf_log (one CTA): log row step % rows [rows, F, NQB_NPTF_LOG_FIELDS] = {E_pot, tr Kt/2, tr Kt / (N_f k_B), V,
+ *   tr(P_int) / 3, H, cell[9], P_int[9]} with V = |det cell|, P_int = (Kt + vir) / V and H = E_pot + tr Kt/2
+ *   + W_g tr(v_g^2)/2 + P V + sum Q_k v_xi_k^2/2 + N_f kT xi_0 + kT sum_{k>=1} xi_k + sum Q'_k v_eta_k^2/2 + 6 kT eta_0
+ *   + kT sum_{k>=1} eta_k; flags [4] as in nqb_md_log; step += 1.  Writes that log row, flags and step, nothing else. */
+#define NQB_NPTF_STATE 50
+#define NQB_NPTF_COEF 39
+#define NQB_NPTF_LOG_FIELDS 24
+#define NQB_NPTF_JACOBI_SWEEPS 6
+int nqb_nptf_pre(int F, int M, int Mp, int tloop, int ploop, double dt, const double* prm, const double* vir,
+                 double* state, double* cell, double* coef, int32_t* err, double* work, nqb_stream_t st);
+int nqb_nptf_move(int F, int nblk, const int64_t* atom_ptr, const double* mass, const double* forces,
+                  const double* coef, double* pos, double* vel, nqb_stream_t st);
+int nqb_nptf_kick(int F, int nblk, const int64_t* atom_ptr, const double* mass, const double* f_new,
+                  const double* coef, double* vel, double* forces, double* part, nqb_stream_t st);
+int nqb_nptf_post(int F, int nblk, int M, int Mp, int tloop, int ploop, double dt, const double* prm,
+                  const double* part, const double* vir_new, const double* cell, double* state, double* vir,
+                  double* coef, int32_t* err, double* work, nqb_stream_t st);
+int nqb_nptf_scale(int F, int nblk, const int64_t* atom_ptr, const double* coef, double* vel, nqb_stream_t st);
+int nqb_nptf_log(int F, int M, int Mp, const double* e_pot, const double* prm, const double* state, const double* vir,
+                 const double* cell, const int64_t* num_edges, const int32_t* overflow, const int32_t* sorted,
+                 int64_t rows, int64_t* step, double* log, int64_t* flags, nqb_stream_t st);
+
 /* First radial layer (K = 8, CUDA cores):  h[E,128] = silu(emb[E,8] @ W1s[8,128])  and
  * grad_emb[E,8] = (grad_h * silu'(emb @ W1s)) @ W1s^T  (pre-activation recomputed, nothing saved).
  * Together with nqb_gemm_grouped for the second layer this is ScalarMLPFunction (nequip/nn/mlp.py:80-195).

@@ -122,6 +122,13 @@ SIGNATURES = {
         _i32, [_i32, _i32, _i32, _i32, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nqb_npt_scale": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp]),
     "nqb_npt_log": (_i32, [_i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "nqb_nptf_pre": (_i32, [_i32, _i32, _i32, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nptf_move": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nptf_kick": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nptf_post": (
+        _i32, [_i32, _i32, _i32, _i32, _i32, _i32, _dbl, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nqb_nptf_scale": (_i32, [_i32, _i32, _vp, _vp, _vp, _vp]),
+    "nqb_nptf_log": (_i32, [_i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "nqb_mlp_hidden_fwd":(_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_fwd_rows": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),

@@ -1,5 +1,5 @@
-"""Constant-pressure (NPT) molecular dynamics on the device: isotropic MTK with Nose-Hoover chains inside one captured
-step.
+"""Constant-pressure (NPT) molecular dynamics on the device: isotropic or fully flexible MTK with Nose-Hoover chains
+inside one captured step.
 
 The equations are Martyna, Tobias & Klein, J. Chem. Phys. 101, 4177 (1994) for an isotropic cell, integrated with the
 measure-preserving splitting of Tuckerman, Alejandre, Lopez-Rendon, Jochim & Martyna, J. Phys. A 39, 5629 (2006); the
@@ -8,7 +8,10 @@ particles and the barostat each carry a Nose-Hoover chain (Martyna, Tuckerman, T
 of the update, the drift of positions and cell, the cell packed into the device neighbour list
 (``NeighborListPlan.set_cell_device``), the list, the model with stress, the second half of the update and one row of
 a log -- as one CUDA graph for a batch of frames, and ``run(n_steps, block=K)`` replays it K times per host read
-(DESIGN.md section 4.16).  Units are those of ``md``: Angstrom, eV, amu, ASE's CODATA-2014 ``KB`` and ``FS``.
+(DESIGN.md section 4.16).  ``barostat="flexible"`` lets the cell's shape move too: the fully flexible MTK equations
+(Martyna, Tobias & Klein 1994; Martyna, Tuckerman, Tobias & Klein 1996) with a symmetric 3x3 cell velocity, in the
+same splitting (DESIGN.md section 4.17).  Units are those of ``md``: Angstrom, eV, amu, ASE's CODATA-2014 ``KB``
+and ``FS``.
 """
 from __future__ import annotations
 
@@ -28,6 +31,13 @@ LOG_FIELDS = ("e_pot", "e_kin", "temperature", "volume", "pressure", "conserved"
 MAX_CHAIN = 8
 _NS, _NP, _NC = 35, 22, 7  # NQB_NPT_STATE, NQB_NPT_PARAMS, NQB_NPT_COEF
 _XI, _VXI, _ETA, _VETA = 3, 3 + MAX_CHAIN, 3 + 2 * MAX_CHAIN, 3 + 3 * MAX_CHAIN  # offsets in a state row
+#: the barostats ``GraphedNPT`` runs
+BAROSTATS = ("isotropic", "flexible")
+# the flexible cell: NQB_NPTF_STATE, NQB_NPTF_COEF, NQB_NPTF_LOG_FIELDS and the offsets in its state row
+_NFS, _NFC, _NFL = 50, 39, 24
+_FKT, _FXI, _FVXI, _FETA, _FVETA = 9, 18, 18 + MAX_CHAIN, 18 + 2 * MAX_CHAIN, 18 + 3 * MAX_CHAIN
+#: the barostat chain's degrees of freedom under the flexible barostat: the components of a symmetric v_g
+FLEX_DOF = 6
 
 
 def _per_frame(value, F: int, what: str) -> torch.Tensor:
@@ -80,13 +90,29 @@ class GraphedNPT(BlockDriver):
 
     ``state`` holds the device buffers ``pos``, ``vel``, ``forces`` [N, 3], ``virial`` and ``cell`` [F, 3, 3], ``eps``,
     ``v_eps`` and ``K2`` (sum m v^2) [F], the chains ``xi``, ``v_xi`` [F, tchain] and ``eta``, ``v_eta`` [F, pchain],
-    ``error`` [F] int32 and ``step`` [1] (views of the buffers the captured step reads and writes)."""
+    ``error`` [F] int32 and ``step`` [1] (views of the buffers the captured step reads and writes).
+
+    ``barostat="flexible"`` runs the fully flexible MTK barostat instead (DESIGN.md section 4.17): a symmetric cell
+    velocity v_g [3, 3] (so the cell does not rotate) driven by sym(Kt + virial) - P V I + (tr Kt / N_f) I, with
+    Kt = sum m v (x) v, V = |det cell| and the cell's rows moving as da/dt = v_g a.  Its mass is
+    W_g = (N_f + 3) k_B T tau_P^2 / 3 and its chain couples to W_g tr(v_g^2) with 6 degrees of freedom
+    (Q'_1 = 6 k_B T tau_P^2, Q'_k = k_B T tau_P^2).  Every other argument, the blocks, rollback and freezing are as
+    above.  ``state`` then holds ``pos``, ``vel``, ``forces``, ``virial``, ``cell``, ``v_g`` and ``kinetic`` (Kt)
+    [F, 3, 3], the chains, ``error`` and ``step`` (no ``eps``: the cell itself is the state), and ``run`` also returns
+    ``cell`` and ``pressure_tensor`` (Kt + virial) / V [n_steps, F, 3, 3]; ``volume`` is |det cell| and ``pressure``
+    tr(pressure_tensor) / 3, and ``conserved`` carries W_g tr(v_g^2) / 2 and 6 k_B T eta_1.  A liquid has no shear
+    resistance, so its cell drifts in shape under this barostat: use ``"isotropic"`` for liquids."""
 
     LOG_FIELDS = LOG_FIELDS
 
     def __init__(self, model, example: Dict[str, torch.Tensor], masses, timestep_fs: float, temperature, pressure, *,
                  tdamp_fs, pdamp_fs, tchain: int = 3, pchain: int = 3, tloop: int = 1, ploop: int = 1,
-                 velocities=None, capacity: Optional[int] = None, seed: int = 0, warmup: int = 3):
+                 velocities=None, capacity: Optional[int] = None, seed: int = 0, warmup: int = 3,
+                 barostat: str = "isotropic"):
+        if barostat not in BAROSTATS:
+            raise ValueError(f"GraphedNPT: barostat must be one of {BAROSTATS}, got {barostat!r}")
+        self.barostat = barostat
+        flex = barostat == "flexible"
         if not (math.isfinite(float(timestep_fs)) and float(timestep_fs) > 0):
             raise ValueError(f"GraphedNPT: timestep_fs must be finite and positive, got {timestep_fs}")
         for name, v, lo, hi in (("tchain", tchain, 0, MAX_CHAIN), ("pchain", pchain, 0, MAX_CHAIN),
@@ -154,6 +180,13 @@ class GraphedNPT(BlockDriver):
         # K2 = sum m v^2 per frame, correctly rounded (math.fsum), so the starting state depends only on the inputs
         k2 = [math.fsum((mass[int(atom_ptr[f]):int(atom_ptr[f + 1])] * (vel[int(atom_ptr[f]):int(atom_ptr[f + 1])] ** 2)
                          .sum(1)).tolist()) for f in range(F)]
+        if flex:  # Kt = sum m v (x) v per frame and component, correctly rounded too
+            kt = torch.zeros(F, 3, 3, dtype=torch.float64)
+            for f in range(F):
+                a, b = int(atom_ptr[f]), int(atom_ptr[f + 1])
+                for i in range(3):
+                    for j in range(i, 3):
+                        kt[f, i, j] = kt[f, j, i] = math.fsum((mass[a:b] * vel[a:b, i] * vel[a:b, j]).tolist())
 
         dev = pos.device
         self.dt = float(timestep_fs) * FS
@@ -169,11 +202,13 @@ class GraphedNPT(BlockDriver):
         prm = torch.ones(F, _NP, dtype=torch.float64)
         prm[:, 0], prm[:, 1], prm[:, 3], prm[:, 5] = kT, pres, Nf, Nf * KB
         prm[:, 2] = (Nf + 3.0) * kT * tau_p ** 2
+        if flex:
+            prm[:, 2] /= 3.0  # W_g
         prm[:, 4] = torch.from_numpy(cells0).double().det().abs()
         for k in range(int(tchain)):
             prm[:, 6 + k] = (Nf if k == 0 else 1.0) * kT * tau_t ** 2
         for k in range(int(pchain)):
-            prm[:, 6 + MAX_CHAIN + k] = kT * tau_p ** 2
+            prm[:, 6 + MAX_CHAIN + k] = (FLEX_DOF if flex and k == 0 else 1.0) * kT * tau_p ** 2
         self._prm = prm.to(dev)
         f64 = dict(dtype=torch.float64, device=dev)
         self._pos = pos.detach().double().clone().to(dev)
@@ -181,13 +216,20 @@ class GraphedNPT(BlockDriver):
         self._forces = torch.zeros(N, 3, **f64)
         self._vir = torch.zeros(F, 3, 3, **f64)
         self._cell = torch.from_numpy(cells0.copy()).to(dev)
-        self._C0 = self._cell.clone()
-        self._st = torch.zeros(F, _NS, **f64)
-        self._st[:, 2] = torch.tensor(k2, dtype=torch.float64)
         self._err = torch.zeros(F, dtype=torch.int32, device=dev)
-        self._coef = torch.zeros(F, _NC, **f64)
-        self._work = torch.zeros(F, _NS, **f64)
-        self._part = torch.zeros(F, self._nblk, **f64)
+        if flex:
+            self._st = torch.zeros(F, _NFS, **f64)
+            self._st[:, _FKT:_FKT + 9] = kt.reshape(F, 9)
+            self._coef = torch.zeros(F, _NFC, **f64)
+            self._work = torch.zeros(F, _NFS, **f64)
+            self._part = torch.zeros(F, self._nblk, 6, **f64)
+        else:
+            self._C0 = self._cell.clone()
+            self._st = torch.zeros(F, _NS, **f64)
+            self._st[:, 2] = torch.tensor(k2, dtype=torch.float64)
+            self._coef = torch.zeros(F, _NC, **f64)
+            self._work = torch.zeros(F, _NS, **f64)
+            self._part = torch.zeros(F, self._nblk, **f64)
         self._err_host = torch.zeros(F, dtype=torch.int32).pin_memory()
         self._cerr_host = torch.zeros(F, dtype=torch.int32).pin_memory()
         self._snap = [t.clone() for t in self._state_list()]
@@ -203,9 +245,24 @@ class GraphedNPT(BlockDriver):
     def _state_list(self):
         return [self._pos, self._vel, self._forces, self._vir, self._cell, self._st, self._err, self._step]
 
+    def _alloc_log(self, rows: int) -> None:
+        if self.barostat != "flexible":
+            return super()._alloc_log(rows)
+        shape = (rows, self.num_frames, _NFL)  # LOG_FIELDS, the cell [9] and the pressure tensor [9]
+        self._log = torch.zeros(shape, dtype=torch.float64, device=self._step.device)
+        self._log_host = torch.zeros(shape, dtype=torch.float64).pin_memory()
+
     @property
     def state(self) -> Dict[str, torch.Tensor]:
         M, Mp = self.chains[:2]
+        if self.barostat == "flexible":
+            F = self.num_frames
+            return {"pos": self._pos, "vel": self._vel, "forces": self._forces, "virial": self._vir,
+                    "cell": self._cell, "v_g": self._st[:, 0:9].view(F, 3, 3),
+                    "kinetic": self._st[:, _FKT:_FKT + 9].view(F, 3, 3),
+                    "xi": self._st[:, _FXI:_FXI + M], "v_xi": self._st[:, _FVXI:_FVXI + M],
+                    "eta": self._st[:, _FETA:_FETA + Mp], "v_eta": self._st[:, _FVETA:_FVETA + Mp],
+                    "error": self._err, "step": self._step}
         return {"pos": self._pos, "vel": self._vel, "forces": self._forces, "virial": self._vir, "cell": self._cell,
                 "eps": self._st[:, 0], "v_eps": self._st[:, 1], "K2": self._st[:, 2],
                 "xi": self._st[:, _XI:_XI + M], "v_xi": self._st[:, _VXI:_VXI + M],
@@ -243,6 +300,8 @@ class GraphedNPT(BlockDriver):
         # the list and the model read the state's position and cell buffers themselves, which the integrator moves
         self.static["pos"] = self._pos
         self.static["cell"] = self._cell
+        if self.barostat == "flexible":
+            return self._run_flexible()
         _capi.check(L.nqb_npt_pre(F, M, Mp, tl, pl, dt, P(self._prm), P(self._C0), P(self._vir), P(self._st),
                                   P(self._cell), P(self._coef), P(self._err), P(self._work), st), "nqb_npt_pre")
         _capi.check(L.nqb_npt_move(F, nb, P(self._atom_ptr), P(self._mass), P(self._forces), P(self._coef),
@@ -260,6 +319,40 @@ class GraphedNPT(BlockDriver):
         _capi.check(L.nqb_npt_log(F, M, Mp, P(e_pot), P(self._prm), P(self._st), P(self._vir),
                                   P(self._out["num_edges"]), P(self._out["overflow"]), P(self._sorted_flag()),
                                   self._log.shape[0], P(self._step), P(self._log), P(self._sticky), st), "nqb_npt_log")
+        return out
+
+    def _run_flexible(self):
+        L, st, P = _capi.lib(), ops._stream(), ops._ptr
+        F, nb, dt = self.num_frames, self._nblk, self.dt
+        M, Mp, tl, pl = self.chains
+        _capi.check(L.nqb_nptf_pre(F, M, Mp, tl, pl, dt, P(self._prm), P(self._vir), P(self._st), P(self._cell),
+                                   P(self._coef), P(self._err), P(self._work), st), "nqb_nptf_pre")
+        _capi.check(L.nqb_nptf_move(F, nb, P(self._atom_ptr), P(self._mass), P(self._forces), P(self._coef),
+                                    P(self._pos), P(self._vel), st), "nqb_nptf_move")
+        self.plan.set_cell_device(self._cell)
+        out = super()._run()
+        f_new = out["forces"].detach().double().contiguous()
+        _capi.check(L.nqb_nptf_kick(F, nb, P(self._atom_ptr), P(self._mass), P(f_new), P(self._coef), P(self._vel),
+                                    P(self._forces), P(self._part), st), "nqb_nptf_kick")
+        vir_new = out["virial"].detach().double().contiguous()
+        _capi.check(L.nqb_nptf_post(F, nb, M, Mp, tl, pl, dt, P(self._prm), P(self._part), P(vir_new), P(self._cell),
+                                    P(self._st), P(self._vir), P(self._coef), P(self._err), P(self._work), st),
+                    "nqb_nptf_post")
+        _capi.check(L.nqb_nptf_scale(F, nb, P(self._atom_ptr), P(self._coef), P(self._vel), st), "nqb_nptf_scale")
+        e_pot = out["total_energy"].detach().double().reshape(-1).contiguous()
+        _capi.check(L.nqb_nptf_log(F, M, Mp, P(e_pot), P(self._prm), P(self._st), P(self._vir), P(self._cell),
+                                   P(self._out["num_edges"]), P(self._out["overflow"]), P(self._sorted_flag()),
+                                   self._log.shape[0], P(self._step), P(self._log), P(self._sticky), st),
+                    "nqb_nptf_log")
+        return out
+
+    def _fields(self, rows: torch.Tensor) -> Dict[str, torch.Tensor]:
+        """Log rows [k, F, width] as the dict ``run`` returns."""
+        out = {name: rows[:, :, j] for j, name in enumerate(LOG_FIELDS)}
+        if self.barostat == "flexible":
+            k, F = rows.shape[:2]
+            out["cell"] = rows[:, :, 6:15].reshape(k, F, 3, 3)
+            out["pressure_tensor"] = rows[:, :, 15:24].reshape(k, F, 3, 3)
         return out
 
     def _check_block(self) -> None:
@@ -285,6 +378,6 @@ class GraphedNPT(BlockDriver):
             done += k
             rows.append(got)
             if on_block is not None:
-                on_block({name: got[:, :, j] for j, name in enumerate(LOG_FIELDS)})
-        log = torch.cat(rows) if rows else torch.zeros(0, self.num_frames, len(LOG_FIELDS), dtype=torch.float64)
-        return {name: log[:, :, j].clone() for j, name in enumerate(LOG_FIELDS)}
+                on_block(self._fields(got))
+        log = torch.cat(rows) if rows else torch.zeros(0, self.num_frames, self._log.shape[2], dtype=torch.float64)
+        return {name: v.clone() for name, v in self._fields(log).items()}

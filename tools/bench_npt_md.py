@@ -1,6 +1,8 @@
 """Constant-pressure MD: ``GraphedMDStep(variable_cell=True)`` plus the same isotropic MTK update in eager torch on the
 device and ``g(pos, cell)`` (a host ``set_cell``) every step (arm A, what a user writes today) against ``GraphedNPT``
-with blocks of 1 and 50 steps (arms B, C).
+with blocks of 1 and 50 steps (arms B, C).  With ``--flexible`` the arms are C and F:
+``GraphedNPT(barostat="flexible")`` with blocks of 50 steps, the fully flexible cell (DESIGN.md section 4.17),
+alternated within each round.
 
 Workloads:
   * water_1k_l2_f32   the 1 000-atom water box, l_max 2, 4 layers, 32 features (tools/bench_md.py);
@@ -15,7 +17,7 @@ steps after ``--warmup`` steps; arm A against arm C over 50 steps from one state
 the drift of H.  The card's name, power limit and SM clock are read in the same process.
 
     python tools/bench_npt_md.py [--workloads ...] [--steps 100] [--warmup 20] [--rounds 3] [--long 40000]
-                                 [--out FILE.jsonl]
+                                 [--flexible] [--out FILE.jsonl]
 """
 import argparse
 import json
@@ -38,6 +40,7 @@ from nequip_b200.npt import GPA, GraphedNPT  # noqa: E402
 
 WORKLOADS = ("water_1k_l2_f32", "S_li3po4_10k", "water_125_x128")
 ARMS = (("A_host_update", None), ("B_block_1", 1), ("C_block_50", 50))
+FLEX_ARMS = (("C_block_50", 50), ("F_flexible_block_50", 50))
 MASS = {"H": 1.008, "O": 15.999, "Li": 6.94, "P": 30.974}
 BAR = 1e-4 * GPA
 BATH = dict(temperature=300.0, pressure=BAR, tdamp_fs=100.0, pdamp_fs=1000.0)
@@ -180,6 +183,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--long", type=int, default=0, help="steps of the long water_1k run (0: none)")
+    ap.add_argument("--flexible", action="store_true",
+                    help="time the flexible barostat against C_block_50 (and skip the A-vs-C agreement)")
     ap.add_argument("--out", default=None, help="append the JSON lines to this file")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -198,17 +203,18 @@ def main():
         model, ex, masses = workload(name, dev)
         atoms, frames = ex["pos"].shape[0], int(ex["num_atoms"].numel())
 
-        def make(block):
-            npt = GraphedNPT(model, ex, masses, DT_FS, tchain=CHAIN, pchain=CHAIN, seed=1, **BATH)
+        def make(block, barostat="isotropic"):
+            npt = GraphedNPT(model, ex, masses, DT_FS, tchain=CHAIN, pchain=CHAIN, seed=1, barostat=barostat, **BATH)
             if block is None:
                 vel = npt.state["vel"].clone()
                 del npt
                 return HostNPT(model, ex, masses, vel)
             return npt
 
-        objs = {arm: make(block) for arm, block in ARMS}
+        arms = FLEX_ARMS if args.flexible else ARMS
+        objs = {arm: make(block, "flexible" if arm.startswith("F_") else "isotropic") for arm, block in arms}
         for rnd in range(args.rounds):
-            for arm, block in ARMS:
+            for arm, block in arms:
                 obj = objs[arm]
                 obj.run(args.warmup, block=block or 1)
                 torch.cuda.synchronize()
@@ -219,8 +225,18 @@ def main():
                 torch.cuda.synchronize()
                 emit({"workload": name, "what": "npt_step", "arm": arm, "round": rnd, "atoms": atoms,
                       "frames": frames, "steps": args.steps, "ms_per_step": e0.elapsed_time(e1) / args.steps,
-                      "block": block, "recaptures": obj.recaptures})
+                      "block": block, "recaptures": obj.recaptures,
+                      "barostat": getattr(obj, "barostat", "isotropic")})
+        if args.flexible:
+            cell = objs["F_flexible_block_50"].state["cell"]
+            off = cell - torch.diag_embed(cell.diagonal(dim1=1, dim2=2))
+            emit({"workload": name, "what": "flexible_cell", "atoms": atoms, "frames": frames,
+                  "steps": objs["F_flexible_block_50"].replays, "max_abs_offdiag_cell": float(off.abs().max())})
         del objs
+        if args.flexible:
+            del model, ex
+            torch.cuda.empty_cache()
+            continue
         # A against C over 50 steps from one state
         a, c = make(None), make(50)
         a.run(50)
