@@ -5,7 +5,7 @@ from __future__ import annotations
 
 from typing import List, Tuple
 
-from .codegen import TPSignature
+from .codegen import GenOptions, TPSignature
 from .irreps import Irreps, build_tp_instructions
 
 # the reference's kernel test grid (tests/unit/nn/test_tp_scatter_kernel.py:38-55)
@@ -61,4 +61,29 @@ def all_known() -> List[TPSignature]:
     uniq = {}
     for s in sigs:
         uniq[s.canonical()] = s
+    return list(uniq.values())
+
+
+def fused_families() -> List[TPSignature]:
+    """Layer signatures of the model families on which the fused radial-MLP -> TP -> scatter kernel is tested
+    (tests/test_tp_fused_signatures.py): every layer of l_max 1 and 2 at 32, 64 and 128 features and of l_max 3 at 32
+    and 64 features, with and without parity.  Left out, as nvcc takes too long on them for every build: the middle
+    layers of l_max 3 at 64 features with parity (64 and 68 paths, 1.6 MB of generated source each) and l_max 3 at 128
+    features (over 20 minutes for one layer)."""
+    sigs = []
+    for parity in (True, False):
+        for (lm, nf, nl) in [(1, 32, 4), (1, 64, 4), (1, 128, 4), (2, 32, 4), (2, 64, 4), (2, 128, 4), (3, 32, 5)]:
+            sigs += nequip_layer_signatures(lm, nf, nl, parity)
+        sigs += [s for li, s in enumerate(nequip_layer_signatures(3, 64, 5, parity)) if not (parity and li in (2, 3))]
+    return sigs
+
+
+def prebuilt() -> List[Tuple[TPSignature, GenOptions]]:
+    """The kernel libraries ``__graft_entry__.build()`` compiles: every signature of ``all_known()`` in both layouts,
+    and ``fused_families()`` in the ir_mul layout, the only one with a fused kernel."""
+    pairs = [(s, GenOptions(layout=lay)) for s in all_known() for lay in ("mul_ir", "ir_mul")]
+    pairs += [(s, GenOptions(layout="ir_mul")) for s in fused_families()]
+    uniq = {}
+    for s, o in pairs:
+        uniq.setdefault((s.canonical(), o.layout), (s, o))
     return list(uniq.values())
