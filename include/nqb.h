@@ -580,6 +580,14 @@ int nqb_edge_pairs(const int64_t* edge_index, int64_t E, int64_t N, const double
  * u < min(*count, capacity).  Writes rows < U of h [capacity, hidden] only; the grid depends on capacity alone. */
 int nqb_mlp_hidden_fwd_rows(const float* emb, const float* W1s, const int64_t* pair_rows, const int64_t* count,
                             int64_t capacity, int num_bessel, int hidden, float* h, nqb_stream_t st);
+/* Its backward on the same slots: for u < U = min(*count, capacity), with p = emb[pair_rows[u][0]] @ W1s,
+ *   grad_emb[pair_rows[u][0]] = (grad_h[u] * silu'(p)) @ W1s^T  and  grad_emb[pair_rows[u][1]] = 0 (when >= 0).
+ * grad_h [capacity, hidden] is read in rows < U (the slot's gradient, summed over both edges).  Writes exactly the
+ * grad_emb rows named in pair_rows[0 .. U): every row when the map covers all E edges.  pair_rows must be 16-byte
+ * aligned; the grid depends on capacity alone. */
+int nqb_mlp_hidden_bwd_rows(const float* emb, const float* W1s, const float* grad_h, const int64_t* pair_rows,
+                            const int64_t* count, int64_t capacity, int num_bessel, int hidden, float* grad_emb,
+                            nqb_stream_t st);
 
 /* Grouped fp32-accurate GEMM on the tensor cores (wgmma tf32, 3xTF32, segmented fp32
  * accumulation):  C_p[M, N_p] (+)= rowscale_p[m] * A_p[M, K_p] @ B_p[K_p, N_p]  for a list of problems
@@ -630,6 +638,14 @@ int nqb_gemm_grouped_act(const void* descs_dev, int ndesc, int ntiles_total, con
 int nqb_gemm_grouped_pairs(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
                            int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
                            const int64_t* pair_rows, const int64_t* count_dev, int64_t capacity, nqb_stream_t st);
+/* The transpose direction on the same slots (plain problems only): M = min(*count_dev, capacity) is read on the
+ * device and row m of the product is (A[pair_rows[m][0]] + A[pair_rows[m][1]]) @ B, the second row only when
+ * pair_rows[m][1] >= 0 (the fp32 sum is formed in the kernel), stored to C row m.  Write contract: C rows < M, columns
+ * < N_p are written, nothing else; A is read in the rows listed in pair_rows[0 .. M), columns < K_p only.
+ * pair_rows must be 16-byte aligned and capacity < 2^31; the grid depends on capacity alone (capturable). */
+int nqb_gemm_grouped_pair_sum(const void* descs_dev, int ndesc, int ntiles_total, const int32_t* tile_ctas_dev,
+                              int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
+                              const int64_t* pair_rows, const int64_t* count_dev, int64_t capacity, nqb_stream_t st);
 
 /* Gate nonlinearity (e3nn nn.Gate with normalize2mom'd SiLU for even / tanh for odd scalars and gates,
  * nequip/nn/convnetlayer.py:42-56,104-112), one kernel per direction.  Column tables (device, int32) are

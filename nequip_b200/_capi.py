@@ -132,6 +132,7 @@ SIGNATURES = {
     "nqb_mlp_hidden_fwd":(_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_bwd": (_i32, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_mlp_hidden_fwd_rows": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
+    "nqb_mlp_hidden_bwd_rows": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "nqb_edge_pairs_work_size": (_i64, [_i64]),
     "nqb_edge_pairs": (_i32, [_vp, _i64, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nqb_gemm_prepared_floats": (_i64, [_i32, _i32]),
@@ -141,6 +142,7 @@ SIGNATURES = {
     "nqb_gemm_grouped": (_i32, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i64, _i64, _vp]),
     "nqb_gemm_grouped_act": (_i32, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp]),
     "nqb_gemm_grouped_pairs": (_i32, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "nqb_gemm_grouped_pair_sum": (_i32, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
 }
 
 

@@ -28,6 +28,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "../../include/nqb.h"
 #include "nqb_tc.cuh"
 
@@ -59,6 +61,22 @@ struct Smem {
   float alo[NWG][NLO][MW * KC];      // 2 x 2 x 8 KB: their tf32 low parts
   uint64_t b_full[BSLOTS], b_empty[BSLOTS];
 };
+
+// the gathered-sum A operand (ROWS = PAIRS_A) lands each partner chunk in the low-part slot of its chunk, so the
+// low-part ring has RAW slots instead of NLO: 128 + 48 + 48 KB
+struct SmemPairsA {
+  float b[BSLOTS][BLOCK_FLOATS];
+  float araw[NWG][RAW][MW * KC];  // representative rows; the low-part pass overwrites them with the sums
+  float alo[NWG][RAW][MW * KC];   // partner rows (zero-filled when a slot has none); overwritten with the low parts
+  uint64_t b_full[BSLOTS], b_empty[BSLOTS];
+};
+
+// how A rows and C rows map to M (nqb_gemm_grouped / _pairs / _pair_sum)
+constexpr int ROWS_PLAIN = 0;  // row m of A and of C
+constexpr int PAIRS_C = 1;     // A row m; C rows pair_rows[m][0] and, when >= 0, pair_rows[m][1]
+constexpr int PAIRS_A = 2;     // A row pair_rows[m][0] + A row pair_rows[m][1] (when >= 0); C row m
+template <int ROWS>
+using SmemFor = std::conditional_t<ROWS == PAIRS_A, SmemPairsA, Smem>;
 
 __device__ __forceinline__ const GemmDesc* find_desc(const GemmDesc* d, int nd, int q) {
   int i = 0;
@@ -115,18 +133,25 @@ __device__ __forceinline__ void bar_wg(int wg) { asm volatile("bar.sync %0, 128;
 
 // ACT = false: the plain GEMM.  ACT = true also honours the activation bits 3-5 of a problem's flags in the
 // epilogue, with the auxiliary matrix at aux_base (addressed with C's c_off and ldc); see nqb.h.
-// PAIRS = true (plain problems only): M = min(M, *m_dev) is read on the device, and result row m is stored to the C
-// rows pair_rows[m][0] and, when it is >= 0, pair_rows[m][1] (nqb_gemm_grouped_pairs).
-template <bool ACT, bool PAIRS = false>
+// ROWS = PAIRS_C / PAIRS_A (plain problems only): M = min(M, *m_dev) is read on the device, and
+//   PAIRS_C: result row m is stored to the C rows pair_rows[m][0] and, when it is >= 0, pair_rows[m][1]
+//            (nqb_gemm_grouped_pairs);
+//   PAIRS_A: row m of the product is (A[pair_rows[m][0]] + A[pair_rows[m][1]]) @ B, the second term only when
+//            pair_rows[m][1] >= 0, stored to C row m (nqb_gemm_grouped_pair_sum).  Both rows are staged with cp.async;
+//            the low-part pass forms the fp32 sum, writes it over the staged representative chunk (the hi operand)
+//            and writes its low part.
+template <bool ACT, int ROWS = ROWS_PLAIN>
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const int32_t* __restrict__ tile_ctas,
          int sched_ctas, const float* __restrict__ a_base, const float* __restrict__ b_base, float* __restrict__ c_base,
          const float* __restrict__ rs_base, int64_t rs_ld, int64_t M, float* __restrict__ aux_base,
          const int64_t* __restrict__ m_dev, const int64_t* __restrict__ pair_rows) {
+  constexpr bool SUMA = ROWS == PAIRS_A;
+  constexpr int NLON = SUMA ? RAW : NLO;  // low-part slots
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  Smem& S = *reinterpret_cast<Smem*>(smem_raw);
+  SmemFor<ROWS>& S = *reinterpret_cast<SmemFor<ROWS>*>(smem_raw);
   const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
-  if constexpr (PAIRS) M = min(M, *m_dev);  // the schedule does not depend on M, only the M-tiles and row guards
+  if constexpr (ROWS != ROWS_PLAIN) M = min(M, *m_dev);  // the schedule does not depend on M, only the M-tiles and row guards
   const int64_t mtiles = (M + TM - 1) / TM;
 
   if (tid == 0) {
@@ -155,18 +180,40 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
   };
   if (pvalid) open_q();
   uint32_t n_issued = 0;
-  auto issue = [&]() {  // cp.async the cursor's chunk into raw stage n_issued % RAW, advance, commit
+  // PAIRS_A: (representative, partner) A rows of this thread's two rows of the cursor's M-tile; -1 = none
+  [[maybe_unused]] int32_t prow[2][2];
+  // cp.async the cursor's chunk into raw stage n_issued % RAW (PAIRS_A: its partner rows into low-part stage
+  // n_issued % RAW, whose last reader, chunk n_issued - RAW, has retired), advance, commit
+  auto issue = [&]() {
     if (pvalid) {
       float* dst = S.araw[wg][n_issued % RAW] + my_off;
+      if constexpr (SUMA) {
+        if (ph_ == 0) {  // the first chunk of an M-tile: read its rows' slots once
+#pragma unroll
+          for (int g = 0; g < 2; ++g) {
+            const int64_t m = pmt * TM + wg * MW + warp * 16 + g * 8 + r8;
+            const longlong2 pr = m < M ? __ldg(reinterpret_cast<const longlong2*>(pair_rows) + m) : make_longlong2(-1, -1);
+            prow[g][0] = (int32_t)pr.x;
+            prow[g][1] = (int32_t)pr.y;
+          }
+        }
+      }
 #pragma unroll
       for (int g = 0; g < 2; ++g) {
         const int64_t m = pmt * TM + wg * MW + warp * 16 + g * 8 + r8;
 #pragma unroll
         for (int kh = 0; kh < 2; ++kh) {
           const int k = ph_ * KC + (kh * 4 + kq) * 4;
-          const bool in = m < M && k < pK;
-          const int64_t off = in ? m * plda + k : 0;
-          cp_async16(dst + g * (KC / 4 * 32) + kh * 128, pA + off, in ? 16u : 0u);
+          if constexpr (SUMA) {
+            const bool in = prow[g][0] >= 0 && k < pK, pin = in && prow[g][1] >= 0;
+            cp_async16(dst + g * (KC / 4 * 32) + kh * 128, pA + (in ? (int64_t)prow[g][0] * plda + k : 0), in ? 16u : 0u);
+            cp_async16(S.alo[wg][n_issued % RAW] + my_off + g * (KC / 4 * 32) + kh * 128,
+                       pA + (pin ? (int64_t)prow[g][1] * plda + k : 0), pin ? 16u : 0u);
+          } else {
+            const bool in = m < M && k < pK;
+            const int64_t off = in ? m * plda + k : 0;
+            cp_async16(dst + g * (KC / 4 * 32) + kh * 128, pA + off, in ? 16u : 0u);
+          }
         }
       }
       if (++ph_ == pnh) {
@@ -242,16 +289,21 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
       for (int seg = 0; seg < nseg; ++seg) {
         const int h1 = min(w.kchunks, (seg + 1) * SEG);
         for (int h = seg * SEG; h < h1; ++h, ++i) {
-          // chunk i - 1's MMAs (if any) run during everything up to this chunk's first wgmma; chunk i - 2, the
-          // last reader of low-part slot i % NLO, has retired
+          // chunk i - 1's MMAs (if any) run during everything up to this chunk's first wgmma; chunk i - NLON, the
+          // last reader of low-part slot i % NLON, has retired
           cp_async_wait<DEPTH - 1>();  // my parts of chunk i have landed
-          const float* raw = S.araw[wg][i % RAW] + my_off;
-          float* lo = S.alo[wg][i % NLO] + my_off;
+          float* raw = S.araw[wg][i % RAW] + my_off;
+          float* lo = S.alo[wg][i % NLON] + my_off;
 #pragma unroll
           for (int g = 0; g < 2; ++g)
 #pragma unroll
             for (int kh = 0; kh < 2; ++kh) {
-              const float4 t = *reinterpret_cast<const float4*>(raw + g * (KC / 4 * 32) + kh * 128);
+              float4 t = *reinterpret_cast<const float4*>(raw + g * (KC / 4 * 32) + kh * 128);
+              if constexpr (SUMA) {  // this thread's own cp.async pieces: the representative + the partner
+                const float4 p = *reinterpret_cast<const float4*>(lo + g * (KC / 4 * 32) + kh * 128);
+                t = make_float4(t.x + p.x, t.y + p.y, t.z + p.z, t.w + p.w);
+                *reinterpret_cast<float4*>(raw + g * (KC / 4 * 32) + kh * 128) = t;
+              }
               *reinterpret_cast<float4*>(lo + g * (KC / 4 * 32) + kh * 128) =
                   make_float4(tf32_lo(t.x), tf32_lo(t.y), tf32_lo(t.z), tf32_lo(t.w));
             }
@@ -266,7 +318,7 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
             mbar_wait(&S.b_full[slot], (bpar >> slot) & 1);
             bpar ^= 1u << slot;
           }
-          const uint64_t a_hi = dR0 + (uint64_t)((i % RAW) * A_STAGE), a_lo = dL0 + (uint64_t)((i % NLO) * A_STAGE);
+          const uint64_t a_hi = dR0 + (uint64_t)((i % RAW) * A_STAGE), a_lo = dL0 + (uint64_t)((i % NLON) * A_STAGE);
           const uint64_t b_hi = dB0 + (uint64_t)(slot * B_SLOT), b_lo = b_hi + B_LO;
           const uint32_t fresh = (h == seg * SEG);  // the first chunk of a segment overwrites the accumulators
           wgmma_fence();
@@ -295,7 +347,7 @@ k_gemm3x(const GemmDesc* __restrict__ descs, int ndesc, int ntiles_total, const 
       }
       // ---- epilogue: C rows r0 and r0 + 8 of this warpgroup, two adjacent columns per store --------------------
       const int64_t m0 = mt * TM + wg * MW + r0;
-      if constexpr (PAIRS) {
+      if constexpr (ROWS == PAIRS_C) {
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
           const int64_t m = m0 + half * 8;
@@ -420,7 +472,7 @@ extern "C" int nqb_gemm_prepare(const float* B, int64_t ldb, int K, int N, int t
 }
 
 // the launcher of the entry points; errors are reported under the entry point's name
-template <bool ACT, bool PAIRS = false>
+template <bool ACT, int ROWS = ROWS_PLAIN>
 static int gemm_grouped_launch(const char* who, const void* descs_dev, int ndesc, int ntiles_total,
                                const int32_t* tile_ctas_dev, int sched_ctas, const float* a_base,
                                const float* prepared_base, float* c_base, float* aux_base, const float* rowscale_base,
@@ -437,8 +489,9 @@ static int gemm_grouped_launch(const char* who, const void* descs_dev, int ndesc
   if (!descs_dev || !a_base || !prepared_base || !c_base) return fail("null pointer");
   // the device descriptors cannot be read here: an activation launch always takes an aux matrix
   if (ACT && !aux_base) return fail("aux_base is null (bit4 / bit5 problems store to or read from it)");
-  if (PAIRS && (!m_dev || !pair_rows)) return fail("pair_rows or count is null");
-  if (PAIRS && ((uintptr_t)pair_rows & 15)) return fail("pair_rows must be 16-byte aligned");
+  if (ROWS != ROWS_PLAIN && (!m_dev || !pair_rows)) return fail("pair_rows or count is null");
+  if (ROWS != ROWS_PLAIN && ((uintptr_t)pair_rows & 15)) return fail("pair_rows must be 16-byte aligned");
+  if (ROWS == PAIRS_A && M > INT32_MAX) return fail("capacity must be < 2^31 (A rows are held as int32)");
   // A is staged with 16-byte cp.async, the weights with bulk copies, C and aux are stored in float2 pairs
   if (((uintptr_t)a_base | (uintptr_t)prepared_base | (uintptr_t)c_base | (uintptr_t)aux_base) & 15)
     return fail(ACT ? "a_base, prepared_base, c_base and aux_base must be 16-byte aligned"
@@ -446,8 +499,8 @@ static int gemm_grouped_launch(const char* who, const void* descs_dev, int ndesc
   static bool attr_set[64] = {false};
   const int dev = gemm_device();
   if (!attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(k_gemm3x<ACT, PAIRS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)sizeof(Smem) + 1024);
+    cudaError_t e = cudaFuncSetAttribute(k_gemm3x<ACT, ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)sizeof(SmemFor<ROWS>) + 1024);
     if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
     attr_set[dev] = true;
   }
@@ -455,7 +508,7 @@ static int gemm_grouped_launch(const char* who, const void* descs_dev, int ndesc
   int grid = (int)(nwork < gemm_sm_count() ? nwork : gemm_sm_count());
   if (tile_ctas_dev != nullptr && sched_ctas > 0 && sched_ctas <= gemm_sm_count()) grid = sched_ctas;
   else tile_ctas_dev = nullptr;
-  k_gemm3x<ACT, PAIRS><<<grid, NTHREADS, sizeof(Smem) + 1024, (cudaStream_t)st>>>(
+  k_gemm3x<ACT, ROWS><<<grid, NTHREADS, sizeof(SmemFor<ROWS>) + 1024, (cudaStream_t)st>>>(
       (const GemmDesc*)descs_dev, ndesc, ntiles_total, tile_ctas_dev, sched_ctas, a_base, prepared_base, c_base,
       rowscale_base, rs_ld, M, aux_base, m_dev, pair_rows);
   nqb_count_launch();
@@ -483,7 +536,16 @@ extern "C" int nqb_gemm_grouped_pairs(const void* descs_dev, int ndesc, int ntil
                                       int sched_ctas, const float* a_base, const float* prepared_base, float* c_base,
                                       const int64_t* pair_rows, const int64_t* count_dev, int64_t capacity,
                                       nqb_stream_t st) {
-  return gemm_grouped_launch<false, true>("nqb_gemm_grouped_pairs", descs_dev, ndesc, ntiles_total, tile_ctas_dev,
+  return gemm_grouped_launch<false, PAIRS_C>("nqb_gemm_grouped_pairs", descs_dev, ndesc, ntiles_total, tile_ctas_dev,
                                           sched_ctas, a_base, prepared_base, c_base, nullptr, nullptr, 0, capacity,
                                           st, count_dev, pair_rows);
+}
+
+extern "C" int nqb_gemm_grouped_pair_sum(const void* descs_dev, int ndesc, int ntiles_total,
+                                         const int32_t* tile_ctas_dev, int sched_ctas, const float* a_base,
+                                         const float* prepared_base, float* c_base, const int64_t* pair_rows,
+                                         const int64_t* count_dev, int64_t capacity, nqb_stream_t st) {
+  return gemm_grouped_launch<false, PAIRS_A>("nqb_gemm_grouped_pair_sum", descs_dev, ndesc, ntiles_total,
+                                             tile_ctas_dev, sched_ctas, a_base, prepared_base, c_base, nullptr,
+                                             nullptr, 0, capacity, st, count_dev, pair_rows);
 }

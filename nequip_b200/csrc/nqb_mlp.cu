@@ -116,9 +116,16 @@ __global__ void __launch_bounds__(256) k_hidden_fwd(const float* __restrict__ em
   }
 }
 
+// ROWS = true: the backward on the slots of nqb_edge_pairs, u < min(E, *count): grad_h row u is the slot's summed
+// gradient, the pre-activation is recomputed from emb[rows[2 u]], and the slot writes its representative's grad_emb row
+// and exact zeros to its partner's row (the grid is sized for E)
+template <bool ROWS = false>
 __global__ void __launch_bounds__(256) k_hidden_bwd(const float* __restrict__ emb, const float* __restrict__ W1s,
-                                                    const float* __restrict__ gh, int64_t E, float* __restrict__ gemb) {
+                                                    const float* __restrict__ gh, int64_t E, float* __restrict__ gemb,
+                                                    const int64_t* __restrict__ rows = nullptr,
+                                                    const int64_t* __restrict__ count = nullptr) {
   const int lane = threadIdx.x & 31, m0 = lane * 4;
+  if constexpr (ROWS) E = min(E, *count);
   float2 w01[NB], w23[NB];
 #pragma unroll
   for (int k = 0; k < NB; ++k) {
@@ -129,10 +136,20 @@ __global__ void __launch_bounds__(256) k_hidden_bwd(const float* __restrict__ em
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   const int64_t nbatch = (E + 31) >> 5;
   int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  Basis8 cur = load_basis(emb, b * 32 + lane, b < nbatch ? E : 0);
+  // ROWS: lane j also keeps the (representative, partner) edges of the batch's slot j
+  [[maybe_unused]] longlong2 cur_pr, nxt_pr;
+  auto load = [&](int64_t u, int64_t n, longlong2& pr) {
+    if constexpr (ROWS) {
+      pr = u < n ? __ldg(reinterpret_cast<const longlong2*>(rows) + u) : make_longlong2(0, -1);
+      return load_basis(emb, pr.x, u < n ? pr.x + 1 : 0);
+    } else {
+      return load_basis(emb, u, n);
+    }
+  };
+  Basis8 cur = load(b * 32 + lane, b < nbatch ? E : 0, cur_pr);
   for (; b < nbatch; b += nwarps) {
     const int64_t bn = b + nwarps;
-    const Basis8 nxt = load_basis(emb, bn * 32 + lane, bn < nbatch ? E : 0);
+    const Basis8 nxt = load(bn * 32 + lane, bn < nbatch ? E : 0, nxt_pr);
     const int64_t e0 = b * 32;
     const int cnt = (int)((E - e0) < 32 ? (E - e0) : 32);  // warp-uniform
     const float* grow = gh + e0 * H + m0;
@@ -178,9 +195,19 @@ __global__ void __launch_bounds__(256) k_hidden_bwd(const float* __restrict__ em
       NQB_HALVE(1, 1)
 #undef NQB_HALVE
       // element `lane` = (edge j0 + lane / 8, component lane % 8): 128 contiguous bytes per warp
-      if (j0 + (lane >> 3) < cnt) gemb[(e0 + j0) * NB + lane] = v[0];
+      if constexpr (ROWS) {
+        const int src = (j0 + (lane >> 3)) & 31;
+        const int64_t rep = __shfl_sync(0xffffffffu, cur_pr.x, src), par = __shfl_sync(0xffffffffu, cur_pr.y, src);
+        if (j0 + (lane >> 3) < cnt) {
+          gemb[rep * NB + (lane & 7)] = v[0];
+          if (par >= 0) gemb[par * NB + (lane & 7)] = 0.f;
+        }
+      } else {
+        if (j0 + (lane >> 3) < cnt) gemb[(e0 + j0) * NB + lane] = v[0];
+      }
     }
     cur = nxt;
+    if constexpr (ROWS) cur_pr = nxt_pr;
   }
 }
 
@@ -329,7 +356,7 @@ extern "C" void nqb_count_launch(void);
 // its next batch is always prefetched; fewer CTAs when there are fewer batches than warps
 template <typename K>
 static unsigned hidden_grid(K kernel, int which, int64_t E) {
-  static int ctas_dev[3][64] = {{0}, {0}, {0}};
+  static int ctas_dev[4][64] = {{0}, {0}, {0}, {0}};
   int dev = 0;
   cudaGetDevice(&dev);
   dev &= 63;
@@ -378,7 +405,25 @@ extern "C" int nqb_mlp_hidden_bwd(const float* emb, const float* W1s, const floa
   if (E < 0) return nqb_set_error("nqb_mlp_hidden_bwd: negative size");
   if (E == 0) return 0;
   if (!emb || !W1s || !grad_h || !grad_emb) return nqb_set_error("nqb_mlp_hidden_bwd: null pointer");
-  k_hidden_bwd<<<hidden_grid(k_hidden_bwd, 1, E), 256, 0, (cudaStream_t)st>>>(emb, W1s, grad_h, E, grad_emb);
+  k_hidden_bwd<<<hidden_grid(k_hidden_bwd<false>, 1, E), 256, 0, (cudaStream_t)st>>>(emb, W1s, grad_h, E, grad_emb);
+  nqb_count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int nqb_mlp_hidden_bwd_rows(const float* emb, const float* W1s, const float* grad_h,
+                                       const int64_t* pair_rows, const int64_t* count, int64_t capacity,
+                                       int num_bessel, int hidden, float* grad_emb, nqb_stream_t st) {
+  if (num_bessel != NB || hidden != H)
+    return nqb_set_error("nqb_mlp_hidden_bwd_rows: only num_bessel=8, hidden=128 is built");
+  if (capacity < 0) return nqb_set_error("nqb_mlp_hidden_bwd_rows: negative size");
+  if (capacity == 0) return 0;
+  if (!emb || !W1s || !grad_h || !pair_rows || !count || !grad_emb)
+    return nqb_set_error("nqb_mlp_hidden_bwd_rows: null pointer");
+  if ((uintptr_t)pair_rows & 15) return nqb_set_error("nqb_mlp_hidden_bwd_rows: pair_rows must be 16-byte aligned");
+  k_hidden_bwd<true><<<hidden_grid(k_hidden_bwd<true>, 3, capacity), 256, 0, (cudaStream_t)st>>>(
+      emb, W1s, grad_h, capacity, grad_emb, pair_rows, count);
   nqb_count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return nqb_set_error(cudaGetErrorString(e));

@@ -147,11 +147,12 @@ class SelfConnectionGemm:
 # ---------------------------------------------------------------------------------------
 class _RadialMLPGemmFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, emb, mlp: "RadialMLPGemm", need_bwd: bool, pairs):
+    def forward(ctx, emb, mlp: "RadialMLPGemm", need_bwd: bool, pairs, pair_grad: bool):
         E = emb.shape[0]
         out = torch.empty((E, mlp.W), dtype=emb.dtype, device=emb.device)
         pre = [] if need_bwd else None
-        if pairs is not None and mlp.shares_pairs:
+        shared = pairs is not None and mlp.shares_pairs
+        if shared:
             # one row of h and of the GEMM per slot of the pair map, stored to both edges of the slot
             h = torch.empty((E, mlp.w1s.shape[1]), dtype=emb.dtype, device=emb.device)  # rows < count are used
             ops.mlp_hidden_fwd_rows(emb, mlp.w1s, pairs, h)
@@ -159,6 +160,7 @@ class _RadialMLPGemmFn(torch.autograd.Function):
         else:
             mlp.fwd.run(mlp.hidden(emb, pre), out, E)
         ctx.mlp = mlp
+        ctx.pairs = pairs if shared and pair_grad else None
         if need_bwd:
             ctx.save_for_backward(emb, *pre)
         return out
@@ -167,7 +169,7 @@ class _RadialMLPGemmFn(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, gw):
         emb, *pre = ctx.saved_tensors
-        return ctx.mlp.grad_emb(emb, gw, pre), None, None, None
+        return ctx.mlp.grad_emb(emb, gw, pre, ctx.pairs), None, None, None, None
 
 
 class RadialMLPGemm:
@@ -179,7 +181,8 @@ class RadialMLPGemm:
     With a backward pass ahead, each hidden layer on ``k_gemm3x`` also stores its pre-activation ([E, H] float32).
     Given the reverse-edge pair map (``ops.edge_pairs``), an [8, 128] -> [128, W] MLP computes one row per slot
     (``k_hidden_fwd`` on the slots' representative edges, then the paired ``k_gemm3x`` that stores each result row to
-    both edges of its slot); deeper MLPs keep the per-edge forward.
+    both edges of its slot), and by default its backward on the slots too (``grad_emb`` with ``pairs``); deeper MLPs
+    keep the per-edge forward and backward.
     Backward: the transposed GEMM of each layer multiplies by silu' of the saved pre-activation of the layer below;
     into an [8, 128] first layer it gives grad_h for ``k_hidden_bwd`` (pre-activation recomputed), and a generic
     first layer ends with a plain transposed GEMM into grad_emb [E, num_bessels]."""
@@ -264,11 +267,27 @@ class RadialMLPGemm:
             x = h
         return x
 
-    def grad_emb(self, emb, gw, pre=()):
+    def grad_emb(self, emb, gw, pre=(), pairs: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
         """Gradient of ``emb`` from the gradient ``gw`` of the edge weights, with ``pre`` the pre-activations that
-        ``hidden`` saved."""
+        ``hidden`` saved.
+
+        ``pairs`` (MLPs with ``shares_pairs`` only): the backward of the pair-shared forward.  Both edges of a slot got
+        the slot's output, so the slot's grad_h is ``(gw[rep] + gw[partner]) @ (W a)^T`` (the sum is formed inside the
+        GEMM), ``k_hidden_bwd`` writes the representative's ``grad_emb`` row from it and zeros to the partner's row.
+        The two edges have bitwise-equal embedding rows, so in exact arithmetic this moves the partner's embedding
+        gradient onto the representative; it leaves forces and ``sym(sum_e r_e (x) dE/dr_e)`` unchanged where the
+        embedding's derivative is the same for both edges (a function of |r| with one cutoff for the pair), not the
+        per-edge ``dE/d(edge vector)``."""
         E = emb.shape[0]
         g = gw.contiguous()
+        if pairs is not None:
+            if not self.shares_pairs:
+                raise ValueError("RadialMLPGemm.grad_emb: pairs given, but this MLP does not share rows between pairs")
+            gh = torch.empty((E, self.w1s.shape[1]), dtype=g.dtype, device=g.device)  # rows < count are used
+            self.bwd.run_pair_sum(g, gh, pairs)
+            gemb = torch.empty_like(emb)
+            ops.mlp_hidden_bwd_rows(emb, self.w1s, gh, pairs, gemb)
+            return gemb
         for gemm, width, k in self._chain:
             out = torch.empty((E, width), dtype=g.dtype, device=g.device)
             gemm.run(g, out, E, aux=None if k is None else pre[k])
@@ -279,9 +298,13 @@ class RadialMLPGemm:
             return gemb
         return g
 
-    def __call__(self, emb, pairs: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
-        """``pairs``: ``ops.edge_pairs`` of the edge list whose embedding ``emb`` is (the per-edge forward without)."""
-        return _RadialMLPGemmFn.apply(emb.contiguous(), self, torch.is_grad_enabled() and emb.requires_grad, pairs)
+    def __call__(self, emb, pairs: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, pair_grad: bool = True):
+        """``pairs``: ``ops.edge_pairs`` of the edge list whose embedding ``emb`` is (the per-edge forward without).
+        ``pair_grad``: with a pair-shared forward, also run the backward on the slots (``grad_emb``); False keeps the
+        per-edge backward, for callers that need each edge's own ``dE/d(emb)`` (per-edge outputs such as ML-IAP edge
+        forces, or an embedding whose derivative differs between the two edges of a pair)."""
+        return _RadialMLPGemmFn.apply(emb.contiguous(), self, torch.is_grad_enabled() and emb.requires_grad, pairs,
+                                      pair_grad)
 
 
 # ---------------------------------------------------------------------------------------

@@ -397,12 +397,13 @@ class InteractionBlock(torch.nn.Module):
                           f"wgmma kernels: {reason}", RuntimeWarning, stacklevel=3)
 
     def forward(self, x, node_attrs, edge_attrs, edge_embedding, edge_index, types=None, type_table=None,
-                n_own: Optional[int] = None, halo=None, pairs=None):
+                n_own: Optional[int] = None, halo=None, pairs=None, pair_grad: bool = True):
         """``n_own``/``halo``: sharded frames (owned atoms first, then ghosts).  As in the reference
         (interaction_block.py:159-199) the first layer sees the type embedding of owned + ghost atoms;
         later layers work on owned rows, refresh the ghosts through ``halo`` right before the
         TP+scatter and truncate to the owned rows right after it.  ``pairs``: the reverse-edge pair map of the
-        edge list (``ops.edge_pairs``), with which the radial MLP computes one row per pair."""
+        edge list (``ops.edge_pairs``), with which the radial MLP computes one row per pair, and with ``pair_grad``
+        also its backward (``RadialMLPGemm``)."""
         if n_own is not None and not self.is_first_layer:
             x = x[:n_own]
             node_attrs = node_attrs[:n_own]
@@ -427,7 +428,7 @@ class InteractionBlock(torch.nn.Module):
                         x = tc["sc"](x_in, types, x)
                     return x
             if tc["mlp"] is not None:
-                w = tc["mlp"](edge_embedding, pairs)
+                w = tc["mlp"](edge_embedding, pairs, pair_grad)
             else:
                 self._note_fallback("radial MLP shape not supported by the grouped GEMM (needs at least one hidden "
                                     "layer, num_bessels and widths multiples of 4)")
@@ -513,8 +514,9 @@ class ConvNetLayer(torch.nn.Module):
         self.irreps_out = layer_out
 
     def forward(self, x, node_attrs, edge_attrs, edge_embedding, edge_index, types=None, type_table=None,
-                n_own=None, halo=None, pairs=None):
-        x = self.conv(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, type_table, n_own, halo, pairs)
+                n_own=None, halo=None, pairs=None, pair_grad=True):
+        x = self.conv(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, type_table, n_own, halo, pairs,
+                      pair_grad)
         return self.equivariant_nonlin(x)
 
 
@@ -664,6 +666,9 @@ class NequIPEnergyModel(torch.nn.Module):
             self.pair_potential = ZBL(type_names, model_dtype=model_dtype, **pair_spec)
             self.config["pair_potential"] = dict(_target_=ZBL_TARGET, **pair_spec)
         self.per_edge_type_cutoff: Optional[torch.Tensor] = cutoff_table
+        # the radial MLP's backward on the pair slots needs both edges of a pair to have the same embedding
+        # derivative: an asymmetric table gives i -> j and j -> i different cutoffs, so it keeps the per-edge backward
+        self._pair_grad = cutoff_table is None or bool(torch.equal(cutoff_table, cutoff_table.t()))
         if cutoff_table is not None:
             self.register_buffer("rmax_recip", cutoff_table.reciprocal().reshape(-1))
             self.config["per_edge_type_cutoff"] = {k: (dict(v) if isinstance(v, dict) else v)
@@ -753,8 +758,12 @@ class NequIPEnergyModel(torch.nn.Module):
                 poly_p=self.poly_p, prefactor=pre, out_dtype=self.model_dtype, edge_grad_sink=sink,
                 **self._edge_type_kwargs(types), **self._frame_kwargs(data, cell))
         pairs = self._edge_pairs(edge_index, None if EDGE_VECTORS_KEY in data else shift, edge_embedding, types.numel())
+        # ML-IAP edge forces are dE/d(edge vector) per edge: moving a partner's gradient onto its representative
+        # would change them, so that input keeps the per-edge radial-MLP backward
+        pair_grad = self._pair_grad and EDGE_VECTORS_KEY not in data
         for layer in self.layers:
-            x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight, pairs=pairs)
+            x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight, pairs=pairs,
+                      pair_grad=pair_grad)
         e_atom = self.readout(x).to(torch.float64)
         if self.scales.numel():
             e_atom = e_atom * self.scales[types]
@@ -790,7 +799,7 @@ class NequIPEnergyModel(torch.nn.Module):
         pairs = self._edge_pairs(edge_index, shift, edge_embedding, types.numel())
         for layer in self.layers:
             x = layer(x, node_attrs, edge_attrs, edge_embedding, edge_index, types, self.type_embed.weight, n_own, halo,
-                      pairs)
+                      pairs, self._pair_grad)
         e_atom = self.readout(x).to(torch.float64)
         t_own = types[:n_own]
         if self.scales.numel():

@@ -955,22 +955,38 @@ class GroupedGemm:
         )
         return c
 
-    def run_pairs(self, a: torch.Tensor, c: torch.Tensor, pairs: Tuple[torch.Tensor, torch.Tensor]):
-        """C on the slots of ``edge_pairs``: ``a`` holds one row per slot (rows < U are read) and result row u is
-        stored to the C rows ``pair_rows[u]`` (the second when >= 0).  Plain problems only."""
+    def _check_pairs(self, a, c, pairs, who):
         pair_rows, count = pairs
         _require_cuda(a, c, pair_rows, count)
         if a.dtype != torch.float32 or c.dtype != torch.float32:
-            raise TypeError("GroupedGemm.run_pairs: float32 only")
+            raise TypeError(f"GroupedGemm.{who}: float32 only")
         if any(p.act != "none" or p.accumulate or p.atomic or p.skip_zero_rows or p.rs_off >= 0 for p in self.problems):
-            raise ValueError("GroupedGemm.run_pairs: plain problems only (no row scale, accumulate, atomic or activation)")
+            raise ValueError(f"GroupedGemm.{who}: plain problems only (no row scale, accumulate, atomic or activation)")
         if pair_rows.dtype != torch.int64 or count.dtype != torch.int64 or pair_rows.dim() != 2 or pair_rows.shape[1] != 2:
-            raise ValueError("GroupedGemm.run_pairs: pair_rows must be [E, 2] and count [1], int64")
+            raise ValueError(f"GroupedGemm.{who}: pair_rows must be [E, 2] and count [1], int64")
+        return pair_rows, count
+
+    def run_pairs(self, a: torch.Tensor, c: torch.Tensor, pairs: Tuple[torch.Tensor, torch.Tensor]):
+        """C on the slots of ``edge_pairs``: ``a`` holds one row per slot (rows < U are read) and result row u is
+        stored to the C rows ``pair_rows[u]`` (the second when >= 0).  Plain problems only."""
+        pair_rows, count = self._check_pairs(a, c, pairs, "run_pairs")
         _capi.check(
             _capi.lib().nqb_gemm_grouped_pairs(_ptr(self.descs), self.ndesc, self.ntiles_total, _ptr(self.tile_ctas),
                                                int(self.sched_ctas), _ptr(a), _ptr(self.prepared), _ptr(c),
                                                _ptr(pair_rows), _ptr(count), int(pair_rows.shape[0]), _stream()),
             "nqb_gemm_grouped_pairs",
+        )
+        return c
+
+    def run_pair_sum(self, a: torch.Tensor, c: torch.Tensor, pairs: Tuple[torch.Tensor, torch.Tensor]):
+        """The transpose of ``run_pairs``: result row u < U is ``(a[pair_rows[u, 0]] + a[pair_rows[u, 1]]) @ B`` (the
+        second row only when >= 0), stored to row u of ``c`` (rows >= U untouched).  Plain problems only."""
+        pair_rows, count = self._check_pairs(a, c, pairs, "run_pair_sum")
+        _capi.check(
+            _capi.lib().nqb_gemm_grouped_pair_sum(_ptr(self.descs), self.ndesc, self.ntiles_total, _ptr(self.tile_ctas),
+                                                  int(self.sched_ctas), _ptr(a), _ptr(self.prepared), _ptr(c),
+                                                  _ptr(pair_rows), _ptr(count), int(pair_rows.shape[0]), _stream()),
+            "nqb_gemm_grouped_pair_sum",
         )
         return c
 
@@ -1035,6 +1051,19 @@ def mlp_hidden_bwd(emb: torch.Tensor, w1s: torch.Tensor, gh: torch.Tensor, gemb:
     _require_cuda(emb, w1s, gh, gemb)
     _capi.check(_capi.lib().nqb_mlp_hidden_bwd(_ptr(emb), _ptr(w1s), _ptr(gh), emb.shape[0], emb.shape[1], w1s.shape[1],
                                                _ptr(gemb), _stream()), "nqb_mlp_hidden_bwd")
+
+
+def mlp_hidden_bwd_rows(emb: torch.Tensor, w1s: torch.Tensor, gh: torch.Tensor, pairs: Tuple[torch.Tensor, torch.Tensor],
+                        gemb: torch.Tensor) -> None:
+    """The backward of ``mlp_hidden_fwd_rows``: for the slots u < count of ``edge_pairs``,
+    ``gemb[pair_rows[u, 0]] = (gh[u] * silu'(emb[pair_rows[u, 0]] @ w1s)) @ w1s^T`` and ``gemb[pair_rows[u, 1]] = 0``
+    (when >= 0)."""
+    pair_rows, count = pairs
+    _require_cuda(emb, w1s, gh, pair_rows, count, gemb)
+    _capi.check(_capi.lib().nqb_mlp_hidden_bwd_rows(_ptr(emb), _ptr(w1s), _ptr(gh), _ptr(pair_rows), _ptr(count),
+                                                    pair_rows.shape[0], emb.shape[1], w1s.shape[1], _ptr(gemb),
+                                                    _stream()),
+                "nqb_mlp_hidden_bwd_rows")
 
 
 # ---------------------------------------------------------------------------------------
